@@ -124,7 +124,7 @@ int rgbl_depth_from_pcd(rgbl_ctx* ctx, const float* pts4xn, int n_pts, const flo
                         float* depth, float* uright, float* raw_map, float* processed_map);
 
 /* ---- Frame::ComputeStereoFromRGBD (src/Frame.cc:1074-1095), the depth association of System::TrackRGBD ---- *
- * depth_map: H x W float32 (row stride in floats), metric depth (the caller applied DepthMapFactor, src/Tracking.cc:1565-1569).
+ * depth_map: H x W float32 (row stride in floats), metric depth (the caller applied DepthMapFactor, src/Tracking.cc:1538-1539).
  * d = depth_map[(int)kp.y][(int)kp.x] at the DISTORTED keypoint; depth[i] = d, uright[i] = kps_un[i].x - bf / d where d > 0, else -1. */
 int rgbl_depth_from_map(rgbl_ctx* ctx, const float* depth_map, int width, int height, int stride_floats, float bf, const rgbl_keypoint* kps,
                         const rgbl_keypoint* kps_un, int n_kp, float* depth, float* uright);
@@ -307,7 +307,7 @@ int rgbl_resident_compute_bow(rgbl_ctx* ctx, const rgbl_vocabulary* voc, int fra
                               int* n_words, int32_t* fv_node, int32_t* fv_start, int32_t* fv_feature, int* n_fv_nodes);
 
 /* Resident tracking chain over the frames of the last batched call, entirely on the device: for t = 1..n-1
- * SearchByProjection(frame t, frame t-1, th) -> PoseOptimization, every LiDAR-depth keypoint of frame t-1 acting as a map
+ * SearchByProjection(frame t, frame t-1, th) -> PoseOptimization, every keypoint of frame t-1 with depth acting as a map
  * point (Frame::UnprojectStereo, src/Frame.cc:1137-1150, with the estimated pose of t-1).  Frame t is searched and its optimisation
  * started at the constant-velocity prediction mVelocity * Tcw(t-1), mVelocity = Tcw(t-1) * Tcw(t-2)^-1 (src/Tracking.cc:2904,
  * 2243-2245; Sophus SE3f products); frame 1 of a sequence has no velocity yet and starts at the pose of frame 0.
@@ -326,12 +326,13 @@ int rgbl_resident_track(rgbl_ctx* ctx, const float pose0[7], float fx, float fy,
 int rgbl_resident_track_begin(rgbl_ctx* ctx, const float pose0[7], float fx, float fy, float cx, float cy, float bf, float th, int mono);
 int rgbl_resident_track_end(rgbl_ctx* ctx, float* poses_out, int* n_matches, int* n_inliers);
 
-/* The full per-frame tracking path of the reference for an RGB-L frame, and batches that continue one sequence:
+/* The full per-frame tracking path of the reference for an RGB-L or RGB-D frame (the chain reads keypoints, descriptors, mvDepth and
+ * mvuRight only), and batches that continue one sequence:
  *   TrackWithMotionModel (src/Tracking.cc:2888-2981): pose predicted by the constant-velocity model (:2904), SearchByProjection(frame t,
  *     frame t-1, th_last) -> PoseOptimization -> outliers discarded;
  *   TrackLocalMap (src/Tracking.cc:2983-3050 with SearchLocalPoints :3377-3460), when local_map_frames = K > 0: Frame::isInFrustum over
  *     the local map, SearchByProjection(frame t, local points, th_local, nn_ratio_local) -> PoseOptimization on all map points.  The
- *     local map of this harness = the LiDAR-depth keypoints of the K frames before t-1, unprojected with their final poses, with
+ *     local map of this harness = the keypoints with depth of the K frames before t-1, unprojected with their final poses, with
  *     MapPoint::UpdateNormalAndDepth's normal / scale-invariance distances for one observation (src/MapPoint.cc:437-490); it lives on
  *     the device as a ring (slot = frame counter mod K) and its points are searched in ring order.
  * continue_sequence != 0: frame 0 of this batch is tracked against the LAST frame of the previous chain of this context (keypoints,
@@ -376,6 +377,39 @@ typedef struct rgbl_sequence_io {
 int rgbl_resident_stage(rgbl_ctx* ctx, int slot, int n_frames, const uint8_t* const* gray, int width, int height, int stride,
                         const float* const* pts4xn, const int* n_pts);
 int rgbl_track_sequence(rgbl_ctx* ctx, const float P[12], const rgbl_depth_params* prm, const rgbl_chain_params* chain, const rgbl_sequence_io* io);
+
+/* ---- RGB-D: System::TrackRGBD (src/System.cc:339) -> Tracking::GrabImageRGBD (src/Tracking.cc:1518) -> RGB-D Frame constructor
+ * (src/Frame.cc:200, ExtractORB + ComputeStereoFromRGBD :237 -> :1074-1095), batched and resident like the RGB-L entry points above.
+ * The depth images stay uint16 in HBM (one plane per frame slot, allocated by the first RGB-D call; max_points may be 0) and are
+ * scaled where ComputeStereoFromRGBD reads them: d = (float)sample * depth_scale, the per-pixel rule of GrabImageRGBD's
+ * imDepth.convertTo(CV_32F, mDepthMapFactor) (:1538-1539), so the bits equal convert-then-gather.  d is read at the truncated
+ * keypoint; mvDepth = d, mvuRight = kpUn.x - bf / d where d > 0, else -1 (mvKeysUn == mvKeys: k1 == 0, as for RGB-L).
+ * After rgbl_resident_process_rgbd, rgbl_resident_download, rgbl_resident_compute_bow and rgbl_resident_track_begin2 / _end2 work
+ * unchanged (chain parameters for RGB-D: th_last 15, th_local 3).
+ * depth[f]: H x W uint16 (CV_16U as imread returns it), row stride depth_stride elements.                                          */
+int rgbl_resident_upload_rgbd(rgbl_ctx* ctx, int n_frames, const uint8_t* const* gray, int width, int height, int stride,
+                              const uint16_t* const* depth, int depth_stride);
+/* Same with the files' bytes: the images as for rgbl_resident_upload_kitti_png, the depth images as 16-bit single-channel PNG
+ * (cv::imread(depth_file, IMREAD_UNCHANGED), Examples/RGB-D/rgbd_kitti.cc; KITTI depth PNGs store metres x 256, TUM x 5000).
+ * The depth stream must be 16-bit gray, non-interlaced, of the context's size; anything else (8-bit, 16-bit RGB, interlaced) is
+ * RGBL_E_UNSUPPORTED.                                                                                                               */
+int rgbl_resident_upload_rgbd_png(rgbl_ctx* ctx, int n_frames, const uint8_t* const* png, const size_t* png_bytes, int camera_rgb,
+                                  const uint8_t* const* depth_png, const size_t* depth_png_bytes);
+/* The depth decode alone: depth_out[f] = what imread(IMREAD_UNCHANGED) returns for depth PNG stream f (H x W uint16, row stride
+ * `stride` elements).  Uses the depth planes of frame slots 0..n_frames-1.                                                          */
+int rgbl_decode_png_depth16(rgbl_ctx* ctx, int n_frames, const uint8_t* const* png, const size_t* png_bytes, uint16_t* const* depth_out, int stride);
+/* Frame construction of the uploaded RGB-D frames.  depth_scale = Tracking::mDepthMapFactor (already 1.0f / RGBD.DepthMapFactor,
+ * src/Tracking.cc:1188-1204), bf = Camera.bf (> 0).  RGBL_E_INVALID when the uploaded frames are not RGB-D frames.               */
+int rgbl_resident_process_rgbd(rgbl_ctx* ctx, float depth_scale, float bf, int* n_out /* nullable */);
+/* Upload one batch of RGB-D frames into staged slot `slot` for the resident mode of rgbl_track_sequence_rgbd. */
+int rgbl_resident_stage_rgbd(rgbl_ctx* ctx, int slot, int n_frames, const uint8_t* const* gray, int width, int height, int stride,
+                             const uint16_t* const* depth, int depth_stride);
+/* The sequence runner for RGB-D (the loop of Examples/RGB-D/rgbd_kitti.cc: load image + depth -> SLAM.TrackRGBD -> pose), as
+ * rgbl_track_sequence: io->pts4xn / io->n_pts must be NULL; host mode (io->gray != NULL) takes depth[] (one per frame of the call),
+ * resident mode takes slots staged with rgbl_resident_stage_rgbd (a slot staged with rgbl_resident_stage is RGBL_E_INVALID, and so is
+ * an RGB-D slot given to rgbl_track_sequence).                                                                                       */
+int rgbl_track_sequence_rgbd(rgbl_ctx* ctx, float depth_scale, float bf, const rgbl_chain_params* chain, const rgbl_sequence_io* io,
+                             const uint16_t* const* depth, int depth_stride);
 
 /* Keypoint distribution (DistributeOctTree) runs on the device by default (one CTA per (frame, level)); on != 0
  * selects the host implementation instead (also: environment RGBL_HOST_QUADTREE=1).  Both are exact.           */

@@ -106,6 +106,12 @@ SYMBOLS = {
     "rgbl_depth_from_map": (_i, [_vp, _vp, _i, _i, _i, _f, _vp, _vp, _i, _vp, _vp]),
     "rgbl_resident_stage": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _vp, _vp]),
     "rgbl_track_sequence": (_i, [_vp, _vp, _vp, _vp, _vp]),
+    "rgbl_resident_upload_rgbd": (_i, [_vp, _i, _vp, _i, _i, _i, _vp, _i]),
+    "rgbl_resident_upload_rgbd_png": (_i, [_vp, _i, _vp, _vp, _i, _vp, _vp]),
+    "rgbl_decode_png_depth16": (_i, [_vp, _i, _vp, _vp, _vp, _i]),
+    "rgbl_resident_process_rgbd": (_i, [_vp, _f, _f, _vp]),
+    "rgbl_resident_stage_rgbd": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _vp, _i]),
+    "rgbl_track_sequence_rgbd": (_i, [_vp, _f, _f, _vp, _vp, _vp, _i]),
     "rgbl_resident_track_end2": (_i, [_vp, _vp, _vp, _vp, _vp, _vp]),
     "rgbl_set_host_quadtree": (_i, [_vp, _i]),
     "rgbl_timer_mark": (_i, [_vp, _i]),

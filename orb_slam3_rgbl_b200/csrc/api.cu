@@ -42,6 +42,7 @@ static void release(Ctx* c) {
     if (c->ev_pyr) cudaEventDestroy(c->ev_pyr);
     if (c->ev_blur) cudaEventDestroy(c->ev_blur);
     if (c->d_pts_raw) cudaFree(c->d_pts_raw);
+    if (c->d_depth16) cudaFree(c->d_depth16);
     if (c->d_png_raw) cudaFree(c->d_png_raw);
     if (c->d_png_band) cudaFree(c->d_png_band);
     if (c->d_png_status) cudaFree(c->d_png_status);
@@ -57,7 +58,7 @@ static void release(Ctx* c) {
         if (c->ev_chain_e[i]) cudaEventDestroy(c->ev_chain_e[i]);
         if (c->ev_chain_done[i]) cudaEventDestroy(c->ev_chain_done[i]);
     }
-    for (Ctx::StageSlot& sl : c->stage) { if (sl.img) cudaFree(sl.img); if (sl.pts) cudaFree(sl.pts); if (sl.n_pts) cudaFree(sl.n_pts); }
+    for (Ctx::StageSlot& sl : c->stage) { if (sl.img) cudaFree(sl.img); if (sl.pts) cudaFree(sl.pts); if (sl.n_pts) cudaFree(sl.n_pts); if (sl.depth) cudaFree(sl.depth); }
     if (c->h_chain_f) cudaFreeHost(c->h_chain_f);
     if (c->h_chain_i) cudaFreeHost(c->h_chain_i);
     if (c->st) cudaStreamDestroy(c->st);
@@ -647,7 +648,7 @@ int rgbl_depth_from_pcd(rgbl_ctx* ctx, const float* pts4xn, int n_pts, const flo
 
 /* Frame::ComputeStereoFromRGBD (src/Frame.cc:1074-1095), the depth association of System::TrackRGBD: d = imDepth(kp.y, kp.x) at the
  * DISTORTED keypoint (C-style truncation of the float coordinates), mvDepth = d and mvuRight = kpUn.x - mbf / d where d > 0, else -1.
- * The gather runs on the device: the depth image (H x W float32, already scaled by DepthMapFactor, src/Tracking.cc:1568) is uploaded
+ * The gather runs on the device: the depth image (H x W float32, already scaled by DepthMapFactor, src/Tracking.cc:1538-1539) is uploaded
  * into the context's processed-depth plane and read by the same kernel that serves DepthModule::GetFeatureDepthFromDepthMap.        */
 int rgbl_depth_from_map(rgbl_ctx* ctx, const float* depth_map, int width, int height, int stride_floats, float bf, const rgbl_keypoint* kps,
                         const rgbl_keypoint* kps_un, int n_kp, float* depth, float* uright) {
@@ -712,13 +713,14 @@ static int upload_rgbl(Ctx* c, int n_frames, const uint8_t* const* gray, int str
     if (gray) { int rc = upload_images(c, n_frames, gray, stride, c->st); if (rc) return rc; }      // else: level 0 was written by decode_png_to_level0
     c->resident_frames = n_frames;
     c->resident_max_pts = max_pts;
+    c->resident_rgbd = false;
     *max_pts_out = max_pts;
     return RGBL_OK;
 }
 
 // cv::imread(PNG, IMREAD_UNCHANGED) + cvtColor to gray (Examples/RGB-L/rgbl_kitti.cc:87, src/Tracking.cc:1567-1580) into level 0 of the
 // frame slots 0..n_frames-1: host inflate into pinned staging, H2D of the filtered scanlines, reconstruction + gray on the device.
-static int decode_png_to_level0(Ctx* c, int n_frames, const uint8_t* const* png, const size_t* png_bytes, int camera_rgb, cudaStream_t st) {
+static int ensure_png_staging(Ctx* c) {
     const int w = c->cfg.width, h = c->cfg.height;
     if (!c->d_png_raw) {
         c->png_raw_stride = (((size_t)w * 4 + 1) * h + 255) & ~(size_t)255;
@@ -730,21 +732,74 @@ static int decode_png_to_level0(Ctx* c, int n_frames, const uint8_t* const* png,
         }
         CU(cudaMemset(c->d_png_status, 0, sizeof(int)));
     }
+    return RGBL_OK;
+}
+
+// host inflate of n PNG streams into the pinned staging buffer + H2D of the filtered scanlines -> bytes per pixel (or < 0)
+static int inflate_png_batch(Ctx* c, int n_frames, const uint8_t* const* png, const size_t* png_bytes, bool depth16, cudaStream_t st) {
+    const int w = c->cfg.width, h = c->cfg.height;
+    int rc = ensure_png_staging(c); if (rc) return rc;
     for (int f = 0; f < n_frames; ++f) if (!png[f] || !png_bytes[f]) { c->err = "empty image"; return RGBL_E_EMPTY; }
     int ch = 0;
     std::string perr;
-    const int prc = png_inflate_batch(n_frames, png, png_bytes, w, h, c->h_png_raw, c->png_raw_stride, &ch, perr);
+    const int prc = png_inflate_batch(n_frames, png, png_bytes, w, h, c->h_png_raw, c->png_raw_stride, &ch, perr, depth16);
     if (prc) { c->err = perr; return prc == -2 ? RGBL_E_UNSUPPORTED : RGBL_E_INVALID; }
     const size_t used = ((size_t)w * ch + 1) * h;
     for (int f = 0; f < n_frames; ++f)
         CU(cudaMemcpyAsync(c->d_png_raw + (size_t)f * c->png_raw_stride, c->h_png_raw + (size_t)f * c->png_raw_stride, used, cudaMemcpyHostToDevice, st));
-    launch_png_unfilter_gray(st, c->d_png_raw, c->png_raw_stride, w, h, ch, camera_rgb, c->d_pyr, c->frame_bytes, c->levels[0], c->d_png_band, c->d_png_status, n_frames);
+    return ch;
+}
+
+// after the reconstruction kernel: wait for it and report a bad scanline filter byte
+static int png_status(Ctx* c, cudaStream_t st) {
     CU(cudaMemcpyAsync(c->h_png_status, c->d_png_status, sizeof(int), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));          // the staging buffer is free again, and a bad scanline filter byte is an error of THIS call
     if (*c->h_png_status) {
         CU(cudaMemsetAsync(c->d_png_status, 0, sizeof(int), st));
         c->err = "corrupt PNG: scanline filter type above 4"; return RGBL_E_INVALID;
     }
+    return RGBL_OK;
+}
+
+static int decode_png_to_level0(Ctx* c, int n_frames, const uint8_t* const* png, const size_t* png_bytes, int camera_rgb, cudaStream_t st) {
+    const int ch = inflate_png_batch(c, n_frames, png, png_bytes, false, st);
+    if (ch < 0) return ch;
+    launch_png_unfilter_gray(st, c->d_png_raw, c->png_raw_stride, c->cfg.width, c->cfg.height, ch, camera_rgb, c->d_pyr, c->frame_bytes, c->levels[0],
+                             c->d_png_band, c->d_png_status, n_frames);
+    return png_status(c, st);
+}
+
+static size_t depth16_frame_elems(const Ctx* c) { return c->depth16_pitch * c->cfg.height; }
+
+static int ensure_depth16(Ctx* c) {
+    if (c->d_depth16) return RGBL_OK;
+    const size_t pitch = ((size_t)c->cfg.width * sizeof(uint16_t) + 63) / 64 * 32;
+    if (cudaMalloc((void**)&c->d_depth16, pitch * c->cfg.height * c->cfg.max_batch * sizeof(uint16_t)) != cudaSuccess) {
+        cudaGetLastError(); c->d_depth16 = nullptr; c->err = "cudaMalloc failed (RGB-D depth planes)"; return RGBL_E_CUDA;
+    }
+    c->depth16_pitch = pitch;
+    return RGBL_OK;
+}
+
+// cv::imread(depth PNG, IMREAD_UNCHANGED) of Examples/RGB-D/rgbd_kitti.cc into the uint16 depth planes of frame slots 0..n_frames-1
+// (16-bit gray only); shares the staging buffer with the image decode, one after the other.
+static int decode_png_to_depth16(Ctx* c, int n_frames, const uint8_t* const* png, const size_t* png_bytes, cudaStream_t st) {
+    int rc = ensure_depth16(c); if (rc) return rc;
+    const int ch = inflate_png_batch(c, n_frames, png, png_bytes, true, st);
+    if (ch < 0) return ch;
+    launch_png_unfilter_depth16(st, c->d_png_raw, c->png_raw_stride, c->cfg.width, c->cfg.height, c->d_depth16, depth16_frame_elems(c), c->depth16_pitch,
+                                c->d_png_band, c->d_png_status, n_frames);
+    return png_status(c, st);
+}
+
+// H2D of n_frames host depth images (CV_16U, row stride depth_stride elements) into the depth planes, on stream st
+static int upload_depth16(Ctx* c, int n_frames, const uint16_t* const* depth, int depth_stride, cudaStream_t st) {
+    if (!depth || depth_stride < c->cfg.width) { c->err = !depth ? "null argument" : "depth_stride < width"; return RGBL_E_INVALID; }
+    for (int f = 0; f < n_frames; ++f) if (!depth[f]) { c->err = "empty depth image"; return RGBL_E_EMPTY; }
+    int rc = ensure_depth16(c); if (rc) return rc;
+    for (int f = 0; f < n_frames; ++f)
+        CU(cudaMemcpy2DAsync(c->d_depth16 + (size_t)f * depth16_frame_elems(c), c->depth16_pitch * sizeof(uint16_t), depth[f], (size_t)depth_stride * sizeof(uint16_t),
+                             (size_t)c->cfg.width * sizeof(uint16_t), c->cfg.height, cudaMemcpyHostToDevice, st));
     return RGBL_OK;
 }
 
@@ -758,6 +813,24 @@ static int process_rgbl(Ctx* c, int n_frames, int max_pts, const float P[12], co
     run_depth_keypoints(c, dd, c->d_kps, c->d_kps, c->d_n_sel, max_n, n_frames, c->st);
     CU(cudaGetLastError());
     return max_n;
+}
+
+// Everything of the RGB-D Frame constructor (src/Frame.cc:200-237) after the inputs are in HBM: extraction, then ComputeStereoFromRGBD
+// as the gather of the uint16 depth plane, scaled per pixel like GrabImageRGBD's convertTo.  mvKeysUn == mvKeys (k1 == 0), as for RGB-L.
+static int process_rgbd(Ctx* c, int n_frames, float depth_scale, float bf) {
+    const int max_n = run_extract(c, n_frames);
+    if (max_n < 0) return max_n;
+    stage_begin(c, ST_DEPTH_GATHER, c->st);
+    launch_depth_gather_u16(c->st, c->d_depth16, depth16_frame_elems(c), c->depth16_pitch, depth_scale, c->d_kps, c->d_kps, c->d_n_sel, c->cap_kp, max_n, bf,
+                            c->d_depth, c->d_uright, n_frames);
+    stage_end(c, ST_DEPTH_GATHER, c->st, max_n > 0 ? 1 : 0);
+    CU(cudaGetLastError());
+    return max_n;
+}
+
+static int check_rgbd_params(Ctx* c, float depth_scale, float bf) {
+    if (!std::isfinite(depth_scale) || !(bf > 0.f) || !std::isfinite(bf)) { c->err = "depth_scale must be finite and bf > 0"; return RGBL_E_INVALID; }
+    return RGBL_OK;
 }
 
 static int download_rgbl(Ctx* c, int n_frames, rgbl_keypoint* kps, uint8_t* desc, float* depth, float* uright, int cap, int* n_out) {
@@ -859,6 +932,7 @@ int rgbl_resident_process(rgbl_ctx* ctx, const float P[12], const rgbl_depth_par
     if (!c) return RGBL_E_INVALID;
     if (!P || !prm) { c->err = "null argument"; return RGBL_E_INVALID; }
     if (c->resident_frames < 1) { c->err = "nothing uploaded"; return RGBL_E_INVALID; }
+    if (c->resident_rgbd) { c->err = "the uploaded frames are RGB-D frames (rgbl_resident_process_rgbd)"; return RGBL_E_INVALID; }
     CU(cudaSetDevice(c->cfg.device));
     int rc = process_rgbl(c, c->resident_frames, c->resident_max_pts, P, prm); if (rc < 0) return rc;
     if (n_out) { rc = fetch_counts(c, c->resident_frames); if (rc) return rc; }
@@ -875,6 +949,20 @@ int rgbl_resident_process(rgbl_ctx* ctx, const float P[12], const rgbl_depth_par
  * frame construction -> tracking chain (queued two deep on the tracking stream, continue_sequence from the second batch on) -> poses
  * (and, if asked for, the frame-construction outputs) back to the host.  Nothing synchronises with the device until a chain's results
  * are collected, one batch behind.                                                                                                   */
+// device buffers of a stage slot (allocated on first use; a slot can hold RGB-L and later RGB-D batches or the reverse)
+static int stage_slot_alloc(Ctx* c, Ctx::StageSlot& sl, bool rgbd) {
+    const size_t img_bytes = (size_t)c->levels[0].pitch * c->cfg.height, B = c->cfg.max_batch;
+    bool ok = sl.img || cudaMalloc((void**)&sl.img, B * img_bytes) == cudaSuccess;
+    if (rgbd) {
+        ok = ok && (sl.depth || cudaMalloc((void**)&sl.depth, B * depth16_frame_elems(c) * sizeof(uint16_t)) == cudaSuccess);
+    } else {
+        ok = ok && (sl.pts || cudaMalloc((void**)&sl.pts, B * 4 * c->cfg.max_points * sizeof(float)) == cudaSuccess);
+        ok = ok && (sl.n_pts || cudaMalloc((void**)&sl.n_pts, B * sizeof(int)) == cudaSuccess);
+    }
+    if (!ok) { cudaGetLastError(); c->err = "cudaMalloc failed (stage slot)"; return RGBL_E_CUDA; }
+    return RGBL_OK;
+}
+
 int rgbl_resident_stage(rgbl_ctx* ctx, int slot, int n_frames, const uint8_t* const* gray, int width, int height, int stride,
                         const float* const* pts4xn, const int* n_pts) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
@@ -887,13 +975,7 @@ int rgbl_resident_stage(rgbl_ctx* ctx, int slot, int n_frames, const uint8_t* co
     const LevelGeom& l0 = c->levels[0];
     const size_t img_bytes = (size_t)l0.pitch * c->cfg.height, pts_floats = (size_t)4 * c->cfg.max_points;
     Ctx::StageSlot& sl = c->stage[slot];
-    if (!sl.img) {
-        if (cudaMalloc((void**)&sl.img, (size_t)c->cfg.max_batch * img_bytes) != cudaSuccess ||
-            cudaMalloc((void**)&sl.pts, (size_t)c->cfg.max_batch * pts_floats * sizeof(float)) != cudaSuccess ||
-            cudaMalloc((void**)&sl.n_pts, (size_t)c->cfg.max_batch * sizeof(int)) != cudaSuccess) {
-            cudaGetLastError(); c->err = "cudaMalloc failed (stage slot)"; return RGBL_E_CUDA;
-        }
-    }
+    rc = stage_slot_alloc(c, sl, false); if (rc) return rc;
     int max_pts = 0;
     for (int f = 0; f < n_frames; ++f) {
         if (gray && !gray[f]) { c->err = "empty image"; return RGBL_E_EMPTY; }
@@ -905,42 +987,80 @@ int rgbl_resident_stage(rgbl_ctx* ctx, int slot, int n_frames, const uint8_t* co
     sl.h_n_pts.assign(n_pts, n_pts + n_frames);
     CU(cudaMemcpyAsync(sl.n_pts, sl.h_n_pts.data(), (size_t)n_frames * sizeof(int), cudaMemcpyHostToDevice, c->st));
     CU(cudaStreamSynchronize(c->st));
-    sl.n_frames = n_frames; sl.max_pts = max_pts;
+    sl.n_frames = n_frames; sl.max_pts = max_pts; sl.rgbd = false;
     return RGBL_OK;
 }
 
-// staged slot -> the context's working input buffers (device-to-device, ~76 MB per 32 KITTI frames: tens of microseconds)
-static int restage(Ctx* c, int slot) {
+int rgbl_resident_stage_rgbd(rgbl_ctx* ctx, int slot, int n_frames, const uint8_t* const* gray, int width, int height, int stride,
+                             const uint16_t* const* depth, int depth_stride) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return RGBL_E_INVALID;
+    if (!gray || !depth) { c->err = "null argument"; return RGBL_E_INVALID; }
+    if (slot < 0 || slot >= Ctx::kMaxStageSlots) { c->err = "stage slot out of range"; return RGBL_E_INVALID; }
+    int rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
+    if (depth_stride < width) { c->err = "depth_stride < width"; return RGBL_E_INVALID; }
+    for (int f = 0; f < n_frames; ++f) if (!gray[f] || !depth[f]) { c->err = "empty image"; return RGBL_E_EMPTY; }
+    CU(cudaSetDevice(c->cfg.device));
+    rc = ensure_depth16(c); if (rc) return rc;
+    const LevelGeom& l0 = c->levels[0];
+    const size_t img_bytes = (size_t)l0.pitch * c->cfg.height, dep = depth16_frame_elems(c);
+    Ctx::StageSlot& sl = c->stage[slot];
+    rc = stage_slot_alloc(c, sl, true); if (rc) return rc;
+    for (int f = 0; f < n_frames; ++f) {
+        CU(cudaMemcpy2DAsync(sl.img + (size_t)f * img_bytes, l0.pitch, gray[f], stride, c->cfg.width, c->cfg.height, cudaMemcpyHostToDevice, c->st));
+        CU(cudaMemcpy2DAsync(sl.depth + (size_t)f * dep, c->depth16_pitch * sizeof(uint16_t), depth[f], (size_t)depth_stride * sizeof(uint16_t),
+                             (size_t)c->cfg.width * sizeof(uint16_t), c->cfg.height, cudaMemcpyHostToDevice, c->st));
+    }
+    CU(cudaStreamSynchronize(c->st));
+    sl.n_frames = n_frames; sl.max_pts = 0; sl.rgbd = true;
+    return RGBL_OK;
+}
+
+// staged slot -> the context's working input buffers (device-to-device, ~76 MB per 32 KITTI frames: tens of microseconds); the slot must hold
+// frames of the kind the caller processes
+static int restage(Ctx* c, int slot, bool rgbd) {
     const Ctx::StageSlot& sl = c->stage[slot];
     if (!sl.img || sl.n_frames < 1) { c->err = "stage slot is empty"; return RGBL_E_INVALID; }
+    if (sl.rgbd != rgbd) { c->err = sl.rgbd ? "stage slot holds RGB-D frames (rgbl_track_sequence_rgbd)" : "stage slot holds RGB-L frames (rgbl_track_sequence)"; return RGBL_E_INVALID; }
     const LevelGeom& l0 = c->levels[0];
     const size_t img_bytes = (size_t)l0.pitch * c->cfg.height, pts_floats = (size_t)4 * c->cfg.max_points;
     for (int f = 0; f < sl.n_frames; ++f)
         CU(cudaMemcpyAsync(c->d_pyr + (size_t)f * c->frame_bytes + l0.off, sl.img + (size_t)f * img_bytes, img_bytes, cudaMemcpyDeviceToDevice, c->st));
-    CU(cudaMemcpyAsync(c->d_pts, sl.pts, (size_t)sl.n_frames * pts_floats * sizeof(float), cudaMemcpyDeviceToDevice, c->st_aux));
-    CU(cudaMemcpyAsync(c->d_n_pts, sl.n_pts, (size_t)sl.n_frames * sizeof(int), cudaMemcpyDeviceToDevice, c->st_aux));
-    for (int f = 0; f < sl.n_frames; ++f) c->h_n_pts[f] = sl.h_n_pts[f];
-    c->resident_frames = sl.n_frames; c->resident_max_pts = sl.max_pts;
+    if (rgbd) {
+        CU(cudaMemcpyAsync(c->d_depth16, sl.depth, (size_t)sl.n_frames * depth16_frame_elems(c) * sizeof(uint16_t), cudaMemcpyDeviceToDevice, c->st_aux));
+    } else {
+        CU(cudaMemcpyAsync(c->d_pts, sl.pts, (size_t)sl.n_frames * pts_floats * sizeof(float), cudaMemcpyDeviceToDevice, c->st_aux));
+        CU(cudaMemcpyAsync(c->d_n_pts, sl.n_pts, (size_t)sl.n_frames * sizeof(int), cudaMemcpyDeviceToDevice, c->st_aux));
+        for (int f = 0; f < sl.n_frames; ++f) c->h_n_pts[f] = sl.h_n_pts[f];
+    }
+    c->resident_frames = sl.n_frames; c->resident_max_pts = sl.max_pts; c->resident_rgbd = rgbd;
     return RGBL_OK;
 }
 
-int rgbl_track_sequence(rgbl_ctx* ctx, const float P[12], const rgbl_depth_params* prm, const rgbl_chain_params* chain, const rgbl_sequence_io* io) {
-    Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    if (!c) return RGBL_E_INVALID;
-    if (!P || !prm || !chain || !io || !io->poses || !io->n_matches || !io->n_inliers) { c->err = "null argument"; return RGBL_E_INVALID; }
+// Argument checks both sequence runners share (batch geometry, no chain in flight, staged-slot count, frame outputs).
+static int check_sequence_io(Ctx* c, const rgbl_chain_params* chain, const rgbl_sequence_io* io) {
+    if (!chain || !io || !io->poses || !io->n_matches || !io->n_inliers) { c->err = "null argument"; return RGBL_E_INVALID; }
     const int T = io->frames_per_batch, nb = io->n_batches;
     if (T < 1 || T > c->cfg.max_batch || nb < 1) { c->err = "bad batch geometry"; return RGBL_E_INVALID; }
     if (c->chain_pending) { c->err = "a tracking chain is in flight (rgbl_resident_track_end not called)"; return RGBL_E_INVALID; }
-    const bool host_in = io->gray != nullptr;
-    if (host_in) {
-        if (!io->pts4xn || !io->n_pts) { c->err = "null argument"; return RGBL_E_INVALID; }
+    if (io->gray) {
         int rc = check_batch_args(c, T, io->width, io->height, io->stride); if (rc) return rc;
     } else if (io->n_slots < 1 || io->n_slots > Ctx::kMaxStageSlots) { c->err = "resident mode needs 1..8 staged slots"; return RGBL_E_INVALID; }
-    const bool want_frames = io->kps != nullptr;
-    if (want_frames && (!io->desc || !io->depth || !io->uright || !io->n_kp || io->cap != c->cap_kp)) {
+    if (io->kps && (!io->desc || !io->depth || !io->uright || !io->n_kp || io->cap != c->cap_kp)) {
         c->err = "frame outputs need kps, desc, depth, uright, n_kp and cap == rgbl_keypoint_capacity()"; return RGBL_E_INVALID;
     }
-    CU(cudaSetDevice(c->cfg.device));
+    return RGBL_OK;
+}
+
+// The batch loop of both sequence runners: per batch  load(b) -> construct() -> (frame outputs D2H) -> tracking chain queued two deep
+// (continue_sequence from the second batch on), results collected one batch behind; on an error the queued chains are drained first.
+// load(b) puts batch b's inputs into the working buffers (host upload or staged slot); construct() runs the frame construction and
+// returns < 0 on error.
+static int run_sequence(Ctx* c, const rgbl_chain_params* chain, const rgbl_sequence_io* io, const std::function<int(int)>& load,
+                        const std::function<int()>& construct) {
+    rgbl_ctx* ctx = reinterpret_cast<rgbl_ctx*>(c);
+    const int T = io->frames_per_batch, nb = io->n_batches;
+    const bool want_frames = io->kps != nullptr;
     rgbl_chain_params cp = *chain;
     int collected = 0;
     auto collect = [&]() -> int {
@@ -951,15 +1071,10 @@ int rgbl_track_sequence(rgbl_ctx* ctx, const float P[12], const rgbl_depth_param
         return rc;
     };
     for (int b = 0; b < nb; ++b) {
-        int max_pts = 0, rc;
-        if (host_in) {
-            rc = upload_rgbl(c, T, io->gray + (size_t)b * T, io->stride, io->pts4xn + (size_t)b * T, io->n_pts + (size_t)b * T, &max_pts);
-        } else {
-            rc = restage(c, (io->first_slot + b) % io->n_slots); max_pts = c->resident_max_pts;
-            if (!rc && c->resident_frames != T) { c->err = "staged slot holds a different number of frames"; rc = RGBL_E_INVALID; }
-        }
+        int rc = load(b);
+        if (!rc && c->resident_frames != T) { c->err = "staged slot holds a different number of frames"; rc = RGBL_E_INVALID; }
         if (rc) { while (c->chain_pending) collect(); return rc; }
-        rc = process_rgbl(c, T, max_pts, P, prm);
+        rc = construct();
         if (rc < 0) { while (c->chain_pending) collect(); return rc; }
         if (want_frames) {        // whole [T][cap] arrays + counts, asynchronously behind the batch's kernels
             const size_t o = (size_t)b * T, n = (size_t)T * c->cap_kp;
@@ -980,6 +1095,105 @@ int rgbl_track_sequence(rgbl_ctx* ctx, const float P[12], const rgbl_depth_param
     CU(cudaStreamSynchronize(c->st_aux));
     prof_collect(c);
     return rc_all;
+}
+
+int rgbl_track_sequence(rgbl_ctx* ctx, const float P[12], const rgbl_depth_params* prm, const rgbl_chain_params* chain, const rgbl_sequence_io* io) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return RGBL_E_INVALID;
+    if (!P || !prm) { c->err = "null argument"; return RGBL_E_INVALID; }
+    int rc = check_sequence_io(c, chain, io); if (rc) return rc;
+    if (io->gray && (!io->pts4xn || !io->n_pts)) { c->err = "null argument"; return RGBL_E_INVALID; }
+    CU(cudaSetDevice(c->cfg.device));
+    const int T = io->frames_per_batch;
+    int max_pts = 0;
+    auto load = [&](int b) -> int {
+        if (io->gray) return upload_rgbl(c, T, io->gray + (size_t)b * T, io->stride, io->pts4xn + (size_t)b * T, io->n_pts + (size_t)b * T, &max_pts);
+        const int r = restage(c, (io->first_slot + b) % io->n_slots, false);
+        max_pts = c->resident_max_pts;
+        return r;
+    };
+    return run_sequence(c, chain, io, load, [&]() { return process_rgbl(c, T, max_pts, P, prm); });
+}
+
+int rgbl_track_sequence_rgbd(rgbl_ctx* ctx, float depth_scale, float bf, const rgbl_chain_params* chain, const rgbl_sequence_io* io,
+                             const uint16_t* const* depth, int depth_stride) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return RGBL_E_INVALID;
+    int rc = check_sequence_io(c, chain, io); if (rc) return rc;
+    rc = check_rgbd_params(c, depth_scale, bf); if (rc) return rc;
+    if (io->pts4xn || io->n_pts) { c->err = "RGB-D sequences take depth images, not point clouds (pts4xn / n_pts must be NULL)"; return RGBL_E_INVALID; }
+    if (io->gray && (!depth || depth_stride < io->width)) { c->err = "host mode needs one depth image per frame and depth_stride >= width"; return RGBL_E_INVALID; }
+    CU(cudaSetDevice(c->cfg.device));
+    const int T = io->frames_per_batch;
+    auto load = [&](int b) -> int {
+        if (!io->gray) return restage(c, (io->first_slot + b) % io->n_slots, true);
+        for (int f = 0; f < T; ++f) if (!io->gray[(size_t)b * T + f]) { c->err = "empty image"; return RGBL_E_EMPTY; }
+        int r = upload_depth16(c, T, depth + (size_t)b * T, depth_stride, c->st_aux); if (r) return r;
+        r = upload_images(c, T, io->gray + (size_t)b * T, io->stride, c->st); if (r) return r;
+        c->resident_frames = T; c->resident_max_pts = 0; c->resident_rgbd = true;
+        return RGBL_OK;
+    };
+    return run_sequence(c, chain, io, load, [&]() { return process_rgbd(c, T, depth_scale, bf); });
+}
+
+// ---- RGB-D frame construction (resident form) ----
+int rgbl_resident_upload_rgbd(rgbl_ctx* ctx, int n_frames, const uint8_t* const* gray, int width, int height, int stride, const uint16_t* const* depth,
+                              int depth_stride) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return RGBL_E_INVALID;
+    if (!gray || !depth) { c->err = "null argument"; return RGBL_E_INVALID; }
+    int rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
+    for (int f = 0; f < n_frames; ++f) if (!gray[f]) { c->err = "empty image"; return RGBL_E_EMPTY; }
+    CU(cudaSetDevice(c->cfg.device));
+    rc = upload_depth16(c, n_frames, depth, depth_stride, c->st_aux); if (rc) return rc;
+    rc = upload_images(c, n_frames, gray, stride, c->st); if (rc) return rc;
+    CU(cudaStreamSynchronize(c->st));
+    CU(cudaStreamSynchronize(c->st_aux));
+    c->resident_frames = n_frames; c->resident_max_pts = 0; c->resident_rgbd = true;
+    return RGBL_OK;
+}
+
+int rgbl_resident_upload_rgbd_png(rgbl_ctx* ctx, int n_frames, const uint8_t* const* png, const size_t* png_bytes, int camera_rgb,
+                                  const uint8_t* const* depth_png, const size_t* depth_png_bytes) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return RGBL_E_INVALID;
+    if (!png || !png_bytes || !depth_png || !depth_png_bytes) { c->err = "null argument"; return RGBL_E_INVALID; }
+    int rc = check_batch_args(c, n_frames, c->cfg.width, c->cfg.height, c->cfg.width); if (rc) return rc;
+    CU(cudaSetDevice(c->cfg.device));
+    rc = decode_png_to_level0(c, n_frames, png, png_bytes, camera_rgb, c->st); if (rc) return rc;
+    rc = decode_png_to_depth16(c, n_frames, depth_png, depth_png_bytes, c->st); if (rc) return rc;
+    c->resident_frames = n_frames; c->resident_max_pts = 0; c->resident_rgbd = true;
+    return RGBL_OK;
+}
+
+int rgbl_decode_png_depth16(rgbl_ctx* ctx, int n_frames, const uint8_t* const* png, const size_t* png_bytes, uint16_t* const* depth_out, int stride) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return RGBL_E_INVALID;
+    if (!png || !png_bytes || !depth_out) { c->err = "null argument"; return RGBL_E_INVALID; }
+    int rc = check_batch_args(c, n_frames, c->cfg.width, c->cfg.height, stride); if (rc) return rc;
+    for (int f = 0; f < n_frames; ++f) if (!depth_out[f]) { c->err = "null output image"; return RGBL_E_INVALID; }
+    CU(cudaSetDevice(c->cfg.device));
+    rc = decode_png_to_depth16(c, n_frames, png, png_bytes, c->st); if (rc) return rc;
+    for (int f = 0; f < n_frames; ++f)
+        CU(cudaMemcpy2DAsync(depth_out[f], (size_t)stride * sizeof(uint16_t), c->d_depth16 + (size_t)f * depth16_frame_elems(c), c->depth16_pitch * sizeof(uint16_t),
+                             (size_t)c->cfg.width * sizeof(uint16_t), c->cfg.height, cudaMemcpyDeviceToHost, c->st));
+    CU(cudaStreamSynchronize(c->st));
+    return RGBL_OK;
+}
+
+int rgbl_resident_process_rgbd(rgbl_ctx* ctx, float depth_scale, float bf, int* n_out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return RGBL_E_INVALID;
+    if (c->resident_frames < 1 || !c->resident_rgbd) { c->err = "no RGB-D frames uploaded (rgbl_resident_upload_rgbd / _rgbd_png)"; return RGBL_E_INVALID; }
+    int rc = check_rgbd_params(c, depth_scale, bf); if (rc) return rc;
+    CU(cudaSetDevice(c->cfg.device));
+    rc = process_rgbd(c, c->resident_frames, depth_scale, bf); if (rc < 0) return rc;
+    if (n_out) { rc = fetch_counts(c, c->resident_frames); if (rc) return rc; }
+    CU(cudaStreamSynchronize(c->st));
+    CU(cudaStreamSynchronize(c->st_aux));
+    prof_collect(c);
+    if (n_out) for (int f = 0; f < c->resident_frames; ++f) n_out[f] = c->h_n_sel[f];
+    return RGBL_OK;
 }
 
 int rgbl_resident_download(rgbl_ctx* ctx, rgbl_keypoint* kps, uint8_t* desc, float* depth, float* uright, int cap, int* n_out) {

@@ -9,7 +9,7 @@
 //   resolve+dilate : per tile, recompute the winning point's depth (same arithmetic), build the
 //              inverted map t = M - d (zeroed above M-1), take the max over the structuring element,
 //              invert back: the exact float pipeline of Upsample_InverseDilation.
-//   gather   : GetFeatureDepthFromDepthMap (:82-104).
+//   gather   : GetFeatureDepthFromDepthMap (:82-104), and Frame::ComputeStereoFromRGBD (src/Frame.cc:1074-1095) on a uint16 RGB-D plane.
 #include <cfloat>
 
 #include "rgbl_device.cuh"
@@ -116,7 +116,14 @@ __global__ void __launch_bounds__(256) depth_resolve_dilate_kernel(const float* 
     }
 }
 
-__global__ void __launch_bounds__(256) depth_gather_kernel(const float* __restrict__ processed, int W, int H,
+// The plane holds metric depth (float: the processed LiDAR depth map, or a scaled RGB-D map) or the raw 16-bit RGB-D samples, scaled here
+// as Tracking::GrabImageRGBD's imDepth.convertTo(CV_32F, mDepthMapFactor) does per pixel (src/Tracking.cc:1538-1539): (float)u * scale,
+// rounded once - so the bits equal convert-then-gather.
+__device__ __forceinline__ float depth_sample(float d, float) { return d; }
+__device__ __forceinline__ float depth_sample(uint16_t u, float scale) { return __fmul_rn((float)u, scale); }
+
+template <class T>
+__global__ void __launch_bounds__(256) depth_gather_kernel(const T* __restrict__ plane, size_t frame_elems, size_t pitch_elems, float scale,
                                                            const rgbl_keypoint* __restrict__ kps,
                                                            const rgbl_keypoint* __restrict__ kps_un,
                                                            const int* __restrict__ n_kp, int cap, float bf,
@@ -126,7 +133,7 @@ __global__ void __launch_bounds__(256) depth_gather_kernel(const float* __restri
     if (k >= n_kp[frame]) return;
     const size_t o = (size_t)frame * cap + k;
     const float u = kps[o].x, v = kps[o].y;
-    const float d = __ldg(processed + (size_t)frame * W * H + (size_t)(int)v * W + (int)u);
+    const float d = depth_sample(__ldg(plane + (size_t)frame * frame_elems + (size_t)(int)v * pitch_elems + (int)u), scale);
     float dd = -1.f, ur = -1.f;
     if (d > 0.f && bf >= 0.f) {          // bf < 0: LiDAR.Method None -> no depth association
         dd = d;
@@ -272,8 +279,15 @@ void launch_depth_gather(cudaStream_t st, const float* processed, int W, int H, 
                          const rgbl_keypoint* kps_un, const int* n_kp, int cap, int max_n, float bf, float* depth,
                          float* uright, int n_frames) {
     if (max_n <= 0) return;
-    depth_gather_kernel<<<dim3((max_n + 255) / 256, n_frames), 256, 0, st>>>(processed, W, H, kps, kps_un, n_kp, cap, bf,
-                                                                            depth, uright);
+    depth_gather_kernel<float><<<dim3((max_n + 255) / 256, n_frames), 256, 0, st>>>(processed, (size_t)W * H, (size_t)W, 1.f, kps, kps_un, n_kp, cap, bf,
+                                                                                   depth, uright);
+}
+
+void launch_depth_gather_u16(cudaStream_t st, const uint16_t* plane, size_t frame_elems, size_t pitch_elems, float scale, const rgbl_keypoint* kps,
+                             const rgbl_keypoint* kps_un, const int* n_kp, int cap, int max_n, float bf, float* depth, float* uright, int n_frames) {
+    if (max_n <= 0) return;
+    depth_gather_kernel<uint16_t><<<dim3((max_n + 255) / 256, n_frames), 256, 0, st>>>(plane, frame_elems, pitch_elems, scale, kps, kps_un, n_kp, cap, bf,
+                                                                                      depth, uright);
 }
 
 }  // namespace rgbl

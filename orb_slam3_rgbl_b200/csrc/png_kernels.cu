@@ -11,6 +11,8 @@
 // The gray formula is cv::cvtColor's 8-bit one (15-bit fixed point: 9798, 19235, 3735, + 2^14, >> 15; pinned against cv2 on all 2^24
 // colours); imread hands colour data over as B, G, R(, A), so with Camera.RGB = 1 (COLOR_RGB2GRAY) channel 0 = the file's BLUE is
 // weighted as red - reproduced as is.
+// The depth input of Tracking::GrabImageRGBD (src/Tracking.cc:1518) runs through the same kernel: a 16-bit gray PNG has two bytes per pixel,
+// filtered byte-wise like any other, and the output stage writes the big-endian sample as uint16 into the frame's depth plane instead.
 #include <zlib.h>
 
 #include <cstring>
@@ -26,7 +28,8 @@ namespace {
 
 constexpr int kPngRows = 512;
 
-template <int CH>
+// DEPTH16: CH = 2 bytes of one big-endian 16-bit sample -> uint16 at (pyr + frame * frame_stride + off0) with row pitch pitch0 bytes
+template <int CH, bool DEPTH16 = false>
 __global__ void __launch_bounds__(kPngRows) png_unfilter_gray_kernel(const uint8_t* __restrict__ raw, size_t raw_stride, int w, int h, int camera_rgb,
                                                                      uint8_t* __restrict__ pyr, size_t frame_stride, int off0, int pitch0,
                                                                      uint32_t* __restrict__ band_rows, int* __restrict__ status) {
@@ -70,12 +73,20 @@ __global__ void __launch_bounds__(kPngRows) png_unfilter_gray_kernel(const uint8
                 a = px; c = b;
                 ex[s & 1][tid] = px;
                 if (tid == rows - 1 && y0 + kPngRows < h) brow[x] = px;             // the row above the next band
-                uint32_t g = px;
-                if (CH >= 3) g = ((px & 255) * k0 + ((px >> 8) & 255) * 19235u + ((px >> 16) & 255) * k2 + (1u << 14)) >> 15;
-                gacc |= (g & 255u) << (8 * (x & 3));
-                if ((x & 3) == 3 || x == w - 1) {                                  // rows are 64-byte aligned and padded: whole words
-                    *reinterpret_cast<uint32_t*>(dst + (size_t)y * pitch0 + (x & ~3)) = gacc;
-                    gacc = 0;
+                if constexpr (DEPTH16) {
+                    gacc |= (((px & 255u) << 8) | ((px >> 8) & 255u)) << (16 * (x & 1));
+                    if ((x & 1) == 1 || x == w - 1) {                              // depth rows are 64-byte aligned and padded too
+                        *reinterpret_cast<uint32_t*>(dst + (size_t)y * pitch0 + (size_t)(x & ~1) * 2) = gacc;
+                        gacc = 0;
+                    }
+                } else {
+                    uint32_t g = px;
+                    if (CH >= 3) g = ((px & 255) * k0 + ((px >> 8) & 255) * 19235u + ((px >> 16) & 255) * k2 + (1u << 14)) >> 15;
+                    gacc |= (g & 255u) << (8 * (x & 3));
+                    if ((x & 3) == 3 || x == w - 1) {                              // rows are 64-byte aligned and padded: whole words
+                        *reinterpret_cast<uint32_t*>(dst + (size_t)y * pitch0 + (x & ~3)) = gacc;
+                        gacc = 0;
+                    }
                 }
             }
             if (live && x + 1 >= 0 && x + 1 < w) f_next = load_px(src, x + 1);      // in flight across the barrier
@@ -89,7 +100,8 @@ inline uint32_t be32(const uint8_t* p) { return ((uint32_t)p[0] << 24) | ((uint3
 }  // namespace
 
 // One PNG stream -> its filtered scanlines ((w * ch + 1) * h bytes) in `out`.  Returns 0 or a negative code with `err` set.
-int png_inflate_host(const uint8_t* png, size_t n, int want_w, int want_h, uint8_t* out, size_t cap, int* ch_out, std::string& err) {
+// depth16: the caller expects a depth image (16-bit gray only, ch = 2 bytes per pixel); else an image (8-bit gray / RGB / RGBA).
+int png_inflate_host(const uint8_t* png, size_t n, int want_w, int want_h, uint8_t* out, size_t cap, int* ch_out, std::string& err, bool depth16) {
     static const uint8_t sig[8] = {137, 80, 78, 71, 13, 10, 26, 10};
     if (!png || n < 8 + 25 || std::memcmp(png, sig, 8)) { err = "not a PNG stream"; return -1; }
     size_t pos = 8;
@@ -109,9 +121,15 @@ int png_inflate_host(const uint8_t* png, size_t n, int want_w, int want_h, uint8
         if (!std::memcmp(type, "IHDR", 4)) {
             if (len != 13 || ch) return fail("bad IHDR", -3);
             const int w = (int)be32(data), h = (int)be32(data + 4), ctype = data[9];
-            if (data[8] != 8 || data[12] != 0 || data[10] != 0 || data[11] != 0) return fail("only 8-bit non-interlaced PNG is supported (what imread returns as CV_8U unchanged)", -2);
-            ch = ctype == 0 ? 1 : ctype == 2 ? 3 : ctype == 6 ? 4 : 0;
-            if (!ch) return fail("PNG colour type not supported (gray, RGB, RGBA only)", -2);
+            if (depth16) {
+                if (data[8] != 16 || ctype != 0 || data[12] != 0 || data[10] != 0 || data[11] != 0)
+                    return fail("a depth PNG must be 16-bit single-channel gray, non-interlaced (what imread returns as CV_16U)", -2);
+                ch = 2;
+            } else {
+                if (data[8] != 8 || data[12] != 0 || data[10] != 0 || data[11] != 0) return fail("only 8-bit non-interlaced PNG is supported (what imread returns as CV_8U unchanged)", -2);
+                ch = ctype == 0 ? 1 : ctype == 2 ? 3 : ctype == 6 ? 4 : 0;
+                if (!ch) return fail("PNG colour type not supported (gray, RGB, RGBA only)", -2);
+            }
             if (w != want_w || h != want_h) return fail("PNG size does not match the context", -4);
             need = ((size_t)w * ch + 1) * h;
             if (need > cap) return fail("PNG staging buffer too small", -4);
@@ -139,14 +157,14 @@ int png_inflate_host(const uint8_t* png, size_t n, int want_w, int want_h, uint8
 
 // n PNG streams -> staged filtered scanlines (pinned h_raw, one slot of raw_stride bytes per frame), in parallel over the frames.
 int png_inflate_batch(int n_frames, const uint8_t* const* png, const size_t* png_bytes, int w, int h, uint8_t* h_raw, size_t raw_stride, int* ch_out,
-                      std::string& err) {
+                      std::string& err, bool depth16) {
     std::vector<int> rc(n_frames, 0), ch(n_frames, 0);
     std::vector<std::string> errs(n_frames);
     const int hw = (int)std::thread::hardware_concurrency();
     const int n_workers = std::max(1, std::min(n_frames, hw > 0 ? hw : 4));
     auto work = [&](int t) {
         for (int f = t; f < n_frames; f += n_workers)
-            rc[f] = png_inflate_host(png[f], png_bytes[f], w, h, h_raw + (size_t)f * raw_stride, raw_stride, &ch[f], errs[f]);
+            rc[f] = png_inflate_host(png[f], png_bytes[f], w, h, h_raw + (size_t)f * raw_stride, raw_stride, &ch[f], errs[f], depth16);
     };
     std::vector<std::thread> th;
     for (int t = 1; t < n_workers; ++t) th.emplace_back(work, t);
@@ -165,6 +183,12 @@ void launch_png_unfilter_gray(cudaStream_t st, const uint8_t* d_raw, size_t raw_
     if (channels == 1) png_unfilter_gray_kernel<1><<<n_frames, kPngRows, 0, st>>>(d_raw, raw_stride, w, h, camera_rgb, pyr, frame_stride, l0.off, l0.pitch, band_rows, status);
     else if (channels == 3) png_unfilter_gray_kernel<3><<<n_frames, kPngRows, 0, st>>>(d_raw, raw_stride, w, h, camera_rgb, pyr, frame_stride, l0.off, l0.pitch, band_rows, status);
     else png_unfilter_gray_kernel<4><<<n_frames, kPngRows, 0, st>>>(d_raw, raw_stride, w, h, camera_rgb, pyr, frame_stride, l0.off, l0.pitch, band_rows, status);
+}
+
+void launch_png_unfilter_depth16(cudaStream_t st, const uint8_t* d_raw, size_t raw_stride, int w, int h, uint16_t* depth, size_t frame_elems,
+                                 size_t pitch_elems, uint32_t* band_rows, int* status, int n_frames) {
+    png_unfilter_gray_kernel<2, true><<<n_frames, kPngRows, 0, st>>>(d_raw, raw_stride, w, h, 0, reinterpret_cast<uint8_t*>(depth), frame_elems * 2, 0,
+                                                                      (int)(pitch_elems * 2), band_rows, status);
 }
 
 }  // namespace rgbl

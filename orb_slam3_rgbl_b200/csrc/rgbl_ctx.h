@@ -116,6 +116,10 @@ struct Ctx {
     uint32_t* d_png_band = nullptr;
     int *d_png_status = nullptr, *h_png_status = nullptr;
     size_t png_raw_stride = 0;
+    // RGB-D (lazily allocated by the first RGB-D call): one uint16 depth plane per frame slot as imread returns it (CV_16U), row pitch
+    // depth16_pitch elements (64-byte rows); scaled to metric depth by the gather
+    uint16_t* d_depth16 = nullptr;
+    size_t depth16_pitch = 0;
     int* d_n_pts = nullptr;
     uint32_t* d_idx_map = nullptr;
     float *d_raw = nullptr, *d_processed = nullptr, *d_depth = nullptr, *d_uright = nullptr;
@@ -185,13 +189,15 @@ struct Ctx {
     ChainGraphKey chain_key[2] = {};
     const void* chain_timing_ev = nullptr;   // RGBL_CHAIN_TIMING development aid
 
-    // staged input slots of the sequence runner (rgbl_resident_stage / rgbl_track_sequence): level-0 planes + clouds of whole batches
+    // staged input slots of the sequence runners (rgbl_resident_stage / rgbl_track_sequence, rgbl_resident_stage_rgbd /
+    // rgbl_track_sequence_rgbd): level-0 planes + clouds (RGB-L) or uint16 depth planes (RGB-D) of whole batches
     static constexpr int kMaxStageSlots = 8;
-    struct StageSlot { uint8_t* img = nullptr; float* pts = nullptr; int* n_pts = nullptr; std::vector<int> h_n_pts; int n_frames = 0, max_pts = 0; };
+    struct StageSlot { uint8_t* img = nullptr; float* pts = nullptr; int* n_pts = nullptr; uint16_t* depth = nullptr; std::vector<int> h_n_pts; int n_frames = 0, max_pts = 0; bool rgbd = false; };
     StageSlot stage[kMaxStageSlots];
 
     int last_frames = 0;         // frames valid in the device buffers
     int resident_frames = 0, resident_max_pts = 0;
+    bool resident_rgbd = false;  // the uploaded frames are RGB-D frames (image + depth plane), not RGB-L ones
     bool blur_valid = false;
 };
 

@@ -37,10 +37,14 @@ void launch_compact(cudaStream_t st, const LevelGeom* d_levels, int n_levels, in
                     const int* counts, int* cell_off, int* level_cnt, int* frame_total, uint32_t* dense, int dense_cap,
                     int* overflow, int n_frames);
 // png_kernels.cu: cv::imread of PNG streams (host: chunks + zlib inflate; device: scanline reconstruction + cvtColor to gray) -----------
+// depth16: the streams are depth images (16-bit gray only, 2 bytes per pixel); else images (8-bit gray / RGB / RGBA)
 int png_inflate_batch(int n_frames, const uint8_t* const* png, const size_t* png_bytes, int w, int h, uint8_t* h_raw, size_t raw_stride, int* ch_out,
-                      std::string& err);
+                      std::string& err, bool depth16 = false);
 void launch_png_unfilter_gray(cudaStream_t st, const uint8_t* d_raw, size_t raw_stride, int w, int h, int channels, int camera_rgb, uint8_t* pyr,
                               size_t frame_stride, const LevelGeom& l0, uint32_t* band_rows, int* status, int n_frames);
+// 16-bit depth PNG scanlines (ch = 2) -> uint16 depth planes (frame f at depth + f * frame_elems, row pitch pitch_elems, pitch a multiple of 32)
+void launch_png_unfilter_depth16(cudaStream_t st, const uint8_t* d_raw, size_t raw_stride, int w, int h, uint16_t* depth, size_t frame_elems,
+                                 size_t pitch_elems, uint32_t* band_rows, int* status, int n_frames);
 // level_tma_kernels.cu: fused per-level TMA tile kernel (blur of level l + level l+1 from one read of level l) -----------------------
 struct LevelTensorMaps { alignas(64) unsigned char map[RGBL_MAX_LEVELS][128]; int n_levels; };     // raw CUtensorMap objects, one per level
 int make_level_tensor_maps(uint8_t* pyr, size_t frame_stride, int n_slots, const LevelGeom* levels, int n_levels, LevelTensorMaps* out);
@@ -91,6 +95,9 @@ void launch_depth_nn_pixel(cudaStream_t st, const float* raw, int W, int H, cons
 void launch_depth_gather(cudaStream_t st, const float* processed, int W, int H, const rgbl_keypoint* kps,
                          const rgbl_keypoint* kps_un, const int* n_kp, int cap, int max_n, float bf, float* depth,
                          float* uright, int n_frames);
+// the same gather on uint16 RGB-D depth planes, metric depth = (float)sample * scale (Tracking::mDepthMapFactor)
+void launch_depth_gather_u16(cudaStream_t st, const uint16_t* plane, size_t frame_elems, size_t pitch_elems, float scale, const rgbl_keypoint* kps,
+                             const rgbl_keypoint* kps_un, const int* n_kp, int cap, int max_n, float bf, float* depth, float* uright, int n_frames);
 
 
 // match_kernels.cu ---------------------------------------------------------------------------------

@@ -94,6 +94,25 @@ def decode_png_gray(ctx: "Context", png_list, camera_rgb=True):
     return outs
 
 
+def decode_png_depth16(ctx: "Context", png_list):
+    """cv::imread(IMREAD_UNCHANGED) of a batch of 16-bit depth PNG streams (rgbl_decode_png_depth16) -> list of uint16 images (H x W)."""
+    n = len(png_list)
+    bufs = [np.frombuffer(b, np.uint8) for b in png_list]
+    pa = (C.c_void_p * n)(*[b.ctypes.data for b in bufs])
+    sizes = (C.c_size_t * n)(*[len(b) for b in bufs])
+    outs = [np.empty((ctx.height, ctx.width), np.uint16) for _ in range(n)]
+    oa = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
+    check(lib().rgbl_decode_png_depth16(ctx.handle, n, pa, sizes, oa, ctx.width), ctx.handle)
+    return outs
+
+
+def depth_map_factor(factor: float) -> float:
+    """Tracking::mDepthMapFactor from the settings' RGBD.DepthMapFactor (src/Tracking.cc:1188-1204): 1.0f / factor computed in float,
+    1 when |factor| < 1e-5.  The depth_scale of the RGB-D entry points."""
+    f = np.float32(factor)
+    return float(np.float32(1.0) if abs(f) < np.float32(1e-5) else np.float32(1.0) / f)
+
+
 class ORBextractor:
     """ORB_SLAM3::ORBextractor drop-in (src/ORBextractor.cc)."""
 
@@ -608,6 +627,54 @@ class RgblBatch:
         return [(self.kps[f, :self.n[f]], self.desc[f, :self.n[f]], self.depth[f, :self.n[f]], self.uright[f, :self.n[f]]) for f in range(self.nF)]
 
 
+class RgbdBatch:
+    """Host buffers of one batch of RGB-D frames (gray image + CV_16U depth image each) for the resident RGB-D API: the RGB-D Frame
+    constructor (src/Frame.cc:200-237) is upload + process_resident; download / track_begin2 / track_end2 as for RgblBatch."""
+
+    def __init__(self, ctx: Context, images, depths, pinned=True):
+        self.ctx = ctx
+        nF = len(images); cap = ctx.cap
+        self.nF, self.cap = nF, cap
+        alloc = _pinned_alloc if pinned else (lambda shape, dt: np.empty(shape, dt))
+        H, W = images[0].shape
+        self.W, self.H = W, H
+        self.img = alloc((nF, H, W), np.uint8); self.dep = alloc((nF, H, W), np.uint16)
+        self.set_inputs(images, depths)
+        self.ia = (C.c_void_p * nF)(*[self.img[f].ctypes.data for f in range(nF)])
+        self.da = (C.c_void_p * nF)(*[self.dep[f].ctypes.data for f in range(nF)])
+        self.kps = alloc((nF, cap), KP_DTYPE); self.desc = alloc((nF, cap, 32), np.uint8)
+        self.depth = alloc((nF, cap), np.float32); self.uright = alloc((nF, cap), np.float32)
+        self.n = np.zeros(nF, np.int32)
+
+    def set_inputs(self, images, depths):
+        assert len(images) == self.nF and len(depths) == self.nF
+        for f in range(self.nF):
+            self.img[f] = images[f]
+            self.dep[f] = np.asarray(depths[f], np.uint16)
+
+    def upload(self):
+        c = self.ctx
+        check(lib().rgbl_resident_upload_rgbd(c.handle, self.nF, self.ia, self.W, self.H, self.W, self.da, self.W), c.handle)
+
+    def upload_png(self, png_list, depth_png_list, camera_rgb=True):
+        """Resident upload of the files' bytes: image PNGs (imread + cvtColor to gray) and 16-bit depth PNGs (imread IMREAD_UNCHANGED)."""
+        c = self.ctx
+        bufs = [np.frombuffer(b, np.uint8) for b in png_list]; dbufs = [np.frombuffer(b, np.uint8) for b in depth_png_list]
+        pa = (C.c_void_p * self.nF)(*[b.ctypes.data for b in bufs]); da = (C.c_void_p * self.nF)(*[b.ctypes.data for b in dbufs])
+        sizes = (C.c_size_t * self.nF)(*[len(b) for b in bufs]); dsizes = (C.c_size_t * self.nF)(*[len(b) for b in dbufs])
+        check(lib().rgbl_resident_upload_rgbd_png(c.handle, self.nF, pa, sizes, int(bool(camera_rgb)), da, dsizes), c.handle)
+
+    def process_resident(self, depth_scale: float, bf: float):
+        """depth_scale = Tracking::mDepthMapFactor (depth_map_factor(RGBD.DepthMapFactor)), bf = Camera.bf -> keypoints per frame"""
+        c = self.ctx
+        check(lib().rgbl_resident_process_rgbd(c.handle, depth_scale, bf, ptr(self.n)), c.handle)
+        return self.n
+
+    download = RgblBatch.download
+    track_begin2 = RgblBatch.track_begin2
+    track_end2 = RgblBatch.track_end2
+
+
 class SequenceIO(C.Structure):
     """rgbl_sequence_io (include/rgbl_b200.h)."""
     _fields_ = [("n_batches", C.c_int), ("frames_per_batch", C.c_int), ("width", C.c_int), ("height", C.c_int), ("stride", C.c_int),
@@ -630,8 +697,28 @@ class SequenceRunner:
         self.P = np.ascontiguousarray(P, np.float32).reshape(12)
         self.prm = depth_params
         self._out = None
+        self.rgbd_mode = False
+
+    @classmethod
+    def rgbd(cls, ctx: Context, depth_scale: float, bf: float, T: int, W: int, H: int, n_host_batches: int, pinned=True) -> "SequenceRunner":
+        """RGB-D mode (rgbl_track_sequence_rgbd, the loop of Examples/RGB-D/rgbd_kitti.cc): batches of gray images + CV_16U depth images;
+        set_batch(m, images, depths).  depth_scale = Tracking::mDepthMapFactor, bf = Camera.bf."""
+        self = cls.__new__(cls)
+        self.ctx, self.T, self.W, self.H, self.M, self.maxn = ctx, T, W, H, n_host_batches, 0
+        self._alloc = _pinned_alloc if pinned else (lambda shape, dt: np.empty(shape, dt))
+        self.img = self._alloc((self.M, T, H, W), np.uint8)
+        self.dep = self._alloc((self.M, T, H, W), np.uint16)
+        self.depth_scale, self.bf = float(depth_scale), float(bf)
+        self._out = None
+        self.rgbd_mode = True
+        return self
 
     def set_batch(self, m: int, images, clouds):
+        """clouds: 4 x N point clouds (RGB-L), or the uint16 depth images in RGB-D mode."""
+        if self.rgbd_mode:
+            for f in range(self.T):
+                self.img[m, f] = images[f]; self.dep[m, f] = np.asarray(clouds[f], np.uint16)
+            return
         for f in range(self.T):
             self.img[m, f] = images[f]
             n = clouds[f].shape[1]
@@ -639,8 +726,12 @@ class SequenceRunner:
             self.npts[m, f] = n
 
     def stage(self, slot: int, m: int):
-        """Upload host batch m into device slot `slot` (rgbl_resident_stage)."""
+        """Upload host batch m into device slot `slot` (rgbl_resident_stage / rgbl_resident_stage_rgbd)."""
         ia = (C.c_void_p * self.T)(*[self.img[m, f].ctypes.data for f in range(self.T)])
+        if self.rgbd_mode:
+            da = (C.c_void_p * self.T)(*[self.dep[m, f].ctypes.data for f in range(self.T)])
+            check(lib().rgbl_resident_stage_rgbd(self.ctx.handle, slot, self.T, ia, self.W, self.H, self.W, da, self.W), self.ctx.handle)
+            return
         pa = (C.c_void_p * self.T)(*[self.pts[m, f].ctypes.data for f in range(self.T)])
         n = np.ascontiguousarray(self.npts[m])
         check(lib().rgbl_resident_stage(self.ctx.handle, slot, self.T, ia, self.W, self.H, self.W, pa, ptr(n)), self.ctx.handle)
@@ -670,8 +761,15 @@ class SequenceRunner:
         io = SequenceIO()
         io.n_batches, io.frames_per_batch, io.width, io.height, io.stride = n_batches, T, self.W, self.H, self.W
         keep = []
+        da = None
         if resident_slots > 0:
             io.gray = None; io.pts4xn = None; io.n_pts = None; io.n_slots = resident_slots; io.first_slot = first % resident_slots
+        elif self.rgbd_mode:
+            idx = [(first + b) % self.M for b in range(n_batches)]
+            ga = (C.c_void_p * (n_batches * T))(*[self.img[m, f].ctypes.data for m in idx for f in range(T)])
+            da = (C.c_void_p * (n_batches * T))(*[self.dep[m, f].ctypes.data for m in idx for f in range(T)])
+            keep += [ga, da]
+            io.gray = C.cast(ga, C.c_void_p); io.pts4xn = None; io.n_pts = None
         else:
             idx = [(first + b) % self.M for b in range(n_batches)]
             ga = (C.c_void_p * (n_batches * T))(*[self.img[m, f].ctypes.data for m in idx for f in range(T)])
@@ -684,10 +782,15 @@ class SequenceRunner:
         if want_frames:
             io.kps = o["kps"].ctypes.data; io.desc = o["desc"].ctypes.data; io.depth = o["depth"].ctypes.data; io.uright = o["uright"].ctypes.data
             io.cap = self.ctx.cap; io.n_kp = o["n_kp"].ctypes.data
-        check(lib().rgbl_track_sequence(self.ctx.handle, ptr(self.P), C.byref(self.prm), C.byref(chain), C.byref(io)), self.ctx.handle)
+        if self.rgbd_mode:
+            check(lib().rgbl_track_sequence_rgbd(self.ctx.handle, self.depth_scale, self.bf, C.byref(chain), C.byref(io), da, self.W), self.ctx.handle)
+        else:
+            check(lib().rgbl_track_sequence(self.ctx.handle, ptr(self.P), C.byref(self.prm), C.byref(chain), C.byref(io)), self.ctx.handle)
         return o
 
     def h2d_bytes_per_batch(self) -> float:
+        if self.rgbd_mode:
+            return float(self.T * self.W * self.H * 3)
         return float(self.T * self.W * self.H + 16.0 * self.npts.sum() / self.M)
 
     def d2h_bytes_per_batch(self, want_frames: bool) -> float:

@@ -174,6 +174,15 @@ class PlaneSequence:
         """Tcw as (qx, qy, qz, qw, tx, ty, tz): identity rotation, camera centre at x = step_index(t) * dX."""
         return np.array([0, 0, 0, 1, -self.step_index(t) * self.dX, 0, 0], np.float32)
 
+    def depth16(self, t: int, factor: float = 256.0, hole_frac: float = 0.05, noise_m: float = 0.01) -> np.ndarray:
+        """uint16 H x W depth image of frame t as an RGB-D sensor delivers it (CV_16U, metres x factor; KITTI depth PNGs use 256, TUM
+        5000): the plane's depth Z with seeded Gaussian noise, rounded, and a seeded fraction of holes (0 = no measurement)."""
+        rng = np.random.default_rng(self.seed * 104729 + t)
+        d = self.Z + rng.normal(0.0, noise_m, (self.H, self.W))
+        u = np.clip(np.rint(d * factor), 0, 65535).astype(np.uint16)
+        u[rng.random((self.H, self.W)) < hole_frac] = 0
+        return u
+
     def cloud(self, t: int) -> np.ndarray:
         """float32 4 x N planar: a Velodyne-like fan of rays hitting the plane z = Z (camera frame)."""
         rng = np.random.default_rng(self.seed * 7919 + t)
@@ -335,3 +344,37 @@ def colorize(gray: np.ndarray, seed: int = 0, alpha: bool = False) -> np.ndarray
     if alpha:
         chans.append(rng.integers(0, 256, gray.shape, dtype=np.uint8))
     return np.stack(chans, -1)
+
+
+def encode_png16(img: np.ndarray, filters=None, idat_chunk: int = 1 << 16, level: int = 6) -> bytes:
+    """A 16-bit PNG file (gray, or RGB for an H x W x 3 array; non-interlaced) of the uint16 `img`, samples stored big-endian: what an
+    RGB-D sensor's depth PNG holds.  `filters` and `idat_chunk` as for encode_png; the filters work byte-wise with 2 bytes per sample."""
+    import struct
+    import zlib
+    img = np.ascontiguousarray(img, np.uint16)
+    h, w = img.shape[:2]
+    ch = 1 if img.ndim == 2 else img.shape[2]
+    bpp = 2 * ch
+    rows = img.astype(">u2").view(np.uint8).reshape(h, w * bpp).astype(np.int16)
+    if filters is None:
+        filters = np.arange(h) % 5
+    filters = np.asarray(filters, np.int64)
+    a = np.zeros_like(rows); a[:, bpp:] = rows[:, :-bpp]
+    b = np.zeros_like(rows); b[1:] = rows[:-1]
+    c = np.zeros_like(rows); c[1:, bpp:] = rows[:-1, :-bpp]
+    p = a + b - c
+    pa, pb, pc = np.abs(p - a), np.abs(p - b), np.abs(p - c)
+    paeth = np.where((pa <= pb) & (pa <= pc), a, np.where(pb <= pc, b, c))
+    pred = np.stack([np.zeros_like(rows), a, b, (a + b) >> 1, paeth])[filters, np.arange(h)]
+    raw = np.empty((h, w * bpp + 1), np.uint8)
+    raw[:, 0] = filters
+    raw[:, 1:] = ((rows - pred) & 0xff).astype(np.uint8)
+    z = zlib.compress(raw.tobytes(), level)
+
+    def chunk(tag: bytes, data: bytes) -> bytes:
+        return struct.pack(">I", len(data)) + tag + data + struct.pack(">I", zlib.crc32(tag + data) & 0xffffffff)
+
+    out = b"\x89PNG\r\n\x1a\n" + chunk(b"IHDR", struct.pack(">IIBBBBB", w, h, 16, {1: 0, 3: 2}[ch], 0, 0, 0))
+    for i in range(0, len(z), idat_chunk):
+        out += chunk(b"IDAT", z[i:i + idat_chunk])
+    return out + chunk(b"IEND", b"")
