@@ -558,7 +558,8 @@ static int chain_begin(Ctx* c, const rgbl_chain_params& cp_) {
     int* h_i = c->h_chain_i + (size_t)slot * (4 * c->h_chain_cap + 8);
 
     // snapshot on the frame-construction stream (ordered after the batch's kernels, before the next batch's)
-    CU(cudaMemcpyAsync(s_kps, c->d_kps, tot * sizeof(rgbl_keypoint), cudaMemcpyDeviceToDevice, c->st));
+    // mvKeysUn: the chain reads nothing but undistorted keypoints (grid, projections, edges, UnprojectStereo, ring, carried frame)
+    CU(cudaMemcpyAsync(s_kps, c->frames_undistorted ? c->d_kps_un : c->d_kps, tot * sizeof(rgbl_keypoint), cudaMemcpyDeviceToDevice, c->st));
     CU(cudaMemcpyAsync(s_desc, c->d_desc, tot * 32, cudaMemcpyDeviceToDevice, c->st));
     CU(cudaMemcpyAsync(s_depth, c->d_depth, tot * sizeof(float), cudaMemcpyDeviceToDevice, c->st));
     CU(cudaMemcpyAsync(s_uright, c->d_uright, tot * sizeof(float), cudaMemcpyDeviceToDevice, c->st));
@@ -582,6 +583,7 @@ static int chain_begin(Ctx* c, const rgbl_chain_params& cp_) {
     float* c_prev = reinterpret_cast<float*>(t.c_misc) + 9;      // pose of the frame before the carried one (valid: c->carry_prev_valid)
     const bool prev_valid = cont && c->carry_prev_valid;
     int n_launches = 0;
+    const float* bounds = c->frame_bounds;
     // Everything the chain does on the tracking stream.  It is captured ONCE per slot into a CUDA graph and
     // replayed: the launch commands then live in device memory, so the dependent-kernel sequence no longer fetches a command
     // packet from the host over PCIe per launch (which the concurrent H2D uploads of the next batch were slowing down) and
@@ -599,7 +601,7 @@ static int chain_begin(Ctx* c, const rgbl_chain_params& cp_) {
         int* d_nm = t.ch_counts; int* d_ni = t.ch_counts + nF; int* d_nml = t.ch_counts + 2 * nF; int* d_ni1 = t.ch_counts + 3 * nF;
         int* d_ne = t.ch_counts + 4 * nF; int* d_ne2 = d_ne + 1; int* d_flags = d_ne + 2; int* d_ovf = d_ne + 4; int* d_nq = d_ne + 5;
         FrameDev f{};
-        f.min_x = 0.f; f.max_x = (float)c->cfg.width; f.min_y = 0.f; f.max_y = (float)c->cfg.height;      // k1 == 0: image bounds
+        f.min_x = bounds[0]; f.max_x = bounds[1]; f.min_y = bounds[2]; f.max_y = bounds[3];      // ComputeImageBounds of the frames' camera
         f.inv_w = static_cast<float>(kGridCols) / static_cast<float>(f.max_x - f.min_x);
         f.inv_h = static_cast<float>(kGridRows) / static_cast<float>(f.max_y - f.min_y);
         f.n_levels = c->tab.nlevels;
@@ -699,7 +701,7 @@ static int chain_begin(Ctx* c, const rgbl_chain_params& cp_) {
     if (chain_graphs && !chain_timing) {
         Ctx::ChainGraphKey key{};
         key.nF = nF; key.cap = cap; key.mono = mono; key.cont = cont ? 1 : 0; key.K = K; key.prev_valid = prev_valid ? 1 : 0; key.th = th; key.th_local = P.th_local; key.nn_local = P.nn_ratio_local;
-        key.fx = fx; key.fy = fy; key.cx = cx; key.cy = cy; key.bf = bf; key.generation = c->scratch_generation;
+        key.fx = fx; key.fy = fy; key.cx = cx; key.cy = cy; key.bf = bf; std::memcpy(key.bounds, bounds, sizeof(key.bounds)); key.generation = c->scratch_generation;
         if (!c->chain_exec[slot] || std::memcmp(&key, &c->chain_key[slot], sizeof(key)) != 0) {
             if (c->chain_exec[slot]) { cudaGraphExecDestroy(c->chain_exec[slot]); c->chain_exec[slot] = nullptr; }
             prepare_match_kernels();

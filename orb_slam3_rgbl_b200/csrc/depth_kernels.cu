@@ -10,6 +10,7 @@
 //              inverted map t = M - d (zeroed above M-1), take the max over the structuring element,
 //              invert back: the exact float pipeline of Upsample_InverseDilation.
 //   gather   : GetFeatureDepthFromDepthMap (:82-104), and Frame::ComputeStereoFromRGBD (src/Frame.cc:1074-1095) on a uint16 RGB-D plane.
+//   undistort: Frame::UndistortKeyPoints (src/Frame.cc:837-869), mvKeys -> mvKeysUn of a distorted camera, before the gather.
 #include <cfloat>
 
 #include "rgbl_device.cuh"
@@ -141,6 +142,19 @@ __global__ void __launch_bounds__(256) depth_gather_kernel(const T* __restrict__
     }
     depth[o] = dd;
     uright[o] = ur;
+}
+
+// Frame::UndistortKeyPoints (src/Frame.cc:837-869): one keypoint per thread, blockIdx.y = frame.  The output keypoint is the input one with
+// only pt replaced, as the reference copies mvKeys[i] and sets pt.x / pt.y.
+__global__ void __launch_bounds__(256) undistort_keypoints_kernel(UndistortDev cam, const rgbl_keypoint* __restrict__ kps,
+                                                                  const int* __restrict__ n_kp, int cap, rgbl_keypoint* __restrict__ kps_un) {
+    const int frame = blockIdx.y;
+    const int k = blockIdx.x * 256 + threadIdx.x;
+    if (k >= n_kp[frame]) return;
+    const size_t o = (size_t)frame * cap + k;
+    rgbl_keypoint kp = kps[o];
+    undistort_point(cam, kp.x, kp.y, &kp.x, &kp.y);
+    kps_un[o] = kp;
 }
 
 // ---- DepthModule::Upsample_AverageFiltering (src/DepthModule.cc:200-228) ------------------------------------------
@@ -281,6 +295,12 @@ void launch_depth_gather(cudaStream_t st, const float* processed, int W, int H, 
     if (max_n <= 0) return;
     depth_gather_kernel<float><<<dim3((max_n + 255) / 256, n_frames), 256, 0, st>>>(processed, (size_t)W * H, (size_t)W, 1.f, kps, kps_un, n_kp, cap, bf,
                                                                                    depth, uright);
+}
+
+void launch_undistort_keypoints(cudaStream_t st, const UndistortDev& cam, const rgbl_keypoint* kps, const int* n_kp, int cap, int max_n,
+                                rgbl_keypoint* kps_un, int n_frames) {
+    if (max_n <= 0) return;
+    undistort_keypoints_kernel<<<dim3((max_n + 255) / 256, n_frames), 256, 0, st>>>(cam, kps, n_kp, cap, kps_un);
 }
 
 void launch_depth_gather_u16(cudaStream_t st, const uint16_t* plane, size_t frame_elems, size_t pitch_elems, float scale, const rgbl_keypoint* kps,

@@ -184,7 +184,7 @@ struct Ctx {
     int* h_chain_i = nullptr;    // pinned, per slot: n_matches | n_inliers | n_local_matches | n_inliers_first | n_edges x2, flags[2], overflow, n_queries
     size_t h_chain_cap = 0;      // frames per slot
     // the chain of a slot as an instantiated CUDA graph (re-captured when any launch parameter or scratch pointer changes)
-    struct ChainGraphKey { int nF, cap, mono, cont, K, prev_valid; float th, th_local, nn_local, fx, fy, cx, cy, bf; unsigned long long generation; };
+    struct ChainGraphKey { int nF, cap, mono, cont, K, prev_valid; float th, th_local, nn_local, fx, fy, cx, cy, bf, bounds[4]; unsigned long long generation; };
     cudaGraphExec_t chain_exec[2] = {};
     ChainGraphKey chain_key[2] = {};
     const void* chain_timing_ev = nullptr;   // RGBL_CHAIN_TIMING development aid
@@ -194,6 +194,16 @@ struct Ctx {
     static constexpr int kMaxStageSlots = 8;
     struct StageSlot { uint8_t* img = nullptr; float* pts = nullptr; int* n_pts = nullptr; uint16_t* depth = nullptr; std::vector<int> h_n_pts; int n_frames = 0, max_pts = 0; bool rgbd = false; };
     StageSlot stage[kMaxStageSlots];
+
+    // camera model of Frame::UndistortKeyPoints / ComputeImageBounds (rgbl_set_camera_distortion): undistort = (k1 != 0); cam_bounds =
+    // mnMinX, mnMaxX, mnMinY, mnMaxY of that camera ((0, W, 0, H) when k1 == 0)
+    bool undistort = false;
+    UndistortDev cam_un{};
+    float cam_bounds[4] = {};
+    // mvKeysUn and image bounds of the frames in the device buffers, set by each batched frame construction: frames_undistorted ->
+    // d_kps_un ([max_batch][cap_kp]) holds mvKeysUn, else mvKeysUn == mvKeys (d_kps).  The tracking chain reads these.
+    bool frames_undistorted = false;
+    float frame_bounds[4] = {};
 
     int last_frames = 0;         // frames valid in the device buffers
     int resident_frames = 0, resident_max_pts = 0;

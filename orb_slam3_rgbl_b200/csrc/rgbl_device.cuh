@@ -25,6 +25,7 @@ namespace rgbl {
 #define RGBL_DMUL(a, b) __dmul_rn((a), (b))
 #define RGBL_DADD(a, b) __dadd_rn((a), (b))
 #define RGBL_DSUB(a, b) __dsub_rn((a), (b))
+#define RGBL_DDIV(a, b) __ddiv_rn((a), (b))
 #else   // host build of the same header (tests/host_math_harness.cpp); compiled with -ffp-contract=off
 #define RGBL_FMUL(a, b) ((float)(a) * (float)(b))
 #define RGBL_FADD(a, b) ((float)(a) + (float)(b))
@@ -33,7 +34,69 @@ namespace rgbl {
 #define RGBL_DMUL(a, b) ((double)(a) * (double)(b))
 #define RGBL_DADD(a, b) ((double)(a) + (double)(b))
 #define RGBL_DSUB(a, b) ((double)(a) - (double)(b))
+#define RGBL_DDIV(a, b) ((double)(a) / (double)(b))
 #endif
+
+// cv::undistortPoints(src, dst, K, D, noArray(), K) for one CV_32FC2 point, as Frame::UndistortKeyPoints and Frame::ComputeImageBounds
+// call it (src/Frame.cc:837-899): OpenCV's cvUndistortPointsInternal (calib3d/src/undistort.dispatch.cpp) in double precision with
+// its default criterion (MAX_ITER 5) and the operations in its order.  K = P and R = I, so the tilt matrix and R P are exact identities
+// and the final projection is xx = fx x + 0 y + cx, yy = 0 x + fy y + cy, ww = 1 / (0 x + 0 y + 1), each term spelled out so that a
+// non-finite intermediate propagates as OpenCV's does.  Pinned against python-cv2 (tests/test_oracle_undistort.py).
+RGBL_HD void undistort_point(const UndistortDev& m, float px, float py, float* ox, float* oy) {
+    const double* k = m.k;
+    const double u = px, v = py;
+    double x = RGBL_DMUL(RGBL_DSUB(u, m.cx), m.ifx), y = RGBL_DMUL(RGBL_DSUB(v, m.cy), m.ify);
+    const double x0 = x, y0 = y;
+    for (int j = 0; j < 5; ++j) {
+        const double r2 = RGBL_DADD(RGBL_DMUL(x, x), RGBL_DMUL(y, y));
+        const double num = RGBL_DADD(1.0, RGBL_DMUL(RGBL_DADD(RGBL_DMUL(RGBL_DADD(RGBL_DMUL(k[7], r2), k[6]), r2), k[5]), r2));
+        const double den = RGBL_DADD(1.0, RGBL_DMUL(RGBL_DADD(RGBL_DMUL(RGBL_DADD(RGBL_DMUL(k[4], r2), k[1]), r2), k[0]), r2));
+        const double icdist = RGBL_DDIV(num, den);
+        if (icdist < 0) {                    // OpenCV's regression_14583 guard: back to the distorted point, no further iteration
+            x = RGBL_DMUL(RGBL_DSUB(u, m.cx), m.ifx);
+            y = RGBL_DMUL(RGBL_DSUB(v, m.cy), m.ify);
+            break;
+        }
+        const double dx = RGBL_DADD(RGBL_DADD(RGBL_DADD(RGBL_DMUL(RGBL_DMUL(RGBL_DMUL(2.0, k[2]), x), y),
+                                                        RGBL_DMUL(k[3], RGBL_DADD(r2, RGBL_DMUL(RGBL_DMUL(2.0, x), x)))),
+                                              RGBL_DMUL(k[8], r2)),
+                                    RGBL_DMUL(RGBL_DMUL(k[9], r2), r2));
+        const double dy = RGBL_DADD(RGBL_DADD(RGBL_DADD(RGBL_DMUL(k[2], RGBL_DADD(r2, RGBL_DMUL(RGBL_DMUL(2.0, y), y))),
+                                                        RGBL_DMUL(RGBL_DMUL(RGBL_DMUL(2.0, k[3]), x), y)),
+                                              RGBL_DMUL(k[10], r2)),
+                                    RGBL_DMUL(RGBL_DMUL(k[11], r2), r2));
+        x = RGBL_DMUL(RGBL_DSUB(x0, dx), icdist);
+        y = RGBL_DMUL(RGBL_DSUB(y0, dy), icdist);
+    }
+    const double xx = RGBL_DADD(RGBL_DADD(RGBL_DMUL(m.fx, x), RGBL_DMUL(0.0, y)), m.cx);
+    const double yy = RGBL_DADD(RGBL_DADD(RGBL_DMUL(0.0, x), RGBL_DMUL(m.fy, y)), m.cy);
+    const double ww = RGBL_DDIV(1.0, RGBL_DADD(RGBL_DADD(RGBL_DMUL(0.0, x), RGBL_DMUL(0.0, y)), 1.0));
+    *ox = (float)RGBL_DMUL(xx, ww);
+    *oy = (float)RGBL_DMUL(yy, ww);
+}
+
+// the camera of rgbl_set_camera_distortion as cvUndistortPointsInternal converts it: float K and mDistCoef (n_dist 4 or 5) to double
+RGBL_HD UndistortDev make_undistort_dev(float fx, float fy, float cx, float cy, const float* dist, int n_dist) {
+    UndistortDev m{};
+    m.fx = fx; m.fy = fy; m.cx = cx; m.cy = cy;
+    m.ifx = RGBL_DDIV(1.0, m.fx); m.ify = RGBL_DDIV(1.0, m.fy);
+    for (int i = 0; i < 12; ++i) m.k[i] = i < n_dist ? (double)dist[i] : 0.0;
+    return m;
+}
+
+// Frame::ComputeImageBounds (src/Frame.cc:871-899) of a W x H image: k1 != 0 -> the undistorted corners (0,0), (W,0), (0,H), (W,H),
+// mnMinX = min(c0.x, c2.x), mnMaxX = max(c1.x, c3.x), mnMinY = min(c0.y, c1.y), mnMaxY = max(c2.y, c3.y); else (0, W, 0, H).
+RGBL_HD void image_bounds(const UndistortDev& m, float k1, int W, int H, float b[4]) {
+    const float w = (float)W, h = (float)H;
+    if (k1 == 0.f) { b[0] = 0.f; b[1] = w; b[2] = 0.f; b[3] = h; return; }
+    const float cxs[4] = {0.f, w, 0.f, w}, cys[4] = {0.f, 0.f, h, h};
+    float px[4], py[4];
+    for (int i = 0; i < 4; ++i) undistort_point(m, cxs[i], cys[i], &px[i], &py[i]);
+    b[0] = (px[2] < px[0]) ? px[2] : px[0];          // std::min(a, b) = (b < a) ? b : a, std::max(a, b) = (a < b) ? b : a
+    b[1] = (px[1] < px[3]) ? px[3] : px[1];
+    b[2] = (py[1] < py[0]) ? py[1] : py[0];
+    b[3] = (py[2] < py[3]) ? py[3] : py[2];
+}
 
 // cv::fastAtan2 scalar path (SURVEY A.4), degrees in [0, 360).
 RGBL_HD float fast_atan2_deg(float y, float x) {

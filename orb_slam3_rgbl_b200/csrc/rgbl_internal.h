@@ -56,6 +56,13 @@ struct LinCoef {
     int16_t pad;
 };
 
+// Pinhole camera + distortion of Frame::UndistortKeyPoints as cvUndistortPointsInternal holds them: K (float) and mDistCoef converted to
+// double, ifx = 1. / fx, ify = 1. / fy; k = OpenCV's 12 distortion coefficients (k1, k2, p1, p2, k3, then zeros for a 4- or 5-element mDistCoef).
+struct UndistortDev {
+    double fx, fy, cx, cy, ifx, ify;
+    double k[12];
+};
+
 struct OrbTables {
     int nlevels;
     float scale[RGBL_MAX_LEVELS], inv_scale[RGBL_MAX_LEVELS];

@@ -95,6 +95,10 @@ void launch_depth_nn_pixel(cudaStream_t st, const float* raw, int W, int H, cons
 void launch_depth_gather(cudaStream_t st, const float* processed, int W, int H, const rgbl_keypoint* kps,
                          const rgbl_keypoint* kps_un, const int* n_kp, int cap, int max_n, float bf, float* depth,
                          float* uright, int n_frames);
+// Frame::UndistortKeyPoints (src/Frame.cc:837-869) of n_frames keypoint lists ([n_frames][cap], n_kp[frame] valid): kps_un = kps with pt
+// replaced by the undistorted point (undistort_point, rgbl_device.cuh)
+void launch_undistort_keypoints(cudaStream_t st, const UndistortDev& cam, const rgbl_keypoint* kps, const int* n_kp, int cap, int max_n,
+                                rgbl_keypoint* kps_un, int n_frames);
 // the same gather on uint16 RGB-D depth planes, metric depth = (float)sample * scale (Tracking::mDepthMapFactor)
 void launch_depth_gather_u16(cudaStream_t st, const uint16_t* plane, size_t frame_elems, size_t pitch_elems, float scale, const rgbl_keypoint* kps,
                              const rgbl_keypoint* kps_un, const int* n_kp, int cap, int max_n, float bf, float* depth, float* uright, int n_frames);

@@ -50,6 +50,15 @@ class Context:
         out["_host_quadtree_ms"] = hq.value
         return out
 
+    def set_camera_distortion(self, fx, fy, cx, cy, dist) -> np.ndarray:
+        """Camera model of Frame::UndistortKeyPoints / ComputeImageBounds for the batched frame constructions and tracking chains of this
+        context (rgbl_set_camera_distortion): K = (fx, fy, cx, cy), dist = mDistCoef (k1, k2, p1, p2[, k3]); k1 == 0 -> mvKeysUn = mvKeys.
+        -> the image bounds (mnMinX, mnMaxX, mnMinY, mnMaxY)."""
+        d = np.ascontiguousarray(dist, np.float32).reshape(-1)
+        b = np.empty(4, np.float32)
+        check(lib().rgbl_set_camera_distortion(self.handle, fx, fy, cx, cy, ptr(d), len(d), ptr(b)), self.handle)
+        return b
+
     def set_host_quadtree(self, on: bool):
         check(lib().rgbl_set_host_quadtree(self.handle, int(on)), self.handle)
 
@@ -379,17 +388,19 @@ def frame_rgbl_batch(ctx: Context, images, clouds, P, depth_params: DepthParams)
 
 
 class FrameView:
-    """The members of ORB_SLAM3::Frame the tracking matchers read (Nleft == -1 frames), see rgbl_frame_view."""
+    """The members of ORB_SLAM3::Frame the tracking matchers read (Nleft == -1 frames), see rgbl_frame_view.  bounds = (mnMinX, mnMaxX,
+    mnMinY, mnMaxY) of a distorted camera (Context.set_camera_distortion); None: (0, width, 0, height)."""
 
-    def __init__(self, keys_un, uright, desc, width, height, scale_factors, fx, fy, cx, cy, bf):
+    def __init__(self, keys_un, uright, desc, width, height, scale_factors, fx, fy, cx, cy, bf, bounds=None):
         self.keys_un = np.ascontiguousarray(keys_un, KP_DTYPE)
         self.uright = np.ascontiguousarray(uright, np.float32)
         self.desc = np.ascontiguousarray(desc, np.uint8)
         self.scale_factors = np.ascontiguousarray(scale_factors, np.float32)
         self.n = len(self.keys_un)
         log_sf = float(np.float32(np.log(np.float32(self.scale_factors[1])))) if len(self.scale_factors) > 1 else 1.0
+        b = (0.0, float(width), 0.0, float(height)) if bounds is None else tuple(float(v) for v in bounds)
         self.c = L.FrameViewC(self.n, self.keys_un.ctypes.data, self.uright.ctypes.data, self.desc.ctypes.data,
-                              0.0, float(width), 0.0, float(height), len(self.scale_factors), self.scale_factors.ctypes.data,
+                              *b, len(self.scale_factors), self.scale_factors.ctypes.data,
                               fx, fy, cx, cy, bf, log_sf)
 
 
@@ -626,6 +637,13 @@ class RgblBatch:
         check(lib().rgbl_resident_download(c.handle, ptr(self.kps), ptr(self.desc), ptr(self.depth), ptr(self.uright), self.cap, ptr(self.n)), c.handle)
         return [(self.kps[f, :self.n[f]], self.desc[f, :self.n[f]], self.depth[f, :self.n[f]], self.uright[f, :self.n[f]]) for f in range(self.nF)]
 
+    def download_keys_un(self):
+        """mvKeysUn of the frames of the last batched call (rgbl_resident_download_keys_un): list of keypoint arrays, one per frame"""
+        c = self.ctx
+        kun = np.empty((self.nF, self.cap), KP_DTYPE); n = np.zeros(self.nF, np.int32)
+        check(lib().rgbl_resident_download_keys_un(c.handle, ptr(kun), self.cap, ptr(n)), c.handle)
+        return [kun[f, :n[f]].copy() for f in range(self.nF)]
+
 
 class RgbdBatch:
     """Host buffers of one batch of RGB-D frames (gray image + CV_16U depth image each) for the resident RGB-D API: the RGB-D Frame
@@ -671,6 +689,7 @@ class RgbdBatch:
         return self.n
 
     download = RgblBatch.download
+    download_keys_un = RgblBatch.download_keys_un
     track_begin2 = RgblBatch.track_begin2
     track_end2 = RgblBatch.track_end2
 

@@ -21,6 +21,12 @@ KITTI_TR = np.array([[4.276802385584e-04, -9.999672484946e-01, -8.084491683471e-
                      [-7.210626507497e-03, 8.081198471645e-03, -9.999413164504e-01, -5.403984729748e-02],
                      [9.999738645903e-01, 4.859485810390e-04, -7.206933692422e-03, -2.921968648686e-01]], np.float64)
 LIDAR_MIN_DIST, LIDAR_MAX_DIST = 5.0, 200.0
+# ORB-SLAM3's Examples/RGB-D/TUM1.yaml (TUM RGB-D fr1 sequences): a 640 x 480 camera with non-zero distortion
+TUM_W, TUM_H = 640, 480
+TUM1_FX, TUM1_FY, TUM1_CX, TUM1_CY = 517.306408, 516.469215, 318.643040, 255.313989
+TUM1_DIST = np.array([0.262383, -0.953104, -0.005358, 0.002628, 1.163314], np.float32)      # k1, k2, p1, p2, k3
+TUM1_BF = 40.0
+TUM_DEPTH_FACTOR = 5000.0
 
 
 def camera_matrix(fx=KITTI_FX, fy=KITTI_FY, cx=KITTI_CX, cy=KITTI_CY) -> np.ndarray:
@@ -147,12 +153,21 @@ class PlaneSequence:
     sequence of any length stays on the texture and consecutive passes over the same `loop` frames form one continuous trajectory."""
 
     def __init__(self, seed: int, n_frames: int, shift_px: int = 7, Z: float = 20.0, W: int = KITTI_W, H: int = KITTI_H,
-                 n_rings: int = 64, n_azimuth: int = 1875, loop: int = 0, cam=None):
+                 n_rings: int = 64, n_azimuth: int = 1875, loop: int = 0, cam=None, dist=None):
+        """dist: the camera's distortion (k1, k2, p1, p2[, k3], OpenCV's model); image(t) is then the distorted view of the scene."""
         self.seed, self.n_frames, self.shift, self.Z, self.W, self.H = seed, n_frames, shift_px, Z, W, H
         self.cam = tuple(cam) if cam is not None else (KITTI_FX, KITTI_FY, KITTI_CX, KITTI_CY, KITTI_BF)      # (fx, fy, cx, cy, bf)
         self.loop = loop
         span = (loop // 2 + 1) if loop > 0 else n_frames
-        self.texture = make_image(seed, W + shift_px * span + 8, H)
+        self.dist = None if dist is None else np.asarray(dist, np.float64).reshape(-1)
+        if self.dist is None:
+            self.texture = make_image(seed, W + shift_px * span + 8, H)
+        else:
+            # where each pixel of the distorted image sees the undistorted (pinhole) image, and a texture margin that covers it
+            self.map_x, self.map_y = undistorted_pixel_map(W, H, self.cam[:4], self.dist)
+            self.margin = int(np.ceil(max(-self.map_x.min(), -self.map_y.min(), self.map_x.max() - (W - 1), self.map_y.max() - (H - 1), 0.0))) + 2
+            m = self.margin
+            self.texture = make_image(seed, W + shift_px * span + 8 + 2 * m, H + 2 * m)
         self.dX = shift_px * Z / self.cam[0]         # camera translation per frame (metres along +x)
         self.n_rings, self.n_az = n_rings, n_azimuth
         Tr4 = np.eye(4); Tr4[:3] = KITTI_TR
@@ -168,7 +183,16 @@ class PlaneSequence:
 
     def image(self, t: int) -> np.ndarray:
         s = self.step_index(t)
-        return np.ascontiguousarray(self.texture[:, s * self.shift: s * self.shift + self.W])
+        if self.dist is None:
+            return np.ascontiguousarray(self.texture[:, s * self.shift: s * self.shift + self.W])
+        # the pinhole view of frame t is the texture crop at (s * shift + margin, margin); sample it bilinearly where the lens maps each pixel
+        tex = self.texture.astype(np.float64)
+        xs = self.map_x + (s * self.shift + self.margin); ys = self.map_y + self.margin
+        x0 = np.floor(xs).astype(np.int64); y0 = np.floor(ys).astype(np.int64)
+        fx = xs - x0; fy = ys - y0
+        top = tex[y0, x0] * (1 - fx) + tex[y0, x0 + 1] * fx
+        bot = tex[y0 + 1, x0] * (1 - fx) + tex[y0 + 1, x0 + 1] * fx
+        return np.ascontiguousarray(np.clip(np.rint(top * (1 - fy) + bot * fy), 0, 255).astype(np.uint8))
 
     def pose(self, t: int) -> np.ndarray:
         """Tcw as (qx, qy, qz, qw, tx, ty, tz): identity rotation, camera centre at x = step_index(t) * dX."""
@@ -195,6 +219,33 @@ class PlaneSequence:
         velo = self.Tr_inv @ cam
         pts = np.stack([velo[0], velo[1], velo[2], np.ones(X.size)]).astype(np.float32)
         return np.ascontiguousarray(pts)
+
+
+def distort_normalized(x, y, dist):
+    """OpenCV's distortion model (k1, k2, p1, p2[, k3]) on normalised camera coordinates -> distorted normalised coordinates"""
+    k1, k2, p1, p2 = dist[:4]
+    k3 = dist[4] if len(dist) > 4 else 0.0
+    r2 = x * x + y * y
+    radial = 1 + r2 * (k1 + r2 * (k2 + r2 * k3))
+    return x * radial + 2 * p1 * x * y + p2 * (r2 + 2 * x * x), y * radial + p1 * (r2 + 2 * y * y) + 2 * p2 * x * y
+
+
+def undistorted_pixel_map(W: int, H: int, cam, dist, iterations: int = 100):
+    """For every pixel (u, v) of a W x H distorted image: the pixel of the undistorted (pinhole) image it shows, (map_x, map_y) float64 H x W.
+    The inverse of the distortion model by fixed-point iteration, run until it has converged (checked by distorting the result again)."""
+    fx, fy, cx, cy = (float(v) for v in cam)
+    dist = np.asarray(dist, np.float64)
+    v, u = np.mgrid[0:H, 0:W].astype(np.float64)
+    xd, yd = (u - cx) / fx, (v - cy) / fy
+    x, y = xd.copy(), yd.copy()
+    for _ in range(iterations):
+        dx, dy = distort_normalized(x, y, dist)
+        x, y = x + (xd - dx), y + (yd - dy)
+    dx, dy = distort_normalized(x, y, dist)
+    err = max(np.abs(dx - xd).max() * fx, np.abs(dy - yd).max() * fy)
+    if not err < 1e-6:
+        raise ValueError(f"the inverse distortion did not converge ({err} px)")
+    return x * fx + cx, y * fy + cy
 
 
 def stereo_disparity_field(W: int = KITTI_W, H: int = KITTI_H) -> np.ndarray:
