@@ -19,53 +19,17 @@ namespace rgbl {
 
 static thread_local std::string g_create_error;
 
-template <class T>
-static cudaError_t dmalloc(T** p, size_t n) { return cudaMalloc((void**)p, n * sizeof(T)); }
-template <class T>
-static cudaError_t hmalloc(T** p, size_t n) { return cudaMallocHost((void**)p, n * sizeof(T)); }
-
+// The members of Ctx own every resource of the context; their destructors release them once no stream has work left.
 static void release(Ctx* c) {
     if (!c) return;
     cudaSetDevice(c->cfg.device);
-    void* dev[] = {c->d_levels, c->d_cells, c->d_coefs, c->d_pyr, c->d_blur, c->d_slots, c->d_counts, c->d_cell_off,
-                   c->d_level_cnt, c->d_frame_total, c->d_overflow, c->d_dense, c->d_sel, c->d_n_sel, c->d_kps,
-                   c->d_kps_un, c->d_desc, c->d_pts, c->d_n_pts, c->d_idx_map, c->d_raw, c->d_processed, c->d_depth,
-                   c->d_uright, c->d_scratch, c->d_kps_in, c->d_n_kp_in, c->qt_scr.perm_a, c->qt_scr.perm_b, c->qt_scr.node_a,
-                   c->qt_scr.node_b, c->qt_scr.scan, c->qt_scr.quad, c->d_sel_lvl, c->d_n_sel_lvl, c->d_lvl_region};
-    for (void* p : dev) if (p) cudaFree(p);
-    c->trk.release();
-    for (cudaEvent_t& e : c->chain_tev) if (e) cudaEventDestroy(e);
-    void* host[] = {c->h_chain_ovf, c->h_scalars, c->h_level_cnt, c->h_frame_total, c->h_overflow, c->h_n_sel, c->h_n_pts, c->h_dense, c->h_sel};
-    for (void* p : host) if (p) cudaFreeHost(p);
-    for (int i = 0; i < kNumStages; ++i) { if (c->ev_b[i]) cudaEventDestroy(c->ev_b[i]); if (c->ev_e[i]) cudaEventDestroy(c->ev_e[i]); }
-    if (c->ev_t0) cudaEventDestroy(c->ev_t0);
-    if (c->ev_t1) cudaEventDestroy(c->ev_t1);
-    if (c->ev_pyr) cudaEventDestroy(c->ev_pyr);
-    if (c->ev_blur) cudaEventDestroy(c->ev_blur);
-    if (c->d_pts_raw) cudaFree(c->d_pts_raw);
-    if (c->d_depth16) cudaFree(c->d_depth16);
-    if (c->d_png_raw) cudaFree(c->d_png_raw);
-    if (c->d_png_band) cudaFree(c->d_png_band);
-    if (c->d_png_status) cudaFree(c->d_png_status);
-    if (c->h_png_raw) cudaFreeHost(c->h_png_raw);
-    if (c->h_png_status) cudaFreeHost(c->h_png_status);
-    if (c->d_strips) cudaFree(c->d_strips);
-    if (c->map_arena) cudaFree(c->map_arena);
-    if (c->st_trk) { cudaStreamSynchronize(c->st_trk); cudaStreamDestroy(c->st_trk); }
-    if (c->ev_snap) cudaEventDestroy(c->ev_snap);
-    for (int i = 0; i < 2; ++i) {
-        if (c->chain_exec[i]) cudaGraphExecDestroy(c->chain_exec[i]);
-        if (c->ev_chain_b[i]) cudaEventDestroy(c->ev_chain_b[i]);
-        if (c->ev_chain_e[i]) cudaEventDestroy(c->ev_chain_e[i]);
-        if (c->ev_chain_done[i]) cudaEventDestroy(c->ev_chain_done[i]);
-    }
-    for (Ctx::StageSlot& sl : c->stage) { if (sl.img) cudaFree(sl.img); if (sl.pts) cudaFree(sl.pts); if (sl.n_pts) cudaFree(sl.n_pts); if (sl.depth) cudaFree(sl.depth); }
-    if (c->h_chain_f) cudaFreeHost(c->h_chain_f);
-    if (c->h_chain_i) cudaFreeHost(c->h_chain_i);
-    if (c->st) cudaStreamDestroy(c->st);
-    if (c->st_aux) cudaStreamDestroy(c->st_aux);
+    for (cudaStream_t s : {c->st.get(), c->st_aux.get(), c->st_trk.get()}) if (s) cudaStreamSynchronize(s);      // st_trk: a chain may be in flight
     delete c;
 }
+
+// a lazily allocated array: allocated by the first call that needs it (and retried by the next call if that allocation failed)
+template <class A>
+static bool ensure(A& a, size_t n) { return a || a.alloc(n) == cudaSuccess; }
 
 static int create(const rgbl_config* cfg, Ctx** out) {
     Ctx* c = new Ctx();
@@ -94,31 +58,31 @@ static int create(const rgbl_config* cfg, Ctx** out) {
     const int nl = c->tab.nlevels;
     const size_t WH = (size_t)cfg->width * cfg->height;
 #define CUF(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { c->err = std::string(#call) + ": " + cudaGetErrorString(e_); return fail(RGBL_E_CUDA); } } while (0)
-    CUF(cudaStreamCreateWithFlags(&c->st, cudaStreamNonBlocking));
-    CUF(cudaStreamCreateWithFlags(&c->st_aux, cudaStreamNonBlocking));
-    CUF(cudaEventCreate(&c->ev_t0));
-    CUF(cudaEventCreate(&c->ev_t1));
-    CUF(cudaEventCreateWithFlags(&c->ev_pyr, cudaEventDisableTiming));
-    CUF(cudaEventCreateWithFlags(&c->ev_blur, cudaEventDisableTiming));
-    for (int i = 0; i < kNumStages; ++i) { CUF(cudaEventCreate(&c->ev_b[i])); CUF(cudaEventCreate(&c->ev_e[i])); }
-    CUF(dmalloc(&c->d_levels, nl));
-    CUF(dmalloc(&c->d_cells, c->cells.size()));
-    CUF(dmalloc(&c->d_coefs, std::max<size_t>(c->coefs.size(), 1)));
+    CUF(c->st.create());
+    CUF(c->st_aux.create());
+    CUF(c->ev_t0.create());
+    CUF(c->ev_t1.create());
+    CUF(c->ev_pyr.create(cudaEventDisableTiming));
+    CUF(c->ev_blur.create(cudaEventDisableTiming));
+    for (int i = 0; i < kNumStages; ++i) { CUF(c->ev_b[i].create()); CUF(c->ev_e[i].create()); }
+    CUF(c->d_levels.alloc(nl));
+    CUF(c->d_cells.alloc(c->cells.size()));
+    CUF(c->d_coefs.alloc(std::max<size_t>(c->coefs.size(), 1)));
     CUF(cudaMemcpy(c->d_levels, c->levels.data(), nl * sizeof(LevelGeom), cudaMemcpyHostToDevice));
     CUF(cudaMemcpy(c->d_cells, c->cells.data(), c->cells.size() * sizeof(CellInfo), cudaMemcpyHostToDevice));
     if (!c->coefs.empty()) CUF(cudaMemcpy(c->d_coefs, c->coefs.data(), c->coefs.size() * sizeof(LinCoef), cudaMemcpyHostToDevice));
-    CUF(dmalloc(&c->d_pyr, c->frame_bytes * B));
-    CUF(dmalloc(&c->d_blur, c->frame_bytes * B));
+    CUF(c->d_pyr.alloc(c->frame_bytes * B));
+    CUF(c->d_blur.alloc(c->frame_bytes * B));
     CUF(cudaMemset(c->d_pyr, 0, c->frame_bytes * B));
     CUF(cudaMemset(c->d_blur, 0, c->frame_bytes * B));
-    CUF(dmalloc(&c->d_slots, (size_t)B * c->n_cells * kCellCap));
-    CUF(dmalloc(&c->d_counts, (size_t)B * c->n_cells));
-    CUF(dmalloc(&c->d_cell_off, (size_t)B * c->n_cells));
-    CUF(dmalloc(&c->d_level_cnt, (size_t)B * RGBL_MAX_LEVELS));
-    CUF(dmalloc(&c->d_frame_total, (size_t)B));
-    CUF(dmalloc(&c->d_overflow, 4));
+    CUF(c->d_slots.alloc((size_t)B * c->n_cells * kCellCap));
+    CUF(c->d_counts.alloc((size_t)B * c->n_cells));
+    CUF(c->d_cell_off.alloc((size_t)B * c->n_cells));
+    CUF(c->d_level_cnt.alloc((size_t)B * RGBL_MAX_LEVELS));
+    CUF(c->d_frame_total.alloc((size_t)B));
+    CUF(c->d_overflow.alloc(4));
     CUF(cudaMemset(c->d_overflow, 0, 4 * sizeof(int)));
-    CUF(dmalloc(&c->d_dense, (size_t)c->dense_cap));
+    CUF(c->d_dense.alloc((size_t)c->dense_cap));
     {   // device quad-tree: per-level survivor regions + scratch mirroring the dense candidate buffer
         std::vector<int> region(nl + 1, 0);
         bool fits = true;
@@ -134,14 +98,15 @@ static int create(const rgbl_config* cfg, Ctx** out) {
         const char* env = getenv("RGBL_HOST_QUADTREE");
         c->qt_device_ok = fits && dev_smem >= quadtree_smem_bytes();
         c->device_quadtree = c->qt_device_ok && !(env && env[0] == '1');
-        CUF(dmalloc(&c->d_lvl_region, nl + 1));
+        CUF(c->d_lvl_region.alloc(nl + 1));
         CUF(cudaMemcpy(c->d_lvl_region, region.data(), (nl + 1) * sizeof(int), cudaMemcpyHostToDevice));
-        CUF(dmalloc(&c->d_sel_lvl, (size_t)B * c->cap_kp));
-        CUF(dmalloc(&c->d_n_sel_lvl, (size_t)B * RGBL_MAX_LEVELS));
-        CUF(dmalloc(&c->qt_scr.perm_a, (size_t)c->dense_cap)); CUF(dmalloc(&c->qt_scr.perm_b, (size_t)c->dense_cap));
-        CUF(dmalloc(&c->qt_scr.node_a, (size_t)c->dense_cap)); CUF(dmalloc(&c->qt_scr.node_b, (size_t)c->dense_cap));
-        CUF(dmalloc(&c->qt_scr.scan, (size_t)c->dense_cap + (size_t)B * nl + 8));
-        CUF(dmalloc(&c->qt_scr.quad, (size_t)c->dense_cap));
+        CUF(c->d_sel_lvl.alloc((size_t)B * c->cap_kp));
+        CUF(c->d_n_sel_lvl.alloc((size_t)B * RGBL_MAX_LEVELS));
+        CUF(c->qt_perm_a.alloc(c->dense_cap)); CUF(c->qt_perm_b.alloc(c->dense_cap));
+        CUF(c->qt_node_a.alloc(c->dense_cap)); CUF(c->qt_node_b.alloc(c->dense_cap));
+        CUF(c->qt_scan.alloc((size_t)c->dense_cap + (size_t)B * nl + 8));
+        CUF(c->qt_quad.alloc(c->dense_cap));
+        c->qt_scr = QtScratchDev{c->qt_perm_a, c->qt_perm_b, c->qt_node_a, c->qt_node_b, c->qt_scan, c->qt_quad};
     }
     {   // strip FAST, staged describe, dilation with the empty-tile shortcut: bit-exact twins of the round-1 kernels and
         // faster, hence the defaults; RGBL_<NAME>=0 selects the round-1 kernel for A/B runs
@@ -154,45 +119,45 @@ static int create(const rgbl_config* cfg, Ctx** out) {
         const char* env = getenv("RGBL_FAST_STRIPS");
         if (!(env && env[0] == '0')) {
             build_fast_strips(c->cells, 8, 264, c->strips, c->strip_rows_cap, c->strip_list_cap);
-            CUF(dmalloc(&c->d_strips, c->strips.size()));
+            CUF(c->d_strips.alloc(c->strips.size()));
             CUF(cudaMemcpy(c->d_strips, c->strips.data(), c->strips.size() * sizeof(StripInfo), cudaMemcpyHostToDevice));
             c->fast_strips = true;
         }
     }
-    CUF(dmalloc(&c->d_sel, (size_t)B * c->cap_kp));
-    CUF(dmalloc(&c->d_n_sel, (size_t)B));
-    CUF(dmalloc(&c->d_kps, (size_t)B * c->cap_kp));
-    CUF(dmalloc(&c->d_kps_un, (size_t)B * c->cap_kp));      // mvKeysUn of batched frame construction with a distorted camera
-    CUF(dmalloc(&c->d_kps_in, 2 * (size_t)c->cap_kp));      // the two-call forms' mvKeys | mvKeysUn uploads
+    CUF(c->d_sel.alloc((size_t)B * c->cap_kp));
+    CUF(c->d_n_sel.alloc((size_t)B));
+    CUF(c->d_kps.alloc((size_t)B * c->cap_kp));
+    CUF(c->d_kps_un.alloc((size_t)B * c->cap_kp));      // mvKeysUn of batched frame construction with a distorted camera
+    CUF(c->d_kps_in.alloc(2 * (size_t)c->cap_kp));      // the two-call forms' mvKeys | mvKeysUn uploads
     c->cam_bounds[0] = c->frame_bounds[0] = 0.f; c->cam_bounds[1] = c->frame_bounds[1] = (float)cfg->width;
     c->cam_bounds[2] = c->frame_bounds[2] = 0.f; c->cam_bounds[3] = c->frame_bounds[3] = (float)cfg->height;
-    CUF(dmalloc(&c->d_n_kp_in, 1));
-    CUF(dmalloc(&c->d_desc, (size_t)B * c->cap_kp * 32));
-    CUF(dmalloc(&c->d_depth, (size_t)B * c->cap_kp));
-    CUF(dmalloc(&c->d_uright, (size_t)B * c->cap_kp));
+    CUF(c->d_n_kp_in.alloc(1));
+    CUF(c->d_desc.alloc((size_t)B * c->cap_kp * 32));
+    CUF(c->d_depth.alloc((size_t)B * c->cap_kp));
+    CUF(c->d_uright.alloc((size_t)B * c->cap_kp));
     if (cfg->max_points > 0) {
-        CUF(dmalloc(&c->d_pts, (size_t)B * 4 * cfg->max_points));
-        CUF(dmalloc(&c->d_n_pts, (size_t)B));
-        CUF(dmalloc(&c->d_idx_map, (size_t)B * WH));
+        CUF(c->d_pts.alloc((size_t)B * 4 * cfg->max_points));
+        CUF(c->d_n_pts.alloc((size_t)B));
+        CUF(c->d_idx_map.alloc((size_t)B * WH));
         CUF(cudaMemset(c->d_idx_map, 0, (size_t)B * WH * sizeof(uint32_t)));
-        CUF(dmalloc(&c->d_raw, (size_t)B * WH));
-        CUF(dmalloc(&c->d_processed, (size_t)B * WH));
-        CUF(hmalloc(&c->h_n_pts, (size_t)B));
+        CUF(c->d_raw.alloc((size_t)B * WH));
+        CUF(c->d_processed.alloc((size_t)B * WH));
+        CUF(c->h_n_pts.alloc((size_t)B));
     }
     c->scratch_bytes = (size_t)(cfg->width + 2 * kEdgeThreshold + 64) * (cfg->height + 2 * kEdgeThreshold);
-    CUF(dmalloc(&c->d_scratch, c->scratch_bytes));
-    CUF(hmalloc(&c->h_scalars, 16));
-    CUF(hmalloc(&c->h_chain_ovf, 4));
+    CUF(c->d_scratch.alloc(c->scratch_bytes));
+    CUF(c->h_scalars.alloc(16));
+    CUF(c->h_chain_ovf.alloc(4));
     for (int i = 0; i < 4; ++i) c->h_chain_ovf[i] = 0;
     c->chain_timing_on = std::getenv("RGBL_CHAIN_TIMING") != nullptr;
     c->chain_graphs_on = !(std::getenv("RGBL_CHAIN_GRAPH") && std::getenv("RGBL_CHAIN_GRAPH")[0] == '0');
     c->chain_pdl_on = !(std::getenv("RGBL_CHAIN_PDL") && std::getenv("RGBL_CHAIN_PDL")[0] == '0');
-    CUF(hmalloc(&c->h_level_cnt, (size_t)B * RGBL_MAX_LEVELS));
-    CUF(hmalloc(&c->h_frame_total, (size_t)B));
-    CUF(hmalloc(&c->h_overflow, 4));
-    CUF(hmalloc(&c->h_n_sel, (size_t)B));
-    CUF(hmalloc(&c->h_dense, (size_t)c->dense_cap));
-    CUF(hmalloc(&c->h_sel, (size_t)B * c->cap_kp));
+    CUF(c->h_level_cnt.alloc((size_t)B * RGBL_MAX_LEVELS));
+    CUF(c->h_frame_total.alloc((size_t)B));
+    CUF(c->h_overflow.alloc(4));
+    CUF(c->h_n_sel.alloc((size_t)B));
+    CUF(c->h_dense.alloc((size_t)c->dense_cap));
+    CUF(c->h_sel.alloc((size_t)B * c->cap_kp));
 #undef CUF
     *out = c;
     return RGBL_OK;
@@ -713,11 +678,7 @@ static int check_batch_args(Ctx* c, int n_frames, int width, int height, int str
 static int upload_rgbl(Ctx* c, int n_frames, const uint8_t* const* gray, int stride, const float* const* pts4xn, const int* n_pts, int* max_pts_out,
                        int layout = 0) {
     if (!c->d_pts) { c->err = "context was created with max_points == 0"; return RGBL_E_INVALID; }
-    if (layout == 1 && !c->d_pts_raw) {
-        if (cudaMalloc((void**)&c->d_pts_raw, (size_t)c->cfg.max_batch * 4 * c->cfg.max_points * sizeof(float)) != cudaSuccess) {
-            cudaGetLastError(); c->err = "cudaMalloc failed (raw point records)"; return RGBL_E_CUDA;
-        }
-    }
+    if (layout == 1 && !ensure(c->d_pts_raw, (size_t)c->cfg.max_batch * 4 * c->cfg.max_points)) { c->err = "device allocation failed (raw point records)"; return RGBL_E_CUDA; }
     int max_pts = 0;
     for (int f = 0; f < n_frames; ++f) {
         if (gray && !gray[f]) { c->err = "empty image"; return RGBL_E_EMPTY; }
@@ -742,16 +703,15 @@ static int upload_rgbl(Ctx* c, int n_frames, const uint8_t* const* gray, int str
 // cv::imread(PNG, IMREAD_UNCHANGED) + cvtColor to gray (Examples/RGB-L/rgbl_kitti.cc:87, src/Tracking.cc:1567-1580) into level 0 of the
 // frame slots 0..n_frames-1: host inflate into pinned staging, H2D of the filtered scanlines, reconstruction + gray on the device.
 static int ensure_png_staging(Ctx* c) {
-    const int w = c->cfg.width, h = c->cfg.height;
-    if (!c->d_png_raw) {
-        c->png_raw_stride = (((size_t)w * 4 + 1) * h + 255) & ~(size_t)255;
-        const size_t total = c->png_raw_stride * c->cfg.max_batch;
-        if (cudaMalloc((void**)&c->d_png_raw, total) != cudaSuccess || cudaMallocHost((void**)&c->h_png_raw, total) != cudaSuccess ||
-            cudaMalloc((void**)&c->d_png_band, (size_t)c->cfg.max_batch * w * sizeof(uint32_t)) != cudaSuccess ||
-            cudaMalloc((void**)&c->d_png_status, sizeof(int)) != cudaSuccess || cudaMallocHost((void**)&c->h_png_status, sizeof(int)) != cudaSuccess) {
-            cudaGetLastError(); c->err = "allocation of the PNG staging buffers failed"; return RGBL_E_CUDA;
-        }
-        CU(cudaMemset(c->d_png_status, 0, sizeof(int)));
+    const size_t w = c->cfg.width, B = c->cfg.max_batch;
+    c->png_raw_stride = ((w * 4 + 1) * c->cfg.height + 255) & ~(size_t)255;
+    if (!c->d_png_status) {          // allocated and zeroed, or not at all
+        if (c->d_png_status.alloc(1) != cudaSuccess) { c->err = "allocation of the PNG staging buffers failed"; return RGBL_E_CUDA; }
+        if (cudaMemset(c->d_png_status, 0, sizeof(int)) != cudaSuccess) { c->d_png_status.reset(); c->err = "cudaMemset failed (PNG status word)"; return RGBL_E_CUDA; }
+    }
+    if (!ensure(c->d_png_raw, c->png_raw_stride * B) || !ensure(c->h_png_raw, c->png_raw_stride * B) || !ensure(c->d_png_band, B * w) ||
+        !ensure(c->h_png_status, 1)) {
+        c->err = "allocation of the PNG staging buffers failed"; return RGBL_E_CUDA;
     }
     return RGBL_OK;
 }
@@ -793,12 +753,8 @@ static int decode_png_to_level0(Ctx* c, int n_frames, const uint8_t* const* png,
 static size_t depth16_frame_elems(const Ctx* c) { return c->depth16_pitch * c->cfg.height; }
 
 static int ensure_depth16(Ctx* c) {
-    if (c->d_depth16) return RGBL_OK;
-    const size_t pitch = ((size_t)c->cfg.width * sizeof(uint16_t) + 63) / 64 * 32;
-    if (cudaMalloc((void**)&c->d_depth16, pitch * c->cfg.height * c->cfg.max_batch * sizeof(uint16_t)) != cudaSuccess) {
-        cudaGetLastError(); c->d_depth16 = nullptr; c->err = "cudaMalloc failed (RGB-D depth planes)"; return RGBL_E_CUDA;
-    }
-    c->depth16_pitch = pitch;
+    c->depth16_pitch = ((size_t)c->cfg.width * sizeof(uint16_t) + 63) / 64 * 32;
+    if (!ensure(c->d_depth16, c->depth16_pitch * c->cfg.height * c->cfg.max_batch)) { c->err = "device allocation failed (RGB-D depth planes)"; return RGBL_E_CUDA; }
     return RGBL_OK;
 }
 
@@ -976,14 +932,9 @@ int rgbl_resident_process(rgbl_ctx* ctx, const float P[12], const rgbl_depth_par
 // device buffers of a stage slot (allocated on first use; a slot can hold RGB-L and later RGB-D batches or the reverse)
 static int stage_slot_alloc(Ctx* c, Ctx::StageSlot& sl, bool rgbd) {
     const size_t img_bytes = (size_t)c->levels[0].pitch * c->cfg.height, B = c->cfg.max_batch;
-    bool ok = sl.img || cudaMalloc((void**)&sl.img, B * img_bytes) == cudaSuccess;
-    if (rgbd) {
-        ok = ok && (sl.depth || cudaMalloc((void**)&sl.depth, B * depth16_frame_elems(c) * sizeof(uint16_t)) == cudaSuccess);
-    } else {
-        ok = ok && (sl.pts || cudaMalloc((void**)&sl.pts, B * 4 * c->cfg.max_points * sizeof(float)) == cudaSuccess);
-        ok = ok && (sl.n_pts || cudaMalloc((void**)&sl.n_pts, B * sizeof(int)) == cudaSuccess);
-    }
-    if (!ok) { cudaGetLastError(); c->err = "cudaMalloc failed (stage slot)"; return RGBL_E_CUDA; }
+    const bool ok = ensure(sl.img, B * img_bytes) &&
+                    (rgbd ? ensure(sl.depth, B * depth16_frame_elems(c)) : ensure(sl.pts, B * 4 * c->cfg.max_points) && ensure(sl.n_pts, B));
+    if (!ok) { c->err = "device allocation failed (stage slot)"; return RGBL_E_CUDA; }
     return RGBL_OK;
 }
 

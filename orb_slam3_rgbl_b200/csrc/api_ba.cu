@@ -478,11 +478,6 @@ __global__ void ba_export_kernel(int n_poses, const Se3d* __restrict__ poses, co
     if (i < n3) pts_f[i] = (float)pts[i];
 }
 
-struct DevBuf {                 // the context's mapping arena, carved up
-    char* base = nullptr; size_t used = 0, cap = 0;
-    template <class T> T* take(size_t n) { used = (used + 255) & ~(size_t)255; T* p = reinterpret_cast<T*>(base + used); used += n * sizeof(T); return p; }
-};
-
 }  // namespace
 }  // namespace rgbl
 
@@ -524,11 +519,9 @@ extern "C" int rgbl_local_bundle_adjustment(rgbl_ctx* ctx, int n_poses, const fl
     const int n_part = std::max(eb, std::max(pb, qb));
 
     // ---- device arena ----
-    DevBuf a;
-    a.cap = (size_t)n_edges * (kEdgeBlk * 8 + 3 * 8 + 4 + 4 + 12 + 1 + 4 + 8) + (size_t)n_points * (4 + 9 * 8 * 2 + 6 * 8 + 12 + 12) + (size_t)n_poses * (2 * 56 + 8 + 2 * 28) +
-            (size_t)n_opt * (27 * 8 + 8 + 6 * 8 * 3) + (size_t)n * n * 8 + (size_t)n_part * 8 * 3 + (1 << 16);
-    a.base = mapping_arena(c, a.cap);
-    if (!a.base) { c->err = "cudaMalloc failed (local BA)"; return RGBL_E_CUDA; }
+    ArenaCarve a(c, (size_t)n_edges * (kEdgeBlk * 8 + 3 * 8 + 4 + 4 + 12 + 1 + 4 + 8) + (size_t)n_points * (4 + 9 * 8 * 2 + 6 * 8 + 12 + 12) + (size_t)n_poses * (2 * 56 + 8 + 2 * 28) +
+                    (size_t)n_opt * (27 * 8 + 8 + 6 * 8 * 3) + (size_t)n * n * 8 + (size_t)n_part * 8 * 3 + (1 << 16));
+    if (!a.base) { c->err = "device allocation failed (local BA)"; return RGBL_E_CUDA; }
     int* d_epoint = a.take<int>(n_edges); int* d_epose = a.take<int>(n_edges); float* d_obs = a.take<float>((size_t)3 * n_edges);
     uint8_t* d_stereo = a.take<uint8_t>(n_edges); float* d_info = a.take<float>(n_edges); uint8_t* d_erase = a.take<uint8_t>(n_edges);
     int* d_slot = a.take<int>(n_poses); int* d_ptstart = a.take<int>(n_points + 1); int* d_ptedges = a.take<int>(n_edges);
@@ -564,7 +557,7 @@ extern "C" int rgbl_local_bundle_adjustment(rgbl_ctx* ctx, int n_poses, const fl
         const int dev = c->cfg.device;
         if (dev >= 0 && dev < 64 && !done[dev]) { cudaFuncSetAttribute(ba_cholesky_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); done[dev] = true; }
     }
-    double* h = reinterpret_cast<double*>(c->h_scalars);      // 16 pinned ints = 8 doubles
+    double* h = reinterpret_cast<double*>(c->h_scalars.get());      // 16 pinned ints = 8 doubles
     int cur = 0, it_run = 0;
     double lambda = 0, ni = 2;
     int n_bad = 0;

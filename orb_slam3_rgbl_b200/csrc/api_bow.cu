@@ -1,6 +1,7 @@
 // C ABI entry points of Frame::ComputeBoW: the DBoW2 vocabulary as a device-resident flat tree and
 // TemplatedVocabulary::transform(features, BowVector, FeatureVector, levelsup) on it (bow_kernels.cu).
 #include <cstring>
+#include <memory>
 #include <vector>
 
 #include "rgbl_ctx.h"
@@ -9,24 +10,9 @@ namespace rgbl {
 
 struct Vocab {
     int device = 0, n_nodes = 0, L = 0;
-    int* child_begin = nullptr; int* child_index = nullptr; uint8_t* node_desc = nullptr; double* node_weight = nullptr; int* word_id = nullptr;
+    DeviceArray<int> child_begin, child_index; DeviceArray<uint8_t> node_desc; DeviceArray<double> node_weight; DeviceArray<int> word_id;
     VocabDev dev() const { return VocabDev{child_begin, child_index, node_desc, node_weight, word_id}; }
-    void release() {
-        void* all[] = {child_begin, child_index, node_desc, node_weight, word_id};
-        for (void* p : all) if (p) cudaFree(p);
-    }
 };
-
-template <class T>
-static bool grow_buf(T** p, size_t* cap, size_t need) {
-    if (need <= *cap) return true;
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    const size_t n = need + need / 4 + 64;
-    if (cudaMalloc((void**)p, n * sizeof(T)) != cudaSuccess) { *cap = 0; return false; }
-    *cap = n;
-    return true;
-}
 
 // descriptors already on the device (desc_dev, n rows)
 static int compute_bow_device(Ctx* c, const Vocab* v, int n, const uint8_t* desc_dev, int levelsup, int32_t* bow_word, double* bow_value,
@@ -36,7 +22,7 @@ static int compute_bow_device(Ctx* c, const Vocab* v, int n, const uint8_t* desc
     while (np2 < n) np2 <<= 1;
     // int layout: f_word[n] f_node[n] bow_word[n] fv_node[n] fv_start[n+1] fv_feature[np2] scratch[np2+1] counts[4]
     const size_t ni = (size_t)5 * n + 1 + 2 * (size_t)np2 + 1 + 4;
-    if (!grow_buf(&t.bw_i, &t.cap_bw_i, ni) || !grow_buf(&t.bw_d, &t.cap_bw_d, (size_t)2 * n + 2)) { c->err = "cudaMalloc failed (BoW scratch)"; return RGBL_E_CUDA; }
+    if (!t.bw_i.grow(ni, c->scratch_generation) || !t.bw_d.grow((size_t)2 * n + 2, c->scratch_generation)) { c->err = "device allocation failed (BoW scratch)"; return RGBL_E_CUDA; }
     int* f_word = t.bw_i; int* f_node = f_word + n; int* d_bow_word = f_node + n; int* d_fv_node = d_bow_word + n;
     int* d_fv_start = d_fv_node + n; int* d_fv_feature = d_fv_start + n + 1; int* scratch = d_fv_feature + np2; int* counts = scratch + np2 + 1;
     double* f_weight = t.bw_d; double* d_bow_value = f_weight + n;
@@ -82,20 +68,18 @@ int rgbl_vocabulary_create(rgbl_ctx* ctx, int n_nodes, const int32_t* child_begi
     for (int i = 0; i < n_nodes; ++i) if (child_begin[i + 1] < child_begin[i]) { c->err = "vocabulary child_begin is not monotone"; return RGBL_E_INVALID; }
     for (int k = 0; k < n_child; ++k) if (child_index[k] <= 0 || child_index[k] >= n_nodes) { c->err = "vocabulary child index out of range"; return RGBL_E_INVALID; }
     CU(cudaSetDevice(c->cfg.device));
-    Vocab* v = new Vocab();
+    std::unique_ptr<Vocab> v(new Vocab());
     v->device = c->cfg.device; v->n_nodes = n_nodes; v->L = levels;
-    bool ok = cudaMalloc((void**)&v->child_begin, (size_t)(n_nodes + 1) * sizeof(int)) == cudaSuccess &&
-              cudaMalloc((void**)&v->child_index, (size_t)std::max(n_child, 1) * sizeof(int)) == cudaSuccess &&
-              cudaMalloc((void**)&v->node_desc, (size_t)n_nodes * 32) == cudaSuccess &&
-              cudaMalloc((void**)&v->node_weight, (size_t)n_nodes * sizeof(double)) == cudaSuccess &&
-              cudaMalloc((void**)&v->word_id, (size_t)n_nodes * sizeof(int)) == cudaSuccess;
+    bool ok = v->child_begin.alloc((size_t)n_nodes + 1) == cudaSuccess && v->child_index.alloc(std::max(n_child, 1)) == cudaSuccess &&
+              v->node_desc.alloc((size_t)n_nodes * 32) == cudaSuccess && v->node_weight.alloc(n_nodes) == cudaSuccess &&
+              v->word_id.alloc(n_nodes) == cudaSuccess;
     ok = ok && cudaMemcpy(v->child_begin, child_begin, (size_t)(n_nodes + 1) * sizeof(int), cudaMemcpyHostToDevice) == cudaSuccess &&
          (n_child == 0 || cudaMemcpy(v->child_index, child_index, (size_t)n_child * sizeof(int), cudaMemcpyHostToDevice) == cudaSuccess) &&
          cudaMemcpy(v->node_desc, node_desc, (size_t)n_nodes * 32, cudaMemcpyHostToDevice) == cudaSuccess &&
          cudaMemcpy(v->node_weight, node_weight, (size_t)n_nodes * sizeof(double), cudaMemcpyHostToDevice) == cudaSuccess &&
          cudaMemcpy(v->word_id, word_id, (size_t)n_nodes * sizeof(int), cudaMemcpyHostToDevice) == cudaSuccess;
-    if (!ok) { v->release(); delete v; cudaGetLastError(); c->err = "cudaMalloc / upload of the vocabulary failed"; return RGBL_E_CUDA; }
-    *out = reinterpret_cast<rgbl_vocabulary*>(v);
+    if (!ok) { cudaGetLastError(); c->err = "allocation / upload of the vocabulary failed"; return RGBL_E_CUDA; }
+    *out = reinterpret_cast<rgbl_vocabulary*>(v.release());
     return RGBL_OK;
 }
 
@@ -103,7 +87,6 @@ void rgbl_vocabulary_destroy(rgbl_vocabulary* voc) {
     Vocab* v = reinterpret_cast<Vocab*>(voc);
     if (!v) return;
     cudaSetDevice(v->device);
-    v->release();
     delete v;
 }
 
@@ -121,7 +104,7 @@ int rgbl_compute_bow(rgbl_ctx* ctx, const rgbl_vocabulary* voc, int n, const uin
     if (n == 0) return RGBL_OK;
     CU(cudaSetDevice(c->cfg.device));
     TrackBufs& t = c->trk;
-    if (!grow_buf(&t.q_desc, &t.cap_q_desc, (size_t)n * 32)) { c->err = "cudaMalloc failed (BoW descriptors)"; return RGBL_E_CUDA; }
+    if (!t.q_desc.grow((size_t)n * 32, c->scratch_generation)) { c->err = "device allocation failed (BoW descriptors)"; return RGBL_E_CUDA; }
     CU(cudaMemcpyAsync(t.q_desc, desc, (size_t)n * 32, cudaMemcpyHostToDevice, c->st));
     return compute_bow_device(c, v, n, t.q_desc, levelsup, bow_word, bow_value, n_words, fv_node, fv_start, fv_feature, n_fv_nodes);
 }

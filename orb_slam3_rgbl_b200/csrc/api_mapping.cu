@@ -158,11 +158,6 @@ __global__ void __launch_bounds__(1024) triangulation_finish_kernel(int n1, int 
     if (tid == 0) *n_matches = s_nm;
 }
 
-struct Arena {
-    char* base = nullptr; size_t used = 0, cap = 0;
-    template <class T> T* take(size_t n) { used = (used + 255) & ~(size_t)255; T* p = reinterpret_cast<T*>(base + used); used += n * sizeof(T); return p; }
-};
-
 }  // namespace
 }  // namespace rgbl
 
@@ -179,10 +174,8 @@ int rgbl_distinctive_descriptors(rgbl_ctx* ctx, int n_points, const int32_t* obs
     if (obs_start[0] != 0 || total < 0 || (total > 0 && !desc)) { c->err = "bad observation table"; return RGBL_E_INVALID; }
     for (int p = 0; p < n_points; ++p) if (obs_start[p + 1] < obs_start[p]) { c->err = "obs_start is not monotone"; return RGBL_E_INVALID; }
     CU(cudaSetDevice(c->cfg.device));
-    Arena a;
-    a.cap = (size_t)(n_points + 1) * 4 + (size_t)total * 32 + (size_t)n_points * 4 + 4096;
-    a.base = mapping_arena(c, a.cap);
-    if (!a.base) { c->err = "cudaMalloc failed (distinctive descriptors)"; return RGBL_E_CUDA; }
+    ArenaCarve a(c, (size_t)(n_points + 1) * 4 + (size_t)total * 32 + (size_t)n_points * 4 + 4096);
+    if (!a.base) { c->err = "device allocation failed (distinctive descriptors)"; return RGBL_E_CUDA; }
     int* d_start = a.take<int>(n_points + 1); uint8_t* d_desc = a.take<uint8_t>((size_t)std::max(total, 1) * 32); int* d_best = a.take<int>(n_points);
     CU(cudaMemcpyAsync(d_start, obs_start, (size_t)(n_points + 1) * 4, cudaMemcpyHostToDevice, c->st));
     if (total) CU(cudaMemcpyAsync(d_desc, desc, (size_t)total * 32, cudaMemcpyHostToDevice, c->st));
@@ -233,10 +226,8 @@ int rgbl_search_for_triangulation(rgbl_ctx* ctx, int n1, const uint8_t* desc1, c
     for (int i = 0; i < n2; ++i) if (keys2[i].octave < 0 || keys2[i].octave >= n_levels) { c->err = "keypoint octave out of range"; return RGBL_E_INVALID; }
     if (n_q == 0 || n2 == 0) return RGBL_OK;
     CU(cudaSetDevice(c->cfg.device));
-    Arena ar;
-    ar.cap = (size_t)(n1 + n2) * (32 + sizeof(rgbl_keypoint) + 1 + 4 + 8) + (size_t)n_q * 12 + (size_t)n_csr2 * 4 + 16384;
-    ar.base = mapping_arena(c, ar.cap);
-    if (!ar.base) { c->err = "cudaMalloc failed (SearchForTriangulation)"; return RGBL_E_CUDA; }
+    ArenaCarve ar(c, (size_t)(n1 + n2) * (32 + sizeof(rgbl_keypoint) + 1 + 4 + 8) + (size_t)n_q * 12 + (size_t)n_csr2 * 4 + 16384);
+    if (!ar.base) { c->err = "device allocation failed (SearchForTriangulation)"; return RGBL_E_CUDA; }
     uint8_t* d_desc1 = ar.take<uint8_t>((size_t)n1 * 32); uint8_t* d_desc2 = ar.take<uint8_t>((size_t)n2 * 32);
     rgbl_keypoint* d_k1 = ar.take<rgbl_keypoint>(n1); rgbl_keypoint* d_k2 = ar.take<rgbl_keypoint>(n2);
     uint8_t* d_mp1 = ar.take<uint8_t>(n1); uint8_t* d_mp2 = ar.take<uint8_t>(n2); float* d_ur1 = ar.take<float>(n1); float* d_ur2 = ar.take<float>(n2);

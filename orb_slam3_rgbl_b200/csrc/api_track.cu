@@ -13,47 +13,32 @@
 
 namespace rgbl {
 
-// every reallocation of tracking scratch bumps the owning context's generation: cached chain graphs hold raw pointers
-static thread_local unsigned long long* g_generation_sink = nullptr;
-
-template <class T>
-static bool grow(T** p, size_t* cap, size_t need) {
-    if (need <= *cap) return true;
-    if (g_generation_sink) ++*g_generation_sink;
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    const size_t n = need + need / 4 + 64;
-    if (cudaMalloc((void**)p, n * sizeof(T)) != cudaSuccess) { *cap = 0; return false; }
-    *cap = n;
-    return true;
-}
-
-#define GROW(ptr, capvar, need) do { g_generation_sink = &c->scratch_generation; if (!grow(&(ptr), &(capvar), (size_t)(need))) { c->err = "cudaMalloc failed (tracking scratch)"; return RGBL_E_CUDA; } } while (0)
+#define GROW(buf, need) do { if (!(buf).grow((size_t)(need), c->scratch_generation)) { c->err = "device allocation failed (tracking scratch)"; return RGBL_E_CUDA; } } while (0)
 
 static int ensure_frame(Ctx* c, int n_frame) {
     TrackBufs& t = c->trk;
-    GROW(t.keys, t.cap_keys, n_frame); GROW(t.uright, t.cap_uright, n_frame); GROW(t.desc, t.cap_desc, (size_t)n_frame * 32);
-    GROW(t.csr_idx, t.cap_csr, n_frame); GROW(t.kp_cell, t.cap_kpcell, n_frame); GROW(t.state, t.cap_state, n_frame);
-    GROW(t.match, t.cap_match, n_frame); GROW(t.minq, t.cap_minq, n_frame);
-    if ((size_t)n_frame + 1 > t.cap_inv_cnt) {                // per-feature entry counters of the collect kernels + the entry total ([cap - 1]): zero between launches
-        GROW(t.inv_cnt, t.cap_inv_cnt, n_frame + 1);
-        CU(cudaMemsetAsync(t.inv_cnt, 0, t.cap_inv_cnt * sizeof(int), c->st));
+    GROW(t.keys, n_frame); GROW(t.uright, n_frame); GROW(t.desc, (size_t)n_frame * 32);
+    GROW(t.csr_idx, n_frame); GROW(t.kp_cell, n_frame); GROW(t.state, n_frame);
+    GROW(t.match, n_frame); GROW(t.minq, n_frame);
+    if ((size_t)n_frame + 1 > t.inv_cnt.size()) {             // per-feature entry counters of the collect kernels + the entry total ([size - 1]): zero between launches
+        GROW(t.inv_cnt, n_frame + 1);
+        CU(cudaMemsetAsync(t.inv_cnt, 0, t.inv_cnt.size() * sizeof(int), c->st));
     }
-    GROW(t.cell_start, t.cap_cellstart, kGridCols * kGridRows + 1);
-    GROW(t.scalars, t.cap_scalars, 16);
+    GROW(t.cell_start, kGridCols * kGridRows + 1);
+    GROW(t.scalars, 16);
     return RGBL_OK;
 }
 
 static int ensure_queries(Ctx* c, int n_q) {
     TrackBufs& t = c->trk;
-    GROW(t.lists, t.cap_lists, (size_t)n_q * kMatchListCap); GROW(t.list_slots, t.cap_list_slots, (size_t)n_q * kMatchListCap); GROW(t.list_n, t.cap_listn, n_q);
-    GROW(t.dense, t.cap_dense, (size_t)n_q * kMatchListCap); GROW(t.dense_slot, t.cap_dense_slot, (size_t)n_q * kMatchListCap);
-    GROW(t.dense_q, t.cap_dense_q, (size_t)n_q * kMatchListCap); GROW(t.list_base, t.cap_list_base, n_q);
-    GROW(t.choice, t.cap_choice, n_q); GROW(t.resolved, t.cap_resolved, n_q);
-    GROW(t.q_u8a, t.cap_q_u8a, n_q); GROW(t.q_u8b, t.cap_q_u8b, n_q); GROW(t.q_desc, t.cap_q_desc, (size_t)n_q * 32);
-    GROW(t.q_f3a, t.cap_q_f3a, (size_t)n_q * 3); GROW(t.q_f3b, t.cap_q_f3b, (size_t)n_q * 3);
-    for (int k = 0; k < 7; ++k) GROW(t.q_f[k], t.cap_q_f[k], n_q);
-    GROW(t.q_i, t.cap_q_i, n_q);
+    GROW(t.lists, (size_t)n_q * kMatchListCap); GROW(t.list_slots, (size_t)n_q * kMatchListCap); GROW(t.list_n, n_q);
+    GROW(t.dense, (size_t)n_q * kMatchListCap); GROW(t.dense_slot, (size_t)n_q * kMatchListCap);
+    GROW(t.dense_q, (size_t)n_q * kMatchListCap); GROW(t.list_base, n_q);
+    GROW(t.choice, n_q); GROW(t.resolved, n_q);
+    GROW(t.q_u8a, n_q); GROW(t.q_u8b, n_q); GROW(t.q_desc, (size_t)n_q * 32);
+    GROW(t.q_f3a, (size_t)n_q * 3); GROW(t.q_f3b, (size_t)n_q * 3);
+    for (int k = 0; k < 7; ++k) GROW(t.q_f[k], n_q);
+    GROW(t.q_i, n_q);
     return RGBL_OK;
 }
 
@@ -89,7 +74,7 @@ static MatchScratch scratch(Ctx* c) {
     TrackBufs& t = c->trk;
     MatchScratch s;
     s.lists = t.lists; s.list_cap = kMatchListCap; s.list_n = t.list_n; s.minq = t.minq; s.choice = t.choice; s.resolved = t.resolved;
-    s.overflow = c->d_overflow; s.rounds = t.scalars + 2; s.slots = t.list_slots; s.inv_cnt = t.inv_cnt; s.total = t.inv_cnt + (t.cap_inv_cnt - 1);
+    s.overflow = c->d_overflow; s.rounds = t.scalars + 2; s.slots = t.list_slots; s.inv_cnt = t.inv_cnt; s.total = t.inv_cnt + (t.inv_cnt.size() - 1);
     s.dense = t.dense; s.dense_slot = t.dense_slot; s.dense_q = t.dense_q; s.base = t.list_base;
     return s;
 }
@@ -269,7 +254,7 @@ int rgbl_pose_optimize(rgbl_ctx* ctx, const float pose_in[7], int n, const float
     int rc = ensure_queries(c, std::max(n, 1)); if (rc) return rc;
     rc = ensure_frame(c, 1); if (rc) return rc;
     TrackBufs& t = c->trk;
-    GROW(t.pose_work, t.cap_pose_work, (size_t)std::max(n, 1) * 3);
+    GROW(t.pose_work, (size_t)std::max(n, 1) * 3);
     if (n) {
         CU(cudaMemcpyAsync(t.q_f3a, xw, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, c->st));
         CU(cudaMemcpyAsync(t.q_f3b, obs, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, c->st));
@@ -310,7 +295,7 @@ int rgbl_fuse_search(rgbl_ctx* ctx, const rgbl_frame_view* kf, const float Tcw[7
     int rc = upload_frame(c, kf, f); if (rc) return rc;
     rc = ensure_queries(c, n); if (rc) return rc;
     TrackBufs& t = c->trk;
-    GROW(t.e_idx, t.cap_e_idx, (size_t)2 * n);
+    GROW(t.e_idx, (size_t)2 * n);
     CU(cudaMemcpyAsync(t.q_u8a, valid, n, cudaMemcpyHostToDevice, c->st));
     CU(cudaMemcpyAsync(t.q_f3a, xw, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, c->st));
     CU(cudaMemcpyAsync(t.q_f3b, normal, (size_t)n * 3 * sizeof(float), cudaMemcpyHostToDevice, c->st));
@@ -341,7 +326,7 @@ int rgbl_stereo_matches(rgbl_ctx* ctx, int slot_left, int slot_right, float mb, 
     if (c->cap_kp > 65535) { c->err = "more than 65535 keypoints per frame"; return RGBL_E_UNSUPPORTED; }
     CU(cudaSetDevice(c->cfg.device));
     TrackBufs& t = c->trk;
-    GROW(t.e_idx, t.cap_e_idx, c->cap_kp);
+    GROW(t.e_idx, c->cap_kp);
     StereoFrameDev L{}, R{};
     L.n = c->d_n_sel + slot_left; L.keys = c->d_kps + (size_t)slot_left * c->cap_kp; L.desc = c->d_desc + (size_t)slot_left * c->cap_kp * 32;
     R.n = c->d_n_sel + slot_right; R.keys = c->d_kps + (size_t)slot_right * c->cap_kp; R.desc = c->d_desc + (size_t)slot_right * c->cap_kp * 32;
@@ -403,7 +388,7 @@ int rgbl_search_by_bow(rgbl_ctx* ctx, int n_kf, const uint8_t* kf_desc, const fl
     int rc = ensure_frame(c, std::max(n_f, n_fcsr)); if (rc) return rc;
     rc = ensure_queries(c, std::max(n_q, n_kf)); if (rc) return rc;
     TrackBufs& t = c->trk;
-    GROW(t.e_idx, t.cap_e_idx, (size_t)3 * n_q);
+    GROW(t.e_idx, (size_t)3 * n_q);
     CU(cudaMemcpyAsync(t.q_desc, kf_desc, (size_t)n_kf * 32, cudaMemcpyHostToDevice, c->st));
     CU(cudaMemcpyAsync(t.desc, f_desc, (size_t)n_f * 32, cudaMemcpyHostToDevice, c->st));
     CU(cudaMemcpyAsync(t.uright, f_angle, (size_t)n_f * sizeof(float), cudaMemcpyHostToDevice, c->st));       // reused as F angles
@@ -496,25 +481,28 @@ static int chain_begin(Ctx* c, const rgbl_chain_params& cp_) {
     if (cont && !c->chain_has_carry) { c->err = "continue_sequence without a previous chain on this context"; return RGBL_E_INVALID; }
     if (cont && (c->carry_K != K || c->carry_cap != cap)) { c->err = "continue_sequence: local_map_frames / keypoint capacity differ from the previous chain"; return RGBL_E_INVALID; }
     CU(cudaSetDevice(c->cfg.device));
+    // the tracking stream and the chain's events: each one created by the first chain that finds it missing
     if (!c->st_trk) {
         int lo = 0, hi = 0;
         CU(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-        CU(cudaStreamCreateWithPriority(&c->st_trk, cudaStreamNonBlocking, hi));
-        CU(cudaEventCreateWithFlags(&c->ev_snap, cudaEventDisableTiming));
-        for (int i = 0; i < 2; ++i) {
-            CU(cudaEventCreate(&c->ev_chain_b[i])); CU(cudaEventCreate(&c->ev_chain_e[i]));
-            CU(cudaEventCreateWithFlags(&c->ev_chain_done[i], cudaEventDisableTiming));
-        }
+        CU(c->st_trk.create(hi));
     }
+    auto have = [](Event& e, unsigned flags) { return e ? cudaSuccess : e.create(flags); };
+    CU(have(c->ev_snap, cudaEventDisableTiming));
+    for (int i = 0; i < 2; ++i) {
+        CU(have(c->ev_chain_b[i], 0)); CU(have(c->ev_chain_e[i], 0));
+        CU(have(c->ev_chain_done[i], cudaEventDisableTiming));
+    }
+    // RGBL_CHAIN_TIMING=1: CUDA events between the launches of the middle frame (warm, in-stream kernel times; stderr at _end)
+    if (c->chain_timing_on) for (Event& e : c->chain_tev) CU(have(e, 0));
     const size_t n_counts = (size_t)4 * nF + 8;          // n_matches | n_inliers | n_local_matches | n_inliers_first | ne, ne2, flags[2], overflow, nq
     if (c->h_chain_cap < (size_t)nF) {
         if (c->chain_pending) { c->err = "batch size grew while a chain is in flight"; return RGBL_E_INVALID; }
-        if (c->h_chain_f) cudaFreeHost(c->h_chain_f);
-        if (c->h_chain_i) cudaFreeHost(c->h_chain_i);
-        c->h_chain_f = nullptr; c->h_chain_i = nullptr; c->h_chain_cap = 0;
-        const size_t capF = (size_t)std::max(nF, c->cfg.max_batch);
-        CU(cudaMallocHost(&c->h_chain_f, 2 * (7 + capF * 7) * sizeof(float)));
-        CU(cudaMallocHost(&c->h_chain_i, 2 * (4 * capF + 8) * sizeof(int)));
+        const size_t capF = (size_t)std::max(nF, c->cfg.max_batch), nf = 2 * (7 + capF * 7), ni = 2 * (4 * capF + 8);
+        c->h_chain_cap = 0;
+        if (!c->h_chain_f.grow(nf, c->scratch_generation, nf) || !c->h_chain_i.grow(ni, c->scratch_generation, ni)) {
+            c->err = "pinned allocation failed (chain result staging)"; return RGBL_E_CUDA;
+        }
         c->h_chain_cap = capF;
     }
     int rc = ensure_frame(c, cap); if (rc) return rc;
@@ -522,23 +510,23 @@ static int chain_begin(Ctx* c, const rgbl_chain_params& cp_) {
     rc = ensure_queries(c, std::max(cap, n_lq)); if (rc) return rc;
     TrackBufs& t = c->trk;
     const size_t tot = (size_t)nF * cap;
-    GROW(t.pose_work, t.cap_pose_work, (size_t)cap * 3);
-    GROW(t.ch_poses, t.cap_ch_poses, (size_t)nF * 7 + 14); GROW(t.ch_counts, t.cap_ch_counts, n_counts);      // poses | pose after TrackWithMotionModel | predicted pose
-    GROW(t.e_xw, t.cap_e_xw, (size_t)cap * 3); GROW(t.e_obs, t.cap_e_obs, (size_t)cap * 3); GROW(t.e_info, t.cap_e_info, cap);
-    GROW(t.e_st, t.cap_e_st, cap); GROW(t.e_lvl, t.cap_e_lvl, cap); GROW(t.e_out, t.cap_e_out, cap); GROW(t.e_idx, t.cap_e_idx, cap);
+    GROW(t.pose_work, (size_t)cap * 3);
+    GROW(t.ch_poses, (size_t)nF * 7 + 14); GROW(t.ch_counts, n_counts);      // poses | pose after TrackWithMotionModel | predicted pose
+    GROW(t.e_xw, (size_t)cap * 3); GROW(t.e_obs, (size_t)cap * 3); GROW(t.e_info, cap);
+    GROW(t.e_st, cap); GROW(t.e_lvl, cap); GROW(t.e_out, cap); GROW(t.e_idx, cap);
     // carried last frame of the sequence + the local map ring (persist across chains of this context)
-    GROW(t.c_kps, t.cap_c_kps, cap); GROW(t.c_desc, t.cap_c_desc, (size_t)cap * 32); GROW(t.c_depth, t.cap_c_depth, cap);
-    GROW(t.c_misc, t.cap_c_misc, 16);                     // int n_sel | float pose[7] (as raw 32-bit words) | ring count | float prev_pose[7]
+    GROW(t.c_kps, cap); GROW(t.c_desc, (size_t)cap * 32); GROW(t.c_depth, cap);
+    GROW(t.c_misc, 16);                     // int n_sel | float pose[7] (as raw 32-bit words) | ring count | float prev_pose[7]
     if (K > 0) {
         const size_t nr = (size_t)K * cap;
-        if (cont && (t.cap_r_valid < nr)) { c->err = "local map ring missing"; return RGBL_E_INVALID; }
-        GROW(t.r_valid, t.cap_r_valid, nr); GROW(t.r_xw, t.cap_r_xw, nr * 3); GROW(t.r_normal, t.cap_r_normal, nr * 3);
-        GROW(t.r_min, t.cap_r_min, nr); GROW(t.r_max, t.cap_r_max, nr); GROW(t.r_desc, t.cap_r_desc, nr * 32);
-        GROW(t.lq_u8, t.cap_lq_u8, 2 * (size_t)n_lq); GROW(t.lq_f, t.cap_lq_f, 8 * (size_t)n_lq); GROW(t.lq_i, t.cap_lq_i, 2 * (size_t)n_lq);
-        GROW(t.lq_desc, t.cap_lq_desc, (size_t)n_lq * 32); GROW(t.match_local, t.cap_match_local, cap);
+        if (cont && t.r_valid.size() < nr) { c->err = "local map ring missing"; return RGBL_E_INVALID; }
+        GROW(t.r_valid, nr); GROW(t.r_xw, nr * 3); GROW(t.r_normal, nr * 3);
+        GROW(t.r_min, nr); GROW(t.r_max, nr); GROW(t.r_desc, nr * 32);
+        GROW(t.lq_u8, 2 * (size_t)n_lq); GROW(t.lq_f, 8 * (size_t)n_lq); GROW(t.lq_i, 2 * (size_t)n_lq);
+        GROW(t.lq_desc, (size_t)n_lq * 32); GROW(t.match_local, cap);
         if (!t.lookback) {
-            GROW(t.lookback, t.cap_lookback, tlm_lookback_ints());
-            CU(cudaMemsetAsync(t.lookback, 0, t.cap_lookback * sizeof(int), c->st));     // ordered before the chain by ev_snap below
+            GROW(t.lookback, tlm_lookback_ints());
+            CU(cudaMemsetAsync(t.lookback, 0, t.lookback.size() * sizeof(int), c->st));     // ordered before the chain by ev_snap below
         }
         if ((n_lq + 255) / 256 + 1 > 1024) { c->err = "local map too large for the compaction slots (local_map_frames x keypoint capacity > 261 k)"; return RGBL_E_UNSUPPORTED; }
     }
@@ -546,11 +534,11 @@ static int chain_begin(Ctx* c, const rgbl_chain_params& cp_) {
     // never move while a chain is in flight)
     const size_t tot_full = (size_t)std::max(nF, c->cfg.max_batch) * cap, nF_full = (size_t)std::max(nF, c->cfg.max_batch);
     const size_t cs_full = nF_full * (kGridCols * kGridRows + 1);
-    if (c->chain_pending && (t.cap_s_kps < 2 * tot_full || t.cap_b_cell_start < 2 * cs_full)) { c->err = "batch size grew while a chain is in flight"; return RGBL_E_INVALID; }
-    GROW(t.s_kps, t.cap_s_kps, 2 * tot_full); GROW(t.s_desc, t.cap_s_desc, 2 * tot_full * 32); GROW(t.s_depth, t.cap_s_depth, 2 * tot_full);
-    GROW(t.s_uright, t.cap_s_uright, 2 * tot_full); GROW(t.s_nsel, t.cap_s_nsel, 2 * nF_full);
-    GROW(t.b_cell_start, t.cap_b_cell_start, 2 * cs_full);
-    GROW(t.b_csr_idx, t.cap_b_csr_idx, 2 * tot_full); GROW(t.b_kp_cell, t.cap_b_kp_cell, 2 * tot_full);
+    if (c->chain_pending && (t.s_kps.size() < 2 * tot_full || t.b_cell_start.size() < 2 * cs_full)) { c->err = "batch size grew while a chain is in flight"; return RGBL_E_INVALID; }
+    GROW(t.s_kps, 2 * tot_full); GROW(t.s_desc, 2 * tot_full * 32); GROW(t.s_depth, 2 * tot_full);
+    GROW(t.s_uright, 2 * tot_full); GROW(t.s_nsel, 2 * nF_full);
+    GROW(t.b_cell_start, 2 * cs_full);
+    GROW(t.b_csr_idx, 2 * tot_full); GROW(t.b_kp_cell, 2 * tot_full);
     rgbl_keypoint* s_kps = t.s_kps + slot * tot_full; uint8_t* s_desc = t.s_desc + slot * tot_full * 32;
     float* s_depth = t.s_depth + slot * tot_full; float* s_uright = t.s_uright + slot * tot_full; int* s_nsel = t.s_nsel + slot * nF_full;
     int* b_cell_start = t.b_cell_start + slot * cs_full; int* b_csr_idx = t.b_csr_idx + slot * tot_full; int* b_kp_cell = t.b_kp_cell + slot * tot_full;
@@ -572,15 +560,13 @@ static int chain_begin(Ctx* c, const rgbl_chain_params& cp_) {
     CU(cudaStreamWaitEvent(cs, c->ev_snap, 0));
 
     for (int i = 0; i < 7; ++i) h_f[i] = P.pose0[i];
-    // RGBL_CHAIN_TIMING=1: CUDA events between the launches of the middle frame (warm, in-stream kernel times; stderr at _end)
     const bool chain_timing = c->chain_timing_on;
     const bool chain_graphs = c->chain_graphs_on;
-    cudaEvent_t* tev = c->chain_tev;
-    if (chain_timing && !tev[0]) for (int i = 0; i < 8; ++i) cudaEventCreate(&tev[i]);
-    int* c_nsel = reinterpret_cast<int*>(t.c_misc);
-    float* c_pose = reinterpret_cast<float*>(t.c_misc) + 1;
-    int* r_count = reinterpret_cast<int*>(t.c_misc) + 8;
-    float* c_prev = reinterpret_cast<float*>(t.c_misc) + 9;      // pose of the frame before the carried one (valid: c->carry_prev_valid)
+    const Event* tev = c->chain_tev;
+    int* c_nsel = reinterpret_cast<int*>(t.c_misc.get());
+    float* c_pose = reinterpret_cast<float*>(t.c_misc.get()) + 1;
+    int* r_count = reinterpret_cast<int*>(t.c_misc.get()) + 8;
+    float* c_prev = reinterpret_cast<float*>(t.c_misc.get()) + 9;      // pose of the frame before the carried one (valid: c->carry_prev_valid)
     const bool prev_valid = cont && c->carry_prev_valid;
     int n_launches = 0;
     const float* bounds = c->frame_bounds;
@@ -690,7 +676,7 @@ static int chain_begin(Ctx* c, const rgbl_chain_params& cp_) {
         if (nF >= 2) CU(cudaMemcpyAsync(c_prev, poses + 7 * (size_t)(nF - 2), 7 * sizeof(float), cudaMemcpyDeviceToDevice, cs));
         else if (cont) CU(cudaMemcpyAsync(c_prev, c_pose, 7 * sizeof(float), cudaMemcpyDeviceToDevice, cs));
         CU(cudaMemcpyAsync(c_pose, poses + 7 * (size_t)(nF - 1), 7 * sizeof(float), cudaMemcpyDeviceToDevice, cs));
-        if (chain_timing) c->chain_timing_ev = tev;
+        if (chain_timing) c->chain_timing_recorded = true;
         CU(cudaGetLastError());
         CU(cudaMemcpyAsync(h_f + 7, poses, (size_t)nF * 7 * sizeof(float), cudaMemcpyDeviceToHost, cs));
         CU(cudaMemcpyAsync(h_i, t.ch_counts, n_counts * sizeof(int), cudaMemcpyDeviceToHost, cs));
@@ -703,7 +689,7 @@ static int chain_begin(Ctx* c, const rgbl_chain_params& cp_) {
         key.nF = nF; key.cap = cap; key.mono = mono; key.cont = cont ? 1 : 0; key.K = K; key.prev_valid = prev_valid ? 1 : 0; key.th = th; key.th_local = P.th_local; key.nn_local = P.nn_ratio_local;
         key.fx = fx; key.fy = fy; key.cx = cx; key.cy = cy; key.bf = bf; std::memcpy(key.bounds, bounds, sizeof(key.bounds)); key.generation = c->scratch_generation;
         if (!c->chain_exec[slot] || std::memcmp(&key, &c->chain_key[slot], sizeof(key)) != 0) {
-            if (c->chain_exec[slot]) { cudaGraphExecDestroy(c->chain_exec[slot]); c->chain_exec[slot] = nullptr; }
+            c->chain_exec[slot].reset();
             prepare_match_kernels();
             CU(cudaStreamBeginCapture(cs, cudaStreamCaptureModeRelaxed));
             chain_launch_pdl() = c->chain_pdl_on;           // programmatic dependent launches between the chain's kernels (rgbl_device.cuh: pdl_wait)
@@ -717,9 +703,9 @@ static int chain_begin(Ctx* c, const rgbl_chain_params& cp_) {
                 if (rc_cap == RGBL_OK) c->err = std::string("chain graph capture failed: ") + cudaGetErrorString(e_cap);
                 return rc_cap != RGBL_OK ? rc_cap : RGBL_E_CUDA;
             }
-            const cudaError_t e_inst = cudaGraphInstantiate(&c->chain_exec[slot], graph, 0);
+            const cudaError_t e_inst = c->chain_exec[slot].instantiate(graph);
             cudaGraphDestroy(graph);
-            if (e_inst != cudaSuccess) { c->chain_exec[slot] = nullptr; c->err = std::string("cudaGraphInstantiate: ") + cudaGetErrorString(e_inst); return RGBL_E_CUDA; }
+            if (e_inst != cudaSuccess) { c->err = std::string("cudaGraphInstantiate: ") + cudaGetErrorString(e_inst); return RGBL_E_CUDA; }
             c->chain_key[slot] = key;
             c->chain_graph_launches[slot] = n_launches;
         }
@@ -775,8 +761,8 @@ int rgbl_resident_track_end2(rgbl_ctx* ctx, float* poses_out, int* n_matches, in
     const int nF = c->chain_frames[slot];
     const float* h_f = c->h_chain_f + (size_t)slot * (7 + c->h_chain_cap * 7);
     const int* h_i = c->h_chain_i + (size_t)slot * (4 * c->h_chain_cap + 8);
-    if (c->chain_timing_ev && c->chain_pending == 0) {
-        const cudaEvent_t* e = static_cast<const cudaEvent_t*>(c->chain_timing_ev);
+    if (c->chain_timing_recorded && c->chain_pending == 0) {
+        const Event* e = c->chain_tev;
         const char* names[6] = {"chain_prep (first frame only)", "search_last (collect+resolve+edges)", "pose_optimize #1", "tlm_prepare + search_local (+edges, hand-over)", "-", "pose_optimize #2"};
         for (int i = 0; i < 6; ++i) { float ms = 0; if (cudaEventElapsedTime(&ms, e[i], e[i + 1]) == cudaSuccess) std::fprintf(stderr, "[chain timing] %-36s %8.2f us\n", names[i], ms * 1e3f); }
         cudaGetLastError();

@@ -54,23 +54,25 @@ FULL_SRCS = ["api.cu", "api_track.cu", "quadtree_kernels.cu", "orb_kernels.cu", 
 # st.async + mbarrier (PTX); emu_stubs.cpp aborts with a message if the emulated library reaches PoseOptimization.
 
 
-def build_full(force: bool = False, defines=()) -> Path:
+def build_full(force: bool = False, defines=(), sanitize: str | None = None, out_dir: Path | None = None) -> Path:
     """The WHOLE library (every .cu / .cpp of csrc/Makefile) against the shim: build/librgbl_b200_emu.so exports the C ABI of
-    include/rgbl_b200.h, so the -m gpu parity tests can run on the CPU (RGBL_LIB_PATH, see orb_slam3_rgbl_b200/_lib.py)."""
+    include/rgbl_b200.h, so the -m gpu parity tests can run on the CPU (RGBL_LIB_PATH, see orb_slam3_rgbl_b200/_lib.py).
+    sanitize ("address" | "thread") builds with -fsanitize=...; out_dir: where the library and its objects go (default build/)."""
     from concurrent.futures import ThreadPoolExecutor
+    out_dir = Path(out_dir) if out_dir else BUILD
+    lib = out_dir / FULL_LIB.name
     hdrs = [f.name for f in CSRC.iterdir() if f.suffix in (".h", ".cuh", ".inc")]
     srcs = [CSRC / f for f in FULL_SRCS + hdrs] + [HERE / "cuda_runtime.h", HERE / "emu_runtime.cpp", Path(__file__)]
-    if FULL_LIB.exists() and not force and all(FULL_LIB.stat().st_mtime > s.stat().st_mtime for s in srcs):
-        return FULL_LIB
-    full = BUILD / "full"
+    if lib.exists() and not force and all(lib.stat().st_mtime > s.stat().st_mtime for s in srcs):
+        return lib
+    full = out_dir / "full"
     if full.exists():
         shutil.rmtree(full)
     full.mkdir(parents=True)
     for f in FULL_SRCS + hdrs:
         out = full / ((f[:-3] + ".emu.cpp") if f.endswith(".cu") else f)
         out.write_text(_transform((CSRC / f).read_text()))
-    import os
-    san = ["-fsanitize=" + os.environ["EMU_SANITIZE"]] if os.environ.get("EMU_SANITIZE") else []      # address | thread (debugging aid)
+    san = ["-fsanitize=" + sanitize] if sanitize else []
     flags = ["-std=c++20", "-O1", "-g", "-pthread", "-fPIC", "-ffp-contract=off", "-Wno-unknown-pragmas", "-Wno-attributes", f"-I{HERE}", f"-I{full}",
              "-include", str(HERE / "cuda_runtime.h"), "-DRGBL_TESTING_EXPORTS"] + list(defines) + san       # the shim first: __CUDA_ARCH__ must be set before any header
     units = [full / ((f[:-3] + ".emu.cpp") if f.endswith(".cu") else f) for f in FULL_SRCS] + [HERE / "emu_runtime.cpp", HERE / "emu_stubs.cpp"]
@@ -86,8 +88,8 @@ def build_full(force: bool = False, defines=()) -> Path:
     errs = [o for o in objs if isinstance(o, Exception)]
     if errs:
         raise RuntimeError("\n".join(str(e) for e in errs))
-    subprocess.run(["g++", "-shared", "-pthread", *san, "-o", str(FULL_LIB), *map(str, objs), "-lz"], check=True)
-    return FULL_LIB
+    subprocess.run(["g++", "-shared", "-pthread", *san, "-o", str(lib), *map(str, objs), "-lz"], check=True)
+    return lib
 
 
 TLM_CHECK = BUILD / "tlm_check"

@@ -169,13 +169,20 @@ typedef void* cudaGraphExec_t;
 enum cudaMemcpyKind { cudaMemcpyHostToHost = 0, cudaMemcpyHostToDevice = 1, cudaMemcpyDeviceToHost = 2, cudaMemcpyDeviceToDevice = 3 };
 enum { cudaStreamNonBlocking = 1, cudaEventDisableTiming = 2 };
 enum cudaStreamCaptureMode { cudaStreamCaptureModeRelaxed = 2 };
-enum { cudaErrorNotSupported = 801 };
+enum { cudaErrorMemoryAllocation = 2, cudaErrorNotSupported = 801 };
 inline const char* cudaGetErrorString(cudaError_t e) { return e == cudaSuccess ? "no error" : "emulated CUDA error"; }
 inline cudaError_t cudaGetLastError() { return cudaSuccess; }
 inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
 inline cudaError_t cudaDeviceGetStreamPriorityRange(int* lo, int* hi) { *lo = 0; *hi = -1; return cudaSuccess; }
-template <class T> inline cudaError_t cudaMalloc(T** p, size_t n) { *p = (T*)calloc(n + 256, 1); return *p ? cudaSuccess : 2; }
-template <class T> inline cudaError_t cudaMallocHost(T** p, size_t n) { *p = (T*)calloc(n + 256, 1); return *p ? cudaSuccess : 2; }
+// allocation-failure injection: emu_fail_allocation(k) makes the k-th cudaMalloc / cudaMallocHost from now on fail (once; -1: none) and
+// returns the countdown it replaces (-1: the previous one has fired, or none was set)
+extern "C" int emu_fail_allocation(int nth);
+namespace emu { bool allocation_fails(); }
+template <class T> inline cudaError_t cudaMalloc(T** p, size_t n) {
+    if (emu::allocation_fails()) return cudaErrorMemoryAllocation;
+    *p = (T*)calloc(n + 256, 1); return *p ? cudaSuccess : cudaErrorMemoryAllocation;
+}
+template <class T> inline cudaError_t cudaMallocHost(T** p, size_t n) { return cudaMalloc(p, n); }
 inline cudaError_t cudaFree(void* p) { free(p); return cudaSuccess; }
 inline cudaError_t cudaFreeHost(void* p) { free(p); return cudaSuccess; }
 inline cudaError_t cudaMemcpy(void* d, const void* s, size_t n, cudaMemcpyKind) { memmove(d, s, n); return cudaSuccess; }

@@ -8,6 +8,12 @@ namespace emu {
 // CUDA graphs are not emulated (cuda_runtime.h): make the library replay its tracking chain launch by launch
 static const int g_no_graphs = setenv("RGBL_CHAIN_GRAPH", "0", 1);
 Cta* g_cta = nullptr;
+static int g_fail_countdown = -1;          // allocations happen on the host thread only
+bool allocation_fails() {
+    if (g_fail_countdown < 0 || --g_fail_countdown > 0) return false;
+    g_fail_countdown = -1;
+    return true;
+}
 thread_local int t_warp = 0, t_lane = 0;
 
 void run(const Cfg& c, const std::function<void()>& body) {
@@ -37,3 +43,9 @@ void run(const Cfg& c, const std::function<void()>& body) {
             }
 }
 }  // namespace emu
+
+extern "C" int emu_fail_allocation(int nth) {
+    const int prev = emu::g_fail_countdown;
+    emu::g_fail_countdown = nth;
+    return prev;
+}
