@@ -412,6 +412,31 @@ int rgbl_resident_stage_rgbd(rgbl_ctx* ctx, int slot, int n_frames, const uint8_
 int rgbl_track_sequence_rgbd(rgbl_ctx* ctx, float depth_scale, float bf, const rgbl_chain_params* chain, const rgbl_sequence_io* io,
                              const uint16_t* const* depth, int depth_stride);
 
+/* ---- Stereo: System::TrackStereo -> Tracking::GrabImageStereo -> stereo Frame constructor (src/Frame.cc:101-197: the two ORBextractor
+ * calls, then ComputeStereoMatches :901-1071), batched and resident like the RGB-D entry points above.  n_pairs rectified pairs are
+ * extracted as ONE batch of 2 n_pairs frames, left images in frame slots [0, n_pairs), right ones in [n_pairs, 2 n_pairs), so
+ * 2 n_pairs <= max_batch (RGBL_E_INVALID otherwise).  After rgbl_resident_process_stereo the left frames are the batch: rgbl_resident_download,
+ * rgbl_resident_download_keys_un, rgbl_resident_compute_bow and rgbl_resident_track_begin2 / _end2 see them as they see RGB-L or RGB-D frames
+ * (chain parameters for stereo: th_last 7, th_local 1).  A capacity overflow in the frame construction of a right frame fails _end2 with
+ * RGBL_E_CAPACITY like one in a left frame.  The images must be rectified: on a context whose camera has k1 != 0
+ * (rgbl_set_camera_distortion) every stereo entry point returns RGBL_E_UNSUPPORTED.                                                      */
+int rgbl_resident_upload_stereo(rgbl_ctx* ctx, int n_pairs, const uint8_t* const* left, const uint8_t* const* right, int width, int height, int stride);
+/* Same with the files' bytes (KITTI image_0 / image_1 PNGs), decoded as for rgbl_resident_upload_kitti_png; every stream must have the
+ * context's size.                                                                                                                      */
+int rgbl_resident_upload_stereo_png(rgbl_ctx* ctx, int n_pairs, const uint8_t* const* left_png, const size_t* left_bytes, const uint8_t* const* right_png,
+                                    const size_t* right_bytes, int camera_rgb);
+/* Frame construction of the uploaded pairs: mb = mbf / fx (the stereo Frame constructor's mb), mbf = Camera.bf; both finite and > 0.
+ * ComputeStereoMatches is billed to the `match` profiling stage.  RGBL_E_INVALID when the uploaded frames are not stereo pairs.         */
+int rgbl_resident_process_stereo(rgbl_ctx* ctx, float mb, float mbf, int* n_out /* nullable, [n_pairs] keypoints of the left frames */);
+/* Upload one batch of n_pairs stereo pairs into staged slot `slot` for the resident mode of rgbl_track_sequence_stereo. */
+int rgbl_resident_stage_stereo(rgbl_ctx* ctx, int slot, int n_pairs, const uint8_t* const* left, const uint8_t* const* right, int width, int height,
+                               int stride);
+/* The sequence runner for stereo (the loop of Examples/Stereo/stereo_kitti.cc: load left + right image -> SLAM.TrackStereo -> pose), as
+ * rgbl_track_sequence with frames_per_batch pairs per batch: io->pts4xn / io->n_pts must be NULL; host mode (io->gray != NULL, the left
+ * images) takes right[] (one per frame of the call), resident mode takes slots staged with rgbl_resident_stage_stereo (a slot of another
+ * kind is RGBL_E_INVALID, and so is a stereo slot given to the other runners).                                                          */
+int rgbl_track_sequence_stereo(rgbl_ctx* ctx, float mb, float mbf, const rgbl_chain_params* chain, const rgbl_sequence_io* io, const uint8_t* const* right);
+
 /* ---- Camera model of Frame::UndistortKeyPoints / ComputeImageBounds (src/Frame.cc:837-899) for every later batched frame construction
  * (rgbl_frame_rgbl_batch, rgbl_resident_process, rgbl_resident_process_rgbd, both sequence runners) and tracking chain of this context:
  * K = (fx, fy, cx, cy) (Pinhole::toK() == mK), dist = mDistCoef (k1, k2, p1, p2[, k3]), n_dist 4 or 5.  The keypoints are undistorted

@@ -189,10 +189,10 @@ void prof_collect(Ctx* c) {
 // Stage 1 (device): pyramid, FAST + compaction on the main stream; blur on the aux stream.
 // Stage 2 (host):   quad-tree per (frame, level) on worker threads -> SelKp lists.
 // Stage 3 (device): describe.  Results stay in d_kps / d_desc (copied out by the callers).
-static int upload_images(Ctx* c, int n_frames, const uint8_t* const* gray, int stride, cudaStream_t st) {
+static int upload_images(Ctx* c, int n_frames, const uint8_t* const* gray, int stride, cudaStream_t st, int first_slot = 0) {
     const LevelGeom& l0 = c->levels[0];
     for (int f = 0; f < n_frames; ++f)
-        CU(cudaMemcpy2DAsync(c->d_pyr + (size_t)f * c->frame_bytes + l0.off, l0.pitch, gray[f], stride, c->cfg.width,
+        CU(cudaMemcpy2DAsync(c->d_pyr + (size_t)(first_slot + f) * c->frame_bytes + l0.off, l0.pitch, gray[f], stride, c->cfg.width,
                              c->cfg.height, cudaMemcpyHostToDevice, st));
     return RGBL_OK;
 }
@@ -433,6 +433,29 @@ static int setup_depth(Ctx* c, const float P[12], const rgbl_depth_params* prm, 
         }
         c->stamp = 1;
     }
+    return RGBL_OK;
+}
+
+int stereo_matches(Ctx* c, int l0, int r0, int n_pairs, float mb, float mbf) {
+    if (c->cap_kp > 65535) { c->err = "more than 65535 keypoints per frame"; return RGBL_E_UNSUPPORTED; }      // the match key holds 16 index bits
+    const int H = c->cfg.height;
+    const size_t pairs = (size_t)std::max(1, c->cfg.max_batch / 2);
+    c->stereo_idx_cap = stereo_row_index_cap(c->cap_kp, c->tab.scale, c->tab.nlevels, H);
+    if (!ensure(c->d_stereo_row_start, pairs * (H + 1)) || !ensure(c->d_stereo_row_idx, pairs * c->stereo_idx_cap) || !ensure(c->d_stereo_sad, pairs * c->cap_kp)) {
+        c->err = "device allocation failed (stereo row index)"; return RGBL_E_CUDA;
+    }
+    StereoBatchDev s{};
+    s.pyr = c->d_pyr; s.frame_stride = c->frame_bytes; s.levels = c->d_levels;
+    s.kps = c->d_kps; s.desc = c->d_desc; s.n_sel = c->d_n_sel; s.cap = c->cap_kp;
+    s.l0 = l0; s.r0 = r0; s.n_rows = H;
+    for (int l = 0; l < c->tab.nlevels; ++l) { s.scale[l] = c->tab.scale[l]; s.inv_scale[l] = c->tab.inv_scale[l]; }
+    s.mb = mb; s.mbf = mbf;
+    s.depth = c->d_depth; s.uright = c->d_uright;
+    s.row_start = c->d_stereo_row_start; s.row_idx = c->d_stereo_row_idx; s.idx_cap = c->stereo_idx_cap; s.sad = c->d_stereo_sad;
+    stage_begin(c, ST_MATCH, c->st);
+    launch_stereo_matches(c->st, s, n_pairs);
+    stage_end(c, ST_MATCH, c->st, 5);
+    CU(cudaGetLastError());
     return RGBL_OK;
 }
 
@@ -695,7 +718,7 @@ static int upload_rgbl(Ctx* c, int n_frames, const uint8_t* const* gray, int str
     if (gray) { int rc = upload_images(c, n_frames, gray, stride, c->st); if (rc) return rc; }      // else: level 0 was written by decode_png_to_level0
     c->resident_frames = n_frames;
     c->resident_max_pts = max_pts;
-    c->resident_rgbd = false;
+    c->resident_kind = InputKind::rgbl;
     *max_pts_out = max_pts;
     return RGBL_OK;
 }
@@ -813,6 +836,41 @@ static int check_rgbd_params(Ctx* c, float depth_scale, float bf) {
     return RGBL_OK;
 }
 
+// The stereo Frame constructor (src/Frame.cc:101-197) after the n_pairs left images are in slots [0, n) and the right ones in [n, 2n):
+// both extracted as one batch of 2n frames (the reference's two ORBextractor threads), then ComputeStereoMatches.  The left frames are
+// then the batch (last_frames = n) for download, ComputeBoW and the tracking chain.  The capacity-overflow flags cover all 2n frames,
+// so an overflow in a right frame, which changes the left frame's depths, fails the chain's _end2 like a left-frame overflow.
+static int process_stereo(Ctx* c, int n_pairs, float mb, float mbf) {
+    const int max_n = run_extract(c, 2 * n_pairs);
+    if (max_n < 0) return max_n;
+    int rc = stereo_matches(c, 0, n_pairs, n_pairs, mb, mbf); if (rc) return rc;
+    c->last_frames = n_pairs;
+    return max_n;
+}
+
+// what every stereo entry point requires: 2 n_pairs <= max_batch, and a rectified camera (mvKeys of the rectified images are matched;
+// the stereo Frame constructor undistorts nothing before ComputeStereoMatches)
+static int check_stereo(Ctx* c, int n_pairs) {
+    if (2 * n_pairs > c->cfg.max_batch) { c->err = "a stereo batch of n pairs takes 2 n frame slots: 2 n_pairs exceeds max_batch"; return RGBL_E_INVALID; }
+    if (c->undistort) { c->err = "stereo needs rectified images: this context's camera has k1 != 0 (rgbl_set_camera_distortion)"; return RGBL_E_UNSUPPORTED; }
+    return RGBL_OK;
+}
+
+static int check_stereo_params(Ctx* c, float mb, float mbf) {
+    if (!(mb > 0.f) || !std::isfinite(mb) || !(mbf > 0.f) || !std::isfinite(mbf)) { c->err = "mb and mbf must be finite and > 0"; return RGBL_E_INVALID; }
+    return RGBL_OK;
+}
+
+// the uploaded frames must be of `kind`; else the message names the process call that takes them
+static int check_resident_kind(Ctx* c, InputKind kind) {
+    if (c->resident_frames < 1) { c->err = "nothing uploaded"; return RGBL_E_INVALID; }
+    if (c->resident_kind == kind) return RGBL_OK;
+    c->err = c->resident_kind == InputKind::rgbd   ? "the uploaded frames are RGB-D frames (rgbl_resident_process_rgbd)"
+             : c->resident_kind == InputKind::stereo ? "the uploaded frames are stereo pairs (rgbl_resident_process_stereo)"
+                                                     : "the uploaded frames are RGB-L frames (rgbl_resident_process)";
+    return RGBL_E_INVALID;
+}
+
 static int download_rgbl(Ctx* c, int n_frames, rgbl_keypoint* kps, uint8_t* desc, float* depth, float* uright, int cap, int* n_out) {
     { int rc = fetch_counts(c, n_frames); if (rc) return rc; }
     for (int f = 0; f < n_frames; ++f) {
@@ -911,10 +969,9 @@ int rgbl_resident_process(rgbl_ctx* ctx, const float P[12], const rgbl_depth_par
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
     if (!P || !prm) { c->err = "null argument"; return RGBL_E_INVALID; }
-    if (c->resident_frames < 1) { c->err = "nothing uploaded"; return RGBL_E_INVALID; }
-    if (c->resident_rgbd) { c->err = "the uploaded frames are RGB-D frames (rgbl_resident_process_rgbd)"; return RGBL_E_INVALID; }
+    int rc = check_resident_kind(c, InputKind::rgbl); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
-    int rc = process_rgbl(c, c->resident_frames, c->resident_max_pts, P, prm); if (rc < 0) return rc;
+    rc = process_rgbl(c, c->resident_frames, c->resident_max_pts, P, prm); if (rc < 0) return rc;
     if (n_out) { rc = fetch_counts(c, c->resident_frames); if (rc) return rc; }
     CU(cudaStreamSynchronize(c->st));
     CU(cudaStreamSynchronize(c->st_aux));
@@ -929,11 +986,12 @@ int rgbl_resident_process(rgbl_ctx* ctx, const float P[12], const rgbl_depth_par
  * frame construction -> tracking chain (queued two deep on the tracking stream, continue_sequence from the second batch on) -> poses
  * (and, if asked for, the frame-construction outputs) back to the host.  Nothing synchronises with the device until a chain's results
  * are collected, one batch behind.                                                                                                   */
-// device buffers of a stage slot (allocated on first use; a slot can hold RGB-L and later RGB-D batches or the reverse)
-static int stage_slot_alloc(Ctx* c, Ctx::StageSlot& sl, bool rgbd) {
+// device buffers of a stage slot (allocated on first use; a slot can hold batches of each kind in turn)
+static int stage_slot_alloc(Ctx* c, Ctx::StageSlot& sl, InputKind kind) {
     const size_t img_bytes = (size_t)c->levels[0].pitch * c->cfg.height, B = c->cfg.max_batch;
-    const bool ok = ensure(sl.img, B * img_bytes) &&
-                    (rgbd ? ensure(sl.depth, B * depth16_frame_elems(c)) : ensure(sl.pts, B * 4 * c->cfg.max_points) && ensure(sl.n_pts, B));
+    bool ok = ensure(sl.img, B * img_bytes);         // stereo: the left and the right planes, 2 n_pairs <= max_batch
+    if (ok && kind == InputKind::rgbd) ok = ensure(sl.depth, B * depth16_frame_elems(c));
+    if (ok && kind == InputKind::rgbl) ok = ensure(sl.pts, B * 4 * c->cfg.max_points) && ensure(sl.n_pts, B);
     if (!ok) { c->err = "device allocation failed (stage slot)"; return RGBL_E_CUDA; }
     return RGBL_OK;
 }
@@ -950,7 +1008,7 @@ int rgbl_resident_stage(rgbl_ctx* ctx, int slot, int n_frames, const uint8_t* co
     const LevelGeom& l0 = c->levels[0];
     const size_t img_bytes = (size_t)l0.pitch * c->cfg.height, pts_floats = (size_t)4 * c->cfg.max_points;
     Ctx::StageSlot& sl = c->stage[slot];
-    rc = stage_slot_alloc(c, sl, false); if (rc) return rc;
+    rc = stage_slot_alloc(c, sl, InputKind::rgbl); if (rc) return rc;
     int max_pts = 0;
     for (int f = 0; f < n_frames; ++f) {
         if (gray && !gray[f]) { c->err = "empty image"; return RGBL_E_EMPTY; }
@@ -962,7 +1020,7 @@ int rgbl_resident_stage(rgbl_ctx* ctx, int slot, int n_frames, const uint8_t* co
     sl.h_n_pts.assign(n_pts, n_pts + n_frames);
     CU(cudaMemcpyAsync(sl.n_pts, sl.h_n_pts.data(), (size_t)n_frames * sizeof(int), cudaMemcpyHostToDevice, c->st));
     CU(cudaStreamSynchronize(c->st));
-    sl.n_frames = n_frames; sl.max_pts = max_pts; sl.rgbd = false;
+    sl.n_frames = n_frames; sl.max_pts = max_pts; sl.kind = InputKind::rgbl;
     return RGBL_OK;
 }
 
@@ -980,35 +1038,63 @@ int rgbl_resident_stage_rgbd(rgbl_ctx* ctx, int slot, int n_frames, const uint8_
     const LevelGeom& l0 = c->levels[0];
     const size_t img_bytes = (size_t)l0.pitch * c->cfg.height, dep = depth16_frame_elems(c);
     Ctx::StageSlot& sl = c->stage[slot];
-    rc = stage_slot_alloc(c, sl, true); if (rc) return rc;
+    rc = stage_slot_alloc(c, sl, InputKind::rgbd); if (rc) return rc;
     for (int f = 0; f < n_frames; ++f) {
         CU(cudaMemcpy2DAsync(sl.img + (size_t)f * img_bytes, l0.pitch, gray[f], stride, c->cfg.width, c->cfg.height, cudaMemcpyHostToDevice, c->st));
         CU(cudaMemcpy2DAsync(sl.depth + (size_t)f * dep, c->depth16_pitch * sizeof(uint16_t), depth[f], (size_t)depth_stride * sizeof(uint16_t),
                              (size_t)c->cfg.width * sizeof(uint16_t), c->cfg.height, cudaMemcpyHostToDevice, c->st));
     }
     CU(cudaStreamSynchronize(c->st));
-    sl.n_frames = n_frames; sl.max_pts = 0; sl.rgbd = true;
+    sl.n_frames = n_frames; sl.max_pts = 0; sl.kind = InputKind::rgbd;
+    return RGBL_OK;
+}
+
+int rgbl_resident_stage_stereo(rgbl_ctx* ctx, int slot, int n_pairs, const uint8_t* const* left, const uint8_t* const* right, int width, int height,
+                               int stride) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return RGBL_E_INVALID;
+    if (!left || !right) { c->err = "null argument"; return RGBL_E_INVALID; }
+    if (slot < 0 || slot >= Ctx::kMaxStageSlots) { c->err = "stage slot out of range"; return RGBL_E_INVALID; }
+    int rc = check_batch_args(c, n_pairs, width, height, stride); if (rc) return rc;
+    rc = check_stereo(c, n_pairs); if (rc) return rc;
+    for (int f = 0; f < n_pairs; ++f) if (!left[f] || !right[f]) { c->err = "empty image"; return RGBL_E_EMPTY; }
+    CU(cudaSetDevice(c->cfg.device));
+    const LevelGeom& l0 = c->levels[0];
+    const size_t img_bytes = (size_t)l0.pitch * c->cfg.height;
+    Ctx::StageSlot& sl = c->stage[slot];
+    rc = stage_slot_alloc(c, sl, InputKind::stereo); if (rc) return rc;
+    for (int f = 0; f < 2 * n_pairs; ++f)
+        CU(cudaMemcpy2DAsync(sl.img + (size_t)f * img_bytes, l0.pitch, f < n_pairs ? left[f] : right[f - n_pairs], stride, c->cfg.width, c->cfg.height,
+                             cudaMemcpyHostToDevice, c->st));
+    CU(cudaStreamSynchronize(c->st));
+    sl.n_frames = n_pairs; sl.max_pts = 0; sl.kind = InputKind::stereo;
     return RGBL_OK;
 }
 
 // staged slot -> the context's working input buffers (device-to-device, ~76 MB per 32 KITTI frames: tens of microseconds); the slot must hold
 // frames of the kind the caller processes
-static int restage(Ctx* c, int slot, bool rgbd) {
+static int restage(Ctx* c, int slot, InputKind kind) {
     const Ctx::StageSlot& sl = c->stage[slot];
     if (!sl.img || sl.n_frames < 1) { c->err = "stage slot is empty"; return RGBL_E_INVALID; }
-    if (sl.rgbd != rgbd) { c->err = sl.rgbd ? "stage slot holds RGB-D frames (rgbl_track_sequence_rgbd)" : "stage slot holds RGB-L frames (rgbl_track_sequence)"; return RGBL_E_INVALID; }
+    if (sl.kind != kind) {
+        c->err = sl.kind == InputKind::rgbd   ? "stage slot holds RGB-D frames (rgbl_track_sequence_rgbd)"
+                 : sl.kind == InputKind::stereo ? "stage slot holds stereo pairs (rgbl_track_sequence_stereo)"
+                                                : "stage slot holds RGB-L frames (rgbl_track_sequence)";
+        return RGBL_E_INVALID;
+    }
     const LevelGeom& l0 = c->levels[0];
     const size_t img_bytes = (size_t)l0.pitch * c->cfg.height, pts_floats = (size_t)4 * c->cfg.max_points;
-    for (int f = 0; f < sl.n_frames; ++f)
+    const int n_img = kind == InputKind::stereo ? 2 * sl.n_frames : sl.n_frames;
+    for (int f = 0; f < n_img; ++f)
         CU(cudaMemcpyAsync(c->d_pyr + (size_t)f * c->frame_bytes + l0.off, sl.img + (size_t)f * img_bytes, img_bytes, cudaMemcpyDeviceToDevice, c->st));
-    if (rgbd) {
+    if (kind == InputKind::rgbd) {
         CU(cudaMemcpyAsync(c->d_depth16, sl.depth, (size_t)sl.n_frames * depth16_frame_elems(c) * sizeof(uint16_t), cudaMemcpyDeviceToDevice, c->st_aux));
-    } else {
+    } else if (kind == InputKind::rgbl) {
         CU(cudaMemcpyAsync(c->d_pts, sl.pts, (size_t)sl.n_frames * pts_floats * sizeof(float), cudaMemcpyDeviceToDevice, c->st_aux));
         CU(cudaMemcpyAsync(c->d_n_pts, sl.n_pts, (size_t)sl.n_frames * sizeof(int), cudaMemcpyDeviceToDevice, c->st_aux));
         for (int f = 0; f < sl.n_frames; ++f) c->h_n_pts[f] = sl.h_n_pts[f];
     }
-    c->resident_frames = sl.n_frames; c->resident_max_pts = sl.max_pts; c->resident_rgbd = rgbd;
+    c->resident_frames = sl.n_frames; c->resident_max_pts = sl.max_pts; c->resident_kind = kind;
     return RGBL_OK;
 }
 
@@ -1083,7 +1169,7 @@ int rgbl_track_sequence(rgbl_ctx* ctx, const float P[12], const rgbl_depth_param
     int max_pts = 0;
     auto load = [&](int b) -> int {
         if (io->gray) return upload_rgbl(c, T, io->gray + (size_t)b * T, io->stride, io->pts4xn + (size_t)b * T, io->n_pts + (size_t)b * T, &max_pts);
-        const int r = restage(c, (io->first_slot + b) % io->n_slots, false);
+        const int r = restage(c, (io->first_slot + b) % io->n_slots, InputKind::rgbl);
         max_pts = c->resident_max_pts;
         return r;
     };
@@ -1101,14 +1187,36 @@ int rgbl_track_sequence_rgbd(rgbl_ctx* ctx, float depth_scale, float bf, const r
     CU(cudaSetDevice(c->cfg.device));
     const int T = io->frames_per_batch;
     auto load = [&](int b) -> int {
-        if (!io->gray) return restage(c, (io->first_slot + b) % io->n_slots, true);
+        if (!io->gray) return restage(c, (io->first_slot + b) % io->n_slots, InputKind::rgbd);
         for (int f = 0; f < T; ++f) if (!io->gray[(size_t)b * T + f]) { c->err = "empty image"; return RGBL_E_EMPTY; }
         int r = upload_depth16(c, T, depth + (size_t)b * T, depth_stride, c->st_aux); if (r) return r;
         r = upload_images(c, T, io->gray + (size_t)b * T, io->stride, c->st); if (r) return r;
-        c->resident_frames = T; c->resident_max_pts = 0; c->resident_rgbd = true;
+        c->resident_frames = T; c->resident_max_pts = 0; c->resident_kind = InputKind::rgbd;
         return RGBL_OK;
     };
     return run_sequence(c, chain, io, load, [&]() { return process_rgbd(c, T, depth_scale, bf); });
+}
+
+int rgbl_track_sequence_stereo(rgbl_ctx* ctx, float mb, float mbf, const rgbl_chain_params* chain, const rgbl_sequence_io* io, const uint8_t* const* right) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return RGBL_E_INVALID;
+    int rc = check_sequence_io(c, chain, io); if (rc) return rc;
+    rc = check_stereo_params(c, mb, mbf); if (rc) return rc;
+    rc = check_stereo(c, io->frames_per_batch); if (rc) return rc;
+    if (io->pts4xn || io->n_pts) { c->err = "stereo sequences take right images, not point clouds (pts4xn / n_pts must be NULL)"; return RGBL_E_INVALID; }
+    if (io->gray && !right) { c->err = "host mode needs one right image per frame"; return RGBL_E_INVALID; }
+    CU(cudaSetDevice(c->cfg.device));
+    const int T = io->frames_per_batch;
+    auto load = [&](int b) -> int {
+        if (!io->gray) return restage(c, (io->first_slot + b) % io->n_slots, InputKind::stereo);
+        const size_t o = (size_t)b * T;
+        for (int f = 0; f < T; ++f) if (!io->gray[o + f] || !right[o + f]) { c->err = "empty image"; return RGBL_E_EMPTY; }
+        int r = upload_images(c, T, io->gray + o, io->stride, c->st); if (r) return r;
+        r = upload_images(c, T, right + o, io->stride, c->st, T); if (r) return r;
+        c->resident_frames = T; c->resident_max_pts = 0; c->resident_kind = InputKind::stereo;
+        return RGBL_OK;
+    };
+    return run_sequence(c, chain, io, load, [&]() { return process_stereo(c, T, mb, mbf); });
 }
 
 // ---- RGB-D frame construction (resident form) ----
@@ -1124,7 +1232,7 @@ int rgbl_resident_upload_rgbd(rgbl_ctx* ctx, int n_frames, const uint8_t* const*
     rc = upload_images(c, n_frames, gray, stride, c->st); if (rc) return rc;
     CU(cudaStreamSynchronize(c->st));
     CU(cudaStreamSynchronize(c->st_aux));
-    c->resident_frames = n_frames; c->resident_max_pts = 0; c->resident_rgbd = true;
+    c->resident_frames = n_frames; c->resident_max_pts = 0; c->resident_kind = InputKind::rgbd;
     return RGBL_OK;
 }
 
@@ -1137,7 +1245,7 @@ int rgbl_resident_upload_rgbd_png(rgbl_ctx* ctx, int n_frames, const uint8_t* co
     CU(cudaSetDevice(c->cfg.device));
     rc = decode_png_to_level0(c, n_frames, png, png_bytes, camera_rgb, c->st); if (rc) return rc;
     rc = decode_png_to_depth16(c, n_frames, depth_png, depth_png_bytes, c->st); if (rc) return rc;
-    c->resident_frames = n_frames; c->resident_max_pts = 0; c->resident_rgbd = true;
+    c->resident_frames = n_frames; c->resident_max_pts = 0; c->resident_kind = InputKind::rgbd;
     return RGBL_OK;
 }
 
@@ -1159,10 +1267,60 @@ int rgbl_decode_png_depth16(rgbl_ctx* ctx, int n_frames, const uint8_t* const* p
 int rgbl_resident_process_rgbd(rgbl_ctx* ctx, float depth_scale, float bf, int* n_out) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
-    if (c->resident_frames < 1 || !c->resident_rgbd) { c->err = "no RGB-D frames uploaded (rgbl_resident_upload_rgbd / _rgbd_png)"; return RGBL_E_INVALID; }
-    int rc = check_rgbd_params(c, depth_scale, bf); if (rc) return rc;
+    int rc = check_resident_kind(c, InputKind::rgbd); if (rc) return rc;
+    rc = check_rgbd_params(c, depth_scale, bf); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     rc = process_rgbd(c, c->resident_frames, depth_scale, bf); if (rc < 0) return rc;
+    if (n_out) { rc = fetch_counts(c, c->resident_frames); if (rc) return rc; }
+    CU(cudaStreamSynchronize(c->st));
+    CU(cudaStreamSynchronize(c->st_aux));
+    prof_collect(c);
+    if (n_out) for (int f = 0; f < c->resident_frames; ++f) n_out[f] = c->h_n_sel[f];
+    return RGBL_OK;
+}
+
+// ---- stereo frame construction (resident form): n pairs = one batch of 2n frames, left images in slots [0, n), right ones in [n, 2n) ----
+int rgbl_resident_upload_stereo(rgbl_ctx* ctx, int n_pairs, const uint8_t* const* left, const uint8_t* const* right, int width, int height, int stride) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return RGBL_E_INVALID;
+    if (!left || !right) { c->err = "null argument"; return RGBL_E_INVALID; }
+    int rc = check_batch_args(c, n_pairs, width, height, stride); if (rc) return rc;
+    rc = check_stereo(c, n_pairs); if (rc) return rc;
+    for (int f = 0; f < n_pairs; ++f) if (!left[f] || !right[f]) { c->err = "empty image"; return RGBL_E_EMPTY; }
+    CU(cudaSetDevice(c->cfg.device));
+    rc = upload_images(c, n_pairs, left, stride, c->st); if (rc) return rc;
+    rc = upload_images(c, n_pairs, right, stride, c->st, n_pairs); if (rc) return rc;
+    CU(cudaStreamSynchronize(c->st));
+    c->resident_frames = n_pairs; c->resident_max_pts = 0; c->resident_kind = InputKind::stereo;
+    return RGBL_OK;
+}
+
+int rgbl_resident_upload_stereo_png(rgbl_ctx* ctx, int n_pairs, const uint8_t* const* left_png, const size_t* left_bytes, const uint8_t* const* right_png,
+                                    const size_t* right_bytes, int camera_rgb) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return RGBL_E_INVALID;
+    if (!left_png || !left_bytes || !right_png || !right_bytes) { c->err = "null argument"; return RGBL_E_INVALID; }
+    int rc = check_batch_args(c, n_pairs, c->cfg.width, c->cfg.height, c->cfg.width); if (rc) return rc;
+    rc = check_stereo(c, n_pairs); if (rc) return rc;
+    CU(cudaSetDevice(c->cfg.device));
+    // one decode of 2n streams: every stream must have the context's size, so left and right sizes that differ are an error
+    std::vector<const uint8_t*> png(left_png, left_png + n_pairs);
+    std::vector<size_t> bytes(left_bytes, left_bytes + n_pairs);
+    png.insert(png.end(), right_png, right_png + n_pairs);
+    bytes.insert(bytes.end(), right_bytes, right_bytes + n_pairs);
+    rc = decode_png_to_level0(c, 2 * n_pairs, png.data(), bytes.data(), camera_rgb, c->st); if (rc) return rc;
+    c->resident_frames = n_pairs; c->resident_max_pts = 0; c->resident_kind = InputKind::stereo;
+    return RGBL_OK;
+}
+
+int rgbl_resident_process_stereo(rgbl_ctx* ctx, float mb, float mbf, int* n_out) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return RGBL_E_INVALID;
+    int rc = check_resident_kind(c, InputKind::stereo); if (rc) return rc;
+    rc = check_stereo_params(c, mb, mbf); if (rc) return rc;
+    rc = check_stereo(c, c->resident_frames); if (rc) return rc;
+    CU(cudaSetDevice(c->cfg.device));
+    rc = process_stereo(c, c->resident_frames, mb, mbf); if (rc < 0) return rc;
     if (n_out) { rc = fetch_counts(c, c->resident_frames); if (rc) return rc; }
     CU(cudaStreamSynchronize(c->st));
     CU(cudaStreamSynchronize(c->st_aux));

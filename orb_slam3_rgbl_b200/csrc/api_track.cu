@@ -323,21 +323,11 @@ int rgbl_stereo_matches(rgbl_ctx* ctx, int slot_left, int slot_right, float mb, 
     if (c->chain_pending) { c->err = "a tracking chain is in flight (rgbl_resident_track_end not called)"; return RGBL_E_INVALID; }
     if (!depth || !uright) { c->err = "null argument"; return RGBL_E_INVALID; }
     if (slot_left < 0 || slot_right < 0 || slot_left >= c->last_frames || slot_right >= c->last_frames) { c->err = "frame slot out of range (extract the stereo pair as one batch first)"; return RGBL_E_INVALID; }
-    if (c->cap_kp > 65535) { c->err = "more than 65535 keypoints per frame"; return RGBL_E_UNSUPPORTED; }
     CU(cudaSetDevice(c->cfg.device));
-    TrackBufs& t = c->trk;
-    GROW(t.e_idx, c->cap_kp);
-    StereoFrameDev L{}, R{};
-    L.n = c->d_n_sel + slot_left; L.keys = c->d_kps + (size_t)slot_left * c->cap_kp; L.desc = c->d_desc + (size_t)slot_left * c->cap_kp * 32;
-    R.n = c->d_n_sel + slot_right; R.keys = c->d_kps + (size_t)slot_right * c->cap_kp; R.desc = c->d_desc + (size_t)slot_right * c->cap_kp * 32;
-    for (int l = 0; l < c->tab.nlevels; ++l) { L.scale[l] = R.scale[l] = c->tab.scale[l]; L.inv_scale[l] = R.inv_scale[l] = c->tab.inv_scale[l]; }
+    int rc = stereo_matches(c, slot_left, slot_right, 1, mb, mbf); if (rc) return rc;
     float* d_depth = c->d_depth + (size_t)slot_left * c->cap_kp;
     float* d_ur = c->d_uright + (size_t)slot_left * c->cap_kp;
-    stage_begin(c, ST_MATCH, c->st);
-    launch_stereo_matches(c->st, c->d_pyr, c->frame_bytes, slot_left, slot_right, c->d_levels, L, R, mb, mbf, c->cfg.height, c->cap_kp, d_depth, d_ur, t.e_idx);
-    stage_end(c, ST_MATCH, c->st, 2);
-    CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(c->h_scalars, L.n, sizeof(int), cudaMemcpyDeviceToHost, c->st));
+    CU(cudaMemcpyAsync(c->h_scalars, c->d_n_sel + slot_left, sizeof(int), cudaMemcpyDeviceToHost, c->st));
     CU(cudaStreamSynchronize(c->st));
     const int n = c->h_scalars[0];
     if (n > cap) { c->err = "output capacity too small"; return RGBL_E_CAPACITY; }

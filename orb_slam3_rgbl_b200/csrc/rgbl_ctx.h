@@ -17,6 +17,10 @@ static const char* const kStageNames[kNumStages] = {"pyramid", "fast", "compact"
 
 constexpr int kMatchListCap = 512;    // admissible candidates kept per map point (overflow is reported)
 
+// the inputs of a resident upload or a staged slot: RGB-L (image + point cloud), RGB-D (image + uint16 depth plane), stereo (left and
+// right image of a rectified pair)
+enum class InputKind { rgbl, rgbd, stereo };
+
 // Lazily grown device scratch of the tracking entry points (api_track.cu).
 struct TrackBufs {
     DeviceArray<rgbl_keypoint> keys; DeviceArray<float> uright; DeviceArray<uint8_t> desc, state;
@@ -84,6 +88,11 @@ struct Ctx {
     // depth16_pitch elements (64-byte rows); scaled to metric depth by the gather
     DeviceArray<uint16_t> d_depth16;
     size_t depth16_pitch = 0;
+    // Frame::ComputeStereoMatches scratch (lazily allocated by the first stereo call, sized once for max(1, max_batch / 2) pairs): per
+    // pair the row index (row starts, row lists of stereo_row_index_cap entries) and the matched SADs.  Never reallocated and never
+    // referenced by the chain's CUDA graphs, so it needs no scratch_generation bump.
+    DeviceArray<int> d_stereo_row_start, d_stereo_row_idx, d_stereo_sad;
+    int stereo_idx_cap = 0;
     DeviceArray<int> d_n_pts;
     DeviceArray<uint32_t> d_idx_map;
     DeviceArray<float> d_raw, d_processed, d_depth, d_uright;
@@ -158,9 +167,10 @@ struct Ctx {
     bool chain_timing_recorded = false;      // RGBL_CHAIN_TIMING development aid: chain_tev hold the timings of a chain
 
     // staged input slots of the sequence runners (rgbl_resident_stage / rgbl_track_sequence, rgbl_resident_stage_rgbd /
-    // rgbl_track_sequence_rgbd): level-0 planes + clouds (RGB-L) or uint16 depth planes (RGB-D) of whole batches
+    // rgbl_track_sequence_rgbd, rgbl_resident_stage_stereo / rgbl_track_sequence_stereo): level-0 planes + clouds (RGB-L), uint16 depth
+    // planes (RGB-D) or the left then the right level-0 planes (stereo: n_frames pairs, 2 n_frames planes) of whole batches
     static constexpr int kMaxStageSlots = 8;
-    struct StageSlot { DeviceArray<uint8_t> img; DeviceArray<float> pts; DeviceArray<int> n_pts; DeviceArray<uint16_t> depth; std::vector<int> h_n_pts; int n_frames = 0, max_pts = 0; bool rgbd = false; };
+    struct StageSlot { DeviceArray<uint8_t> img; DeviceArray<float> pts; DeviceArray<int> n_pts; DeviceArray<uint16_t> depth; std::vector<int> h_n_pts; int n_frames = 0, max_pts = 0; InputKind kind = InputKind::rgbl; };
     StageSlot stage[kMaxStageSlots];
 
     // camera model of Frame::UndistortKeyPoints / ComputeImageBounds (rgbl_set_camera_distortion): undistort = (k1 != 0); cam_bounds =
@@ -174,8 +184,8 @@ struct Ctx {
     float frame_bounds[4] = {};
 
     int last_frames = 0;         // frames valid in the device buffers
-    int resident_frames = 0, resident_max_pts = 0;
-    bool resident_rgbd = false;  // the uploaded frames are RGB-D frames (image + depth plane), not RGB-L ones
+    int resident_frames = 0, resident_max_pts = 0;   // stereo: resident_frames pairs in slots [0, 2 resident_frames)
+    InputKind resident_kind = InputKind::rgbl;      // what the uploaded frames are
     bool blur_valid = false;
 };
 
@@ -205,6 +215,10 @@ struct ArenaCarve {
 void stage_begin(Ctx* c, int stage, cudaStream_t st);
 void stage_end(Ctx* c, int stage, cudaStream_t st, int launches);
 void prof_collect(Ctx* c);
+
+// Frame::ComputeStereoMatches for the pairs (l0 + p, r0 + p), p < n_pairs, of the last batched extraction, on the main stream and billed to
+// the match stage (api.cu): mvDepth / mvuRight of the left slots in d_depth / d_uright.  Allocates the stereo scratch on first use.
+int stereo_matches(Ctx* c, int l0, int r0, int n_pairs, float mb, float mbf);
 
 }  // namespace rgbl
 #endif

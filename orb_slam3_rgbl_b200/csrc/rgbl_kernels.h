@@ -206,10 +206,21 @@ struct ChainTlmTail {
 int tlm_lookback_ints();
 
 // stereo_kernels.cu --------------------------------------------------------------------------------
-struct StereoFrameDev { const int* n; const rgbl_keypoint* keys; const uint8_t* desc; float scale[RGBL_MAX_LEVELS], inv_scale[RGBL_MAX_LEVELS]; };
-void launch_stereo_matches(cudaStream_t st, const uint8_t* pyr, size_t frame_stride, int slot_l, int slot_r, const LevelGeom* d_levels,
-                           const StereoFrameDev& L, const StereoFrameDev& R, float mb, float mbf, int n_rows, int cap, float* depth,
-                           float* uright, int* sad);
+// Frame::ComputeStereoMatches for n_pairs pairs of frame slots of one batched extraction: pair p = (left slot l0 + p, right slot r0 + p).
+// Keypoints, descriptors and counts are the batch's [slot][cap] outputs; mvDepth / mvuRight of the left slot are written in place.
+struct StereoBatchDev {
+    const uint8_t* pyr; size_t frame_stride; const LevelGeom* levels;
+    const rgbl_keypoint* kps; const uint8_t* desc; const int* n_sel; int cap;
+    int l0, r0, n_rows;
+    float scale[RGBL_MAX_LEVELS], inv_scale[RGBL_MAX_LEVELS];
+    float mb, mbf;
+    float* depth; float* uright;
+    // scratch, per pair: row_start [n_rows + 1] (vRowIndices as CSR), row_idx [idx_cap], sad [cap]
+    int* row_start; int* row_idx; int idx_cap; int* sad;
+};
+// row_idx entries one pair needs at most: a right keypoint of octave o is listed in ceil(y + r) - floor(y - r) + 1 <= 2r + 4 rows, r = 2 scale[o]
+int stereo_row_index_cap(int cap, const float* scale, int n_levels, int n_rows);
+void launch_stereo_matches(cudaStream_t st, const StereoBatchDev& s, int n_pairs);
 
 // pose_kernels.cu ----------------------------------------------------------------------------------
 struct PoseProblemDev {

@@ -694,6 +694,55 @@ class RgbdBatch:
     track_end2 = RgblBatch.track_end2
 
 
+class StereoBatch:
+    """Host buffers of one batch of rectified stereo pairs for the resident stereo API: the stereo Frame constructor (src/Frame.cc:101-197)
+    is upload + process_resident (the 2n images extracted as one batch, then ComputeStereoMatches, ctx.max_batch >= 2n); download /
+    download_keys_un / track_begin2 / track_end2 then see the left frames, as for RgblBatch."""
+
+    def __init__(self, ctx: Context, lefts, rights, pinned=True):
+        self.ctx = ctx
+        nF = len(lefts); cap = ctx.cap
+        self.nF, self.cap = nF, cap
+        alloc = _pinned_alloc if pinned else (lambda shape, dt: np.empty(shape, dt))
+        H, W = lefts[0].shape
+        self.W, self.H = W, H
+        self.left = alloc((nF, H, W), np.uint8); self.right = alloc((nF, H, W), np.uint8)
+        self.set_inputs(lefts, rights)
+        self.la = (C.c_void_p * nF)(*[self.left[f].ctypes.data for f in range(nF)])
+        self.ra = (C.c_void_p * nF)(*[self.right[f].ctypes.data for f in range(nF)])
+        self.kps = alloc((nF, cap), KP_DTYPE); self.desc = alloc((nF, cap, 32), np.uint8)
+        self.depth = alloc((nF, cap), np.float32); self.uright = alloc((nF, cap), np.float32)
+        self.n = np.zeros(nF, np.int32)
+
+    def set_inputs(self, lefts, rights):
+        assert len(lefts) == self.nF and len(rights) == self.nF
+        for f in range(self.nF):
+            self.left[f] = lefts[f]; self.right[f] = rights[f]
+
+    def upload(self):
+        c = self.ctx
+        check(lib().rgbl_resident_upload_stereo(c.handle, self.nF, self.la, self.ra, self.W, self.H, self.W), c.handle)
+
+    def upload_png(self, left_pngs, right_pngs, camera_rgb=True):
+        """Resident upload of the files' bytes (KITTI image_0 / image_1 PNGs: imread + cvtColor to gray on the way)."""
+        c = self.ctx
+        lb = [np.frombuffer(b, np.uint8) for b in left_pngs]; rb = [np.frombuffer(b, np.uint8) for b in right_pngs]
+        la = (C.c_void_p * self.nF)(*[b.ctypes.data for b in lb]); ra = (C.c_void_p * self.nF)(*[b.ctypes.data for b in rb])
+        ls = (C.c_size_t * self.nF)(*[len(b) for b in lb]); rs = (C.c_size_t * self.nF)(*[len(b) for b in rb])
+        check(lib().rgbl_resident_upload_stereo_png(c.handle, self.nF, la, ls, ra, rs, int(bool(camera_rgb))), c.handle)
+
+    def process_resident(self, mb: float, mbf: float):
+        """mb = mbf / fx, mbf = Camera.bf -> keypoints per left frame"""
+        c = self.ctx
+        check(lib().rgbl_resident_process_stereo(c.handle, mb, mbf, ptr(self.n)), c.handle)
+        return self.n
+
+    download = RgblBatch.download
+    download_keys_un = RgblBatch.download_keys_un
+    track_begin2 = RgblBatch.track_begin2
+    track_end2 = RgblBatch.track_end2
+
+
 class SequenceIO(C.Structure):
     """rgbl_sequence_io (include/rgbl_b200.h)."""
     _fields_ = [("n_batches", C.c_int), ("frames_per_batch", C.c_int), ("width", C.c_int), ("height", C.c_int), ("stride", C.c_int),
@@ -716,7 +765,7 @@ class SequenceRunner:
         self.P = np.ascontiguousarray(P, np.float32).reshape(12)
         self.prm = depth_params
         self._out = None
-        self.rgbd_mode = False
+        self.kind = "rgbl"
 
     @classmethod
     def rgbd(cls, ctx: Context, depth_scale: float, bf: float, T: int, W: int, H: int, n_host_batches: int, pinned=True) -> "SequenceRunner":
@@ -729,14 +778,29 @@ class SequenceRunner:
         self.dep = self._alloc((self.M, T, H, W), np.uint16)
         self.depth_scale, self.bf = float(depth_scale), float(bf)
         self._out = None
-        self.rgbd_mode = True
+        self.kind = "rgbd"
+        return self
+
+    @classmethod
+    def stereo(cls, ctx: Context, mb: float, mbf: float, T: int, W: int, H: int, n_host_batches: int, pinned=True) -> "SequenceRunner":
+        """Stereo mode (rgbl_track_sequence_stereo, the loop of Examples/Stereo/stereo_kitti.cc): batches of T rectified pairs, extracted as
+        batches of 2T frames (ctx.max_batch >= 2T); set_batch(m, lefts, rights).  mb = mbf / fx, mbf = Camera.bf."""
+        self = cls.__new__(cls)
+        self.ctx, self.T, self.W, self.H, self.M, self.maxn = ctx, T, W, H, n_host_batches, 0
+        self._alloc = _pinned_alloc if pinned else (lambda shape, dt: np.empty(shape, dt))
+        self.img = self._alloc((self.M, T, H, W), np.uint8)
+        self.right = self._alloc((self.M, T, H, W), np.uint8)
+        self.mb, self.mbf = float(mb), float(mbf)
+        self._out = None
+        self.kind = "stereo"
         return self
 
     def set_batch(self, m: int, images, clouds):
-        """clouds: 4 x N point clouds (RGB-L), or the uint16 depth images in RGB-D mode."""
-        if self.rgbd_mode:
+        """clouds: 4 x N point clouds (RGB-L), the uint16 depth images in RGB-D mode, or the right images in stereo mode."""
+        if self.kind != "rgbl":
+            other = self.dep if self.kind == "rgbd" else self.right
             for f in range(self.T):
-                self.img[m, f] = images[f]; self.dep[m, f] = np.asarray(clouds[f], np.uint16)
+                self.img[m, f] = images[f]; other[m, f] = np.asarray(clouds[f], other.dtype)
             return
         for f in range(self.T):
             self.img[m, f] = images[f]
@@ -745,9 +809,13 @@ class SequenceRunner:
             self.npts[m, f] = n
 
     def stage(self, slot: int, m: int):
-        """Upload host batch m into device slot `slot` (rgbl_resident_stage / rgbl_resident_stage_rgbd)."""
+        """Upload host batch m into device slot `slot` (rgbl_resident_stage / _stage_rgbd / _stage_stereo)."""
         ia = (C.c_void_p * self.T)(*[self.img[m, f].ctypes.data for f in range(self.T)])
-        if self.rgbd_mode:
+        if self.kind == "stereo":
+            ra = (C.c_void_p * self.T)(*[self.right[m, f].ctypes.data for f in range(self.T)])
+            check(lib().rgbl_resident_stage_stereo(self.ctx.handle, slot, self.T, ia, ra, self.W, self.H, self.W), self.ctx.handle)
+            return
+        if self.kind == "rgbd":
             da = (C.c_void_p * self.T)(*[self.dep[m, f].ctypes.data for f in range(self.T)])
             check(lib().rgbl_resident_stage_rgbd(self.ctx.handle, slot, self.T, ia, self.W, self.H, self.W, da, self.W), self.ctx.handle)
             return
@@ -783,10 +851,11 @@ class SequenceRunner:
         da = None
         if resident_slots > 0:
             io.gray = None; io.pts4xn = None; io.n_pts = None; io.n_slots = resident_slots; io.first_slot = first % resident_slots
-        elif self.rgbd_mode:
+        elif self.kind != "rgbl":
             idx = [(first + b) % self.M for b in range(n_batches)]
+            other = self.dep if self.kind == "rgbd" else self.right
             ga = (C.c_void_p * (n_batches * T))(*[self.img[m, f].ctypes.data for m in idx for f in range(T)])
-            da = (C.c_void_p * (n_batches * T))(*[self.dep[m, f].ctypes.data for m in idx for f in range(T)])
+            da = (C.c_void_p * (n_batches * T))(*[other[m, f].ctypes.data for m in idx for f in range(T)])
             keep += [ga, da]
             io.gray = C.cast(ga, C.c_void_p); io.pts4xn = None; io.n_pts = None
         else:
@@ -801,15 +870,17 @@ class SequenceRunner:
         if want_frames:
             io.kps = o["kps"].ctypes.data; io.desc = o["desc"].ctypes.data; io.depth = o["depth"].ctypes.data; io.uright = o["uright"].ctypes.data
             io.cap = self.ctx.cap; io.n_kp = o["n_kp"].ctypes.data
-        if self.rgbd_mode:
+        if self.kind == "stereo":
+            check(lib().rgbl_track_sequence_stereo(self.ctx.handle, self.mb, self.mbf, C.byref(chain), C.byref(io), da), self.ctx.handle)
+        elif self.kind == "rgbd":
             check(lib().rgbl_track_sequence_rgbd(self.ctx.handle, self.depth_scale, self.bf, C.byref(chain), C.byref(io), da, self.W), self.ctx.handle)
         else:
             check(lib().rgbl_track_sequence(self.ctx.handle, ptr(self.P), C.byref(self.prm), C.byref(chain), C.byref(io)), self.ctx.handle)
         return o
 
     def h2d_bytes_per_batch(self) -> float:
-        if self.rgbd_mode:
-            return float(self.T * self.W * self.H * 3)
+        if self.kind != "rgbl":
+            return float(self.T * self.W * self.H * (3 if self.kind == "rgbd" else 2))
         return float(self.T * self.W * self.H + 16.0 * self.npts.sum() / self.M)
 
     def d2h_bytes_per_batch(self, want_frames: bool) -> float:

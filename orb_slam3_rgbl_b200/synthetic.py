@@ -194,6 +194,23 @@ class PlaneSequence:
         bot = tex[y0 + 1, x0] * (1 - fx) + tex[y0 + 1, x0 + 1] * fx
         return np.ascontiguousarray(np.clip(np.rint(top * (1 - fy) + bot * fy), 0, 255).astype(np.uint8))
 
+    def disparity_px(self) -> int:
+        """Disparity of the plane in a rectified stereo rig with baseline bf / fx: bf / Z pixels (5 at the defaults)."""
+        d = self.cam[4] / self.Z
+        if self.dist is not None:
+            raise ValueError("right_image needs a pinhole camera: stereo pairs are rectified, this sequence has a distortion model")
+        if abs(d - round(d)) > 1e-9:
+            raise ValueError(f"right_image needs a whole-pixel disparity bf / Z, got {d} px")
+        if round(d) > self.shift + 8:
+            raise ValueError(f"disparity {d} px exceeds the texture's slack of shift_px + 8 = {self.shift + 8} px beyond the last crop")
+        return int(round(d))
+
+    def right_image(self, t: int) -> np.ndarray:
+        """Frame t of the right camera of a rectified stereo rig (baseline bf / fx along +x): the plane point at left pixel u appears at
+        u - d, d = bf / Z, so the view is the texture crop of image(t) shifted by d columns."""
+        s, d = self.step_index(t), self.disparity_px()
+        return np.ascontiguousarray(self.texture[:, s * self.shift + d: s * self.shift + d + self.W])
+
     def pose(self, t: int) -> np.ndarray:
         """Tcw as (qx, qy, qz, qw, tx, ty, tz): identity rotation, camera centre at x = step_index(t) * dX."""
         return np.array([0, 0, 0, 1, -self.step_index(t) * self.dX, 0, 0], np.float32)
