@@ -436,6 +436,19 @@ int rgbl_resident_stage_stereo(rgbl_ctx* ctx, int slot, int n_pairs, const uint8
  * images) takes right[] (one per frame of the call), resident mode takes slots staged with rgbl_resident_stage_stereo (a slot of another
  * kind is RGBL_E_INVALID, and so is a stereo slot given to the other runners).                                                          */
 int rgbl_track_sequence_stereo(rgbl_ctx* ctx, float mb, float mbf, const rgbl_chain_params* chain, const rgbl_sequence_io* io, const uint8_t* const* right);
+/* Stereo rectification on the device: the cv::remap(im, imRect, M1, M2, INTER_LINEAR) that System::TrackStereo runs on both images before
+ * GrabImageStereo when Settings::needToRectify() (src/System.cc:251 ff.; BORDER_CONSTANT 0, bit-exact with OpenCV).  m1l / m2l / m1r / m2r
+ * are Settings' M1l, M2l, M1r, M2r (cv::initUndistortRectifyMap, CV_32F): H x W float32 maps at the context's size, row stride map_stride
+ * floats.  They are converted once to OpenCV's fixed-point form on the device.  All four NULL turns rectification off (the default); a
+ * partial set of NULLs, map_stride < width or a value that is not finite is RGBL_E_INVALID and the previous setting stays.
+ * While rectification is on, the stereo entry points take the RAW images at the context's size (Settings without resize): uploads and
+ * PNG decodes keep them in raw planes, staged slots hold them as they always do, and rgbl_resident_process_stereo / the stereo runner
+ * remap both images of every pair into level 0 before the extraction, billed to the `pyramid` profiling stage.  PNG streams must then
+ * be 8-bit gray (colour: RGBL_E_UNSUPPORTED, since the reference remaps before its conversion to gray).  The camera model
+ * (rgbl_set_camera_distortion) keeps describing the rectified images, so it stays k1 = 0; mb / mbf and the chain's camera are the
+ * rectified ones (Settings: P1's intrinsics, bf = b * P1(0,0)).  Setting or clearing the maps discards a pending stereo upload (the process
+ * call then reports "nothing uploaded"); staged slots stay valid.                                                                       */
+int rgbl_set_stereo_rectification(rgbl_ctx* ctx, const float* m1l, const float* m2l, const float* m1r, const float* m2r, int map_stride);
 
 /* ---- Camera model of Frame::UndistortKeyPoints / ComputeImageBounds (src/Frame.cc:837-899) for every later batched frame construction
  * (rgbl_frame_rgbl_batch, rgbl_resident_process, rgbl_resident_process_rgbd, both sequence runners) and tracking chain of this context:

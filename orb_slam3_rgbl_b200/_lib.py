@@ -117,6 +117,7 @@ SYMBOLS = {
     "rgbl_resident_process_stereo": (_i, [_vp, _f, _f, _vp]),
     "rgbl_resident_stage_stereo": (_i, [_vp, _i, _i, _vp, _vp, _i, _i, _i]),
     "rgbl_track_sequence_stereo": (_i, [_vp, _f, _f, _vp, _vp, _vp]),
+    "rgbl_set_stereo_rectification": (_i, [_vp, _vp, _vp, _vp, _vp, _i]),
     "rgbl_resident_track_end2": (_i, [_vp, _vp, _vp, _vp, _vp, _vp]),
     "rgbl_set_camera_distortion": (_i, [_vp, _f, _f, _f, _f, _vp, _i, _vp]),
     "rgbl_resident_download_keys_un": (_i, [_vp, _vp, _i, _vp]),

@@ -197,16 +197,19 @@ static int upload_images(Ctx* c, int n_frames, const uint8_t* const* gray, int s
     return RGBL_OK;
 }
 
-static int run_extract(Ctx* c, int n_frames, const std::function<void()>& aux_work = nullptr) {
+// level0: if set, enqueues the kernels that write level 0 on the main stream (rectification of stereo pairs) and returns their count;
+// billed to the pyramid stage.
+static int run_extract(Ctx* c, int n_frames, const std::function<void()>& aux_work = nullptr, const std::function<int()>& level0 = nullptr) {
     const int nl = c->tab.nlevels;
     // new frames: mvKeysUn == mvKeys and image bounds until undistort_keypoints says otherwise
     c->frames_undistorted = false;
     c->frame_bounds[0] = 0.f; c->frame_bounds[1] = (float)c->cfg.width; c->frame_bounds[2] = 0.f; c->frame_bounds[3] = (float)c->cfg.height;
     stage_begin(c, ST_PYRAMID, c->st);
+    const int level0_launches = level0 ? level0() : 0;
     // fused TMA tile kernel: level l's launch writes blur(l) and level l+1 (the separate blur stage below is then empty)
     const bool fused_levels = c->level_tma && launch_level_tiles(c->st, c->level_tms, c->d_pyr, c->d_blur, c->frame_bytes, c->levels.data(), nl, c->d_coefs, n_frames) == 0;
     if (!fused_levels) launch_pyramid(c->st, c->d_pyr, c->frame_bytes, c->levels.data(), nl, c->d_coefs, n_frames);
-    stage_end(c, ST_PYRAMID, c->st, fused_levels ? nl : nl - 1);
+    stage_end(c, ST_PYRAMID, c->st, level0_launches + (fused_levels ? nl : nl - 1));
     stage_begin(c, ST_FAST, c->st);
     if (c->fast_strips) {
         if (launch_fast_strips(c->st, c->d_pyr, c->frame_bytes, c->d_levels, c->d_cells, c->n_cells, c->d_strips, (int)c->strips.size(),
@@ -739,8 +742,9 @@ static int ensure_png_staging(Ctx* c) {
     return RGBL_OK;
 }
 
-// host inflate of n PNG streams into the pinned staging buffer + H2D of the filtered scanlines -> bytes per pixel (or < 0)
-static int inflate_png_batch(Ctx* c, int n_frames, const uint8_t* const* png, const size_t* png_bytes, bool depth16, cudaStream_t st) {
+// host inflate of n PNG streams into the pinned staging buffer + H2D of the filtered scanlines -> bytes per pixel (or < 0).
+// gray_only: a colour stream is RGBL_E_UNSUPPORTED, refused before anything is copied.
+static int inflate_png_batch(Ctx* c, int n_frames, const uint8_t* const* png, const size_t* png_bytes, bool depth16, cudaStream_t st, bool gray_only = false) {
     const int w = c->cfg.width, h = c->cfg.height;
     int rc = ensure_png_staging(c); if (rc) return rc;
     for (int f = 0; f < n_frames; ++f) if (!png[f] || !png_bytes[f]) { c->err = "empty image"; return RGBL_E_EMPTY; }
@@ -748,6 +752,11 @@ static int inflate_png_batch(Ctx* c, int n_frames, const uint8_t* const* png, co
     std::string perr;
     const int prc = png_inflate_batch(n_frames, png, png_bytes, w, h, c->h_png_raw, c->png_raw_stride, &ch, perr, depth16);
     if (prc) { c->err = perr; return prc == -2 ? RGBL_E_UNSUPPORTED : RGBL_E_INVALID; }
+    if (gray_only && ch != 1) {
+        // the reference remaps the image imread returned and converts it to gray afterwards, which differs for colour images
+        c->err = "rectified stereo takes 8-bit gray PNGs only (the reference remaps colour images before their conversion to gray)";
+        return RGBL_E_UNSUPPORTED;
+    }
     const size_t used = ((size_t)w * ch + 1) * h;
     for (int f = 0; f < n_frames; ++f)
         CU(cudaMemcpyAsync(c->d_png_raw + (size_t)f * c->png_raw_stride, c->h_png_raw + (size_t)f * c->png_raw_stride, used, cudaMemcpyHostToDevice, st));
@@ -769,6 +778,25 @@ static int decode_png_to_level0(Ctx* c, int n_frames, const uint8_t* const* png,
     const int ch = inflate_png_batch(c, n_frames, png, png_bytes, false, st);
     if (ch < 0) return ch;
     launch_png_unfilter_gray(st, c->d_png_raw, c->png_raw_stride, c->cfg.width, c->cfg.height, ch, camera_rgb, c->d_pyr, c->frame_bytes, c->levels[0],
+                             c->d_png_band, c->d_png_status, n_frames);
+    return png_status(c, st);
+}
+
+// one raw plane of a stereo pair awaiting rectification: level 0's layout without the frame slot around it
+static size_t raw_plane_bytes(const Ctx* c) { return (size_t)c->levels[0].pitch * c->cfg.height; }
+
+static int ensure_rect_raw(Ctx* c) {
+    if (!ensure(c->d_rect_raw, c->cfg.max_batch * raw_plane_bytes(c))) { c->err = "device allocation failed (raw stereo planes)"; return RGBL_E_CUDA; }
+    return RGBL_OK;
+}
+
+// with rectification on: 8-bit gray PNG streams into the raw planes 0..n_frames-1 (d_rect_raw, allocated by the caller)
+static int decode_png_to_raw(Ctx* c, int n_frames, const uint8_t* const* png, const size_t* png_bytes, cudaStream_t st) {
+    const int ch = inflate_png_batch(c, n_frames, png, png_bytes, false, st, true);
+    if (ch < 0) return ch;
+    LevelGeom raw = c->levels[0];
+    raw.off = 0;
+    launch_png_unfilter_gray(st, c->d_png_raw, c->png_raw_stride, c->cfg.width, c->cfg.height, ch, 0, c->d_rect_raw, raw_plane_bytes(c), raw,
                              c->d_png_band, c->d_png_status, n_frames);
     return png_status(c, st);
 }
@@ -840,8 +868,24 @@ static int check_rgbd_params(Ctx* c, float depth_scale, float bf) {
 // both extracted as one batch of 2n frames (the reference's two ORBextractor threads), then ComputeStereoMatches.  The left frames are
 // then the batch (last_frames = n) for download, ComputeBoW and the tracking chain.  The capacity-overflow flags cover all 2n frames,
 // so an overflow in a right frame, which changes the left frame's depths, fails the chain's _end2 like a left-frame overflow.
+// With rectification on, the raw planes of the pairs (rect_src) are first remapped into level 0 of the slots, in one launch billed to the
+// pyramid stage: System::TrackStereo's cv::remap of both images (src/System.cc:251 ff.).
 static int process_stereo(Ctx* c, int n_pairs, float mb, float mbf) {
-    const int max_n = run_extract(c, 2 * n_pairs);
+    std::function<int()> rectify;
+    if (c->rectify) {
+        if (!c->rect_src) { c->err = "no raw stereo planes to rectify"; return RGBL_E_INVALID; }
+        rectify = [&]() {
+            const LevelGeom& l0 = c->levels[0];
+            RectifyDev r{};
+            r.xy = c->d_rect_xy; r.a = c->d_rect_a; r.map_pitch = c->rect_pitch;
+            r.W = c->cfg.width; r.H = c->cfg.height;
+            r.src = c->rect_src; r.src_stride = raw_plane_bytes(c); r.src_pitch = l0.pitch;
+            r.dst = c->d_pyr; r.dst_stride = c->frame_bytes; r.dst_off = l0.off; r.dst_pitch = l0.pitch;
+            launch_rectify(c->st, r, n_pairs);
+            return 1;
+        };
+    }
+    const int max_n = run_extract(c, 2 * n_pairs, nullptr, rectify);
     if (max_n < 0) return max_n;
     int rc = stereo_matches(c, 0, n_pairs, n_pairs, mb, mbf); if (rc) return rc;
     c->last_frames = n_pairs;
@@ -853,6 +897,24 @@ static int process_stereo(Ctx* c, int n_pairs, float mb, float mbf) {
 static int check_stereo(Ctx* c, int n_pairs) {
     if (2 * n_pairs > c->cfg.max_batch) { c->err = "a stereo batch of n pairs takes 2 n frame slots: 2 n_pairs exceeds max_batch"; return RGBL_E_INVALID; }
     if (c->undistort) { c->err = "stereo needs rectified images: this context's camera has k1 != 0 (rgbl_set_camera_distortion)"; return RGBL_E_UNSUPPORTED; }
+    return RGBL_OK;
+}
+
+// H2D of n_pairs host pairs: left images into slots [0, n), right ones into [n, 2n), at level 0, or into the raw planes when the
+// context rectifies them (process_stereo then remaps them into level 0)
+static int upload_stereo(Ctx* c, int n_pairs, const uint8_t* const* left, const uint8_t* const* right, int stride) {
+    if (!c->rectify) {
+        int rc = upload_images(c, n_pairs, left, stride, c->st); if (rc) return rc;
+        rc = upload_images(c, n_pairs, right, stride, c->st, n_pairs); if (rc) return rc;
+    } else {
+        int rc = ensure_rect_raw(c); if (rc) return rc;
+        const size_t plane = raw_plane_bytes(c);
+        for (int f = 0; f < 2 * n_pairs; ++f)
+            CU(cudaMemcpy2DAsync(c->d_rect_raw + f * plane, c->levels[0].pitch, f < n_pairs ? left[f] : right[f - n_pairs], stride, c->cfg.width,
+                                 c->cfg.height, cudaMemcpyHostToDevice, c->st));
+        c->rect_src = c->d_rect_raw;
+    }
+    c->resident_frames = n_pairs; c->resident_max_pts = 0; c->resident_kind = InputKind::stereo;
     return RGBL_OK;
 }
 
@@ -1085,8 +1147,10 @@ static int restage(Ctx* c, int slot, InputKind kind) {
     const LevelGeom& l0 = c->levels[0];
     const size_t img_bytes = (size_t)l0.pitch * c->cfg.height, pts_floats = (size_t)4 * c->cfg.max_points;
     const int n_img = kind == InputKind::stereo ? 2 * sl.n_frames : sl.n_frames;
-    for (int f = 0; f < n_img; ++f)
-        CU(cudaMemcpyAsync(c->d_pyr + (size_t)f * c->frame_bytes + l0.off, sl.img + (size_t)f * img_bytes, img_bytes, cudaMemcpyDeviceToDevice, c->st));
+    if (kind == InputKind::stereo && c->rectify) c->rect_src = sl.img;      // the slot's raw planes are the remap's source: no copy
+    else
+        for (int f = 0; f < n_img; ++f)
+            CU(cudaMemcpyAsync(c->d_pyr + (size_t)f * c->frame_bytes + l0.off, sl.img + (size_t)f * img_bytes, img_bytes, cudaMemcpyDeviceToDevice, c->st));
     if (kind == InputKind::rgbd) {
         CU(cudaMemcpyAsync(c->d_depth16, sl.depth, (size_t)sl.n_frames * depth16_frame_elems(c) * sizeof(uint16_t), cudaMemcpyDeviceToDevice, c->st_aux));
     } else if (kind == InputKind::rgbl) {
@@ -1211,10 +1275,7 @@ int rgbl_track_sequence_stereo(rgbl_ctx* ctx, float mb, float mbf, const rgbl_ch
         if (!io->gray) return restage(c, (io->first_slot + b) % io->n_slots, InputKind::stereo);
         const size_t o = (size_t)b * T;
         for (int f = 0; f < T; ++f) if (!io->gray[o + f] || !right[o + f]) { c->err = "empty image"; return RGBL_E_EMPTY; }
-        int r = upload_images(c, T, io->gray + o, io->stride, c->st); if (r) return r;
-        r = upload_images(c, T, right + o, io->stride, c->st, T); if (r) return r;
-        c->resident_frames = T; c->resident_max_pts = 0; c->resident_kind = InputKind::stereo;
-        return RGBL_OK;
+        return upload_stereo(c, T, io->gray + o, right + o, io->stride);
     };
     return run_sequence(c, chain, io, load, [&]() { return process_stereo(c, T, mb, mbf); });
 }
@@ -1288,10 +1349,8 @@ int rgbl_resident_upload_stereo(rgbl_ctx* ctx, int n_pairs, const uint8_t* const
     rc = check_stereo(c, n_pairs); if (rc) return rc;
     for (int f = 0; f < n_pairs; ++f) if (!left[f] || !right[f]) { c->err = "empty image"; return RGBL_E_EMPTY; }
     CU(cudaSetDevice(c->cfg.device));
-    rc = upload_images(c, n_pairs, left, stride, c->st); if (rc) return rc;
-    rc = upload_images(c, n_pairs, right, stride, c->st, n_pairs); if (rc) return rc;
+    rc = upload_stereo(c, n_pairs, left, right, stride); if (rc) return rc;
     CU(cudaStreamSynchronize(c->st));
-    c->resident_frames = n_pairs; c->resident_max_pts = 0; c->resident_kind = InputKind::stereo;
     return RGBL_OK;
 }
 
@@ -1308,7 +1367,13 @@ int rgbl_resident_upload_stereo_png(rgbl_ctx* ctx, int n_pairs, const uint8_t* c
     std::vector<size_t> bytes(left_bytes, left_bytes + n_pairs);
     png.insert(png.end(), right_png, right_png + n_pairs);
     bytes.insert(bytes.end(), right_bytes, right_bytes + n_pairs);
-    rc = decode_png_to_level0(c, 2 * n_pairs, png.data(), bytes.data(), camera_rgb, c->st); if (rc) return rc;
+    if (c->rectify) {      // gray streams into the raw planes, remapped by the process call
+        rc = ensure_rect_raw(c); if (rc) return rc;
+        rc = decode_png_to_raw(c, 2 * n_pairs, png.data(), bytes.data(), c->st); if (rc) return rc;
+        c->rect_src = c->d_rect_raw;
+    } else {
+        rc = decode_png_to_level0(c, 2 * n_pairs, png.data(), bytes.data(), camera_rgb, c->st); if (rc) return rc;
+    }
     c->resident_frames = n_pairs; c->resident_max_pts = 0; c->resident_kind = InputKind::stereo;
     return RGBL_OK;
 }
@@ -1326,6 +1391,43 @@ int rgbl_resident_process_stereo(rgbl_ctx* ctx, float mb, float mbf, int* n_out)
     CU(cudaStreamSynchronize(c->st_aux));
     prof_collect(c);
     if (n_out) for (int f = 0; f < c->resident_frames; ++f) n_out[f] = c->h_n_sel[f];
+    return RGBL_OK;
+}
+
+// Settings::precomputeRectificationMaps' M1l / M2l / M1r / M2r (cv::initUndistortRectifyMap, CV_32F) -> OpenCV's fixed-point form on the
+// device.  Every check runs before anything is written, so a refused setting leaves the previous one in place.
+int rgbl_set_stereo_rectification(rgbl_ctx* ctx, const float* m1l, const float* m2l, const float* m1r, const float* m2r, int map_stride) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return RGBL_E_INVALID;
+    const float* maps[4] = {m1l, m2l, m1r, m2r};
+    int n_null = 0;
+    for (const float* m : maps) n_null += m == nullptr;
+    if (n_null == 4) {
+        c->rectify = false;
+        if (c->resident_kind == InputKind::stereo) c->resident_frames = 0;      // the uploaded pairs were staged for the other setting
+        return RGBL_OK;
+    }
+    if (n_null) { c->err = "the four rectification maps are all given or all NULL"; return RGBL_E_INVALID; }
+    const int W = c->cfg.width, H = c->cfg.height;
+    if (map_stride < W) { c->err = "map_stride < width"; return RGBL_E_INVALID; }
+    for (const float* m : maps)
+        for (int y = 0; y < H; ++y)
+            for (int x = 0; x < W; ++x)
+                if (!std::isfinite(m[(size_t)y * map_stride + x])) { c->err = "a rectification map holds a value that is not finite"; return RGBL_E_INVALID; }
+    CU(cudaSetDevice(c->cfg.device));
+    c->rect_pitch = (W + 3) & ~3;
+    const size_t entries = (size_t)2 * H * c->rect_pitch;
+    if (!ensure(c->d_rect_xy, entries) || !ensure(c->d_rect_a, entries)) { c->err = "device allocation failed (rectification maps)"; return RGBL_E_CUDA; }
+    DeviceArray<float> staged;       // the float maps, for the conversion only
+    if (staged.alloc((size_t)4 * H * W) != cudaSuccess) { c->err = "device allocation failed (rectification map staging)"; return RGBL_E_CUDA; }
+    for (int i = 0; i < 4; ++i)
+        CU(cudaMemcpy2DAsync(staged + (size_t)i * H * W, (size_t)W * sizeof(float), maps[i], (size_t)map_stride * sizeof(float), (size_t)W * sizeof(float), H,
+                             cudaMemcpyHostToDevice, c->st));
+    launch_rectify_maps(c->st, staged, W, H, c->d_rect_xy, c->d_rect_a, c->rect_pitch);
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(c->st));
+    c->rectify = true;
+    if (c->resident_kind == InputKind::stereo) c->resident_frames = 0;
     return RGBL_OK;
 }
 

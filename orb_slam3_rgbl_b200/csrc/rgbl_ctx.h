@@ -18,7 +18,7 @@ static const char* const kStageNames[kNumStages] = {"pyramid", "fast", "compact"
 constexpr int kMatchListCap = 512;    // admissible candidates kept per map point (overflow is reported)
 
 // the inputs of a resident upload or a staged slot: RGB-L (image + point cloud), RGB-D (image + uint16 depth plane), stereo (left and
-// right image of a rectified pair)
+// right image of a pair: rectified, or raw when the context rectifies them)
 enum class InputKind { rgbl, rgbd, stereo };
 
 // Lazily grown device scratch of the tracking entry points (api_track.cu).
@@ -93,6 +93,16 @@ struct Ctx {
     // referenced by the chain's CUDA graphs, so it needs no scratch_generation bump.
     DeviceArray<int> d_stereo_row_start, d_stereo_row_idx, d_stereo_sad;
     int stereo_idx_cap = 0;
+    // stereo rectification (rgbl_set_stereo_rectification, stereo_kernels.cu).  d_rect_xy / d_rect_a: OpenCV's fixed-point form of the
+    // left and right maps, H rows of rect_pitch entries per camera, allocated by the first setting and never reallocated.  d_rect_raw:
+    // max_batch raw planes in level 0's layout (row pitch levels[0].pitch), allocated by the first stereo upload with rectification on;
+    // host uploads and PNG decodes of pairs write there instead of level 0.  rect_src: the raw planes of the uploaded pairs (d_rect_raw,
+    // or a staged slot's planes).  No chain graph references these buffers, so they need no scratch_generation bump.
+    bool rectify = false;
+    DeviceArray<uint32_t> d_rect_xy; DeviceArray<uint16_t> d_rect_a;
+    int rect_pitch = 0;
+    DeviceArray<uint8_t> d_rect_raw;
+    const uint8_t* rect_src = nullptr;
     DeviceArray<int> d_n_pts;
     DeviceArray<uint32_t> d_idx_map;
     DeviceArray<float> d_raw, d_processed, d_depth, d_uright;

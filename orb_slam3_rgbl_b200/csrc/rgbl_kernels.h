@@ -222,6 +222,19 @@ struct StereoBatchDev {
 int stereo_row_index_cap(int cap, const float* scale, int n_levels, int n_rows);
 void launch_stereo_matches(cudaStream_t st, const StereoBatchDev& s, int n_pairs);
 
+// stereo_kernels.cu, rectification: cv::remap(INTER_LINEAR, BORDER_CONSTANT 0) of stereo pairs with fixed-point maps -----------------
+// maps = [m1l | m2l | m1r | m2r] (H x W floats each) -> per camera (left 0, right 1) H rows of `pitch` (a multiple of 4) entries:
+// xy = sx | sy << 16 (int16 each), a = ay * 32 + ax
+void launch_rectify_maps(cudaStream_t st, const float* maps, int W, int H, uint32_t* xy, uint16_t* a, int pitch);
+struct RectifyDev {
+    const uint32_t* xy; const uint16_t* a; int map_pitch;
+    int W, H;
+    const uint8_t* src; size_t src_stride; int src_pitch;            // raw plane of slot s at src + s * src_stride
+    uint8_t* dst; size_t dst_stride; int dst_off, dst_pitch;         // rectified plane of slot s at dst + s * dst_stride + dst_off (4-byte aligned rows)
+};
+// slots [0, n_pairs) through the left camera's map, [n_pairs, 2 n_pairs) through the right camera's, in one launch
+void launch_rectify(cudaStream_t st, const RectifyDev& r, int n_pairs);
+
 // pose_kernels.cu ----------------------------------------------------------------------------------
 struct PoseProblemDev {
     int n;                           // edges (keypoint order)

@@ -221,4 +221,92 @@ void launch_stereo_matches(cudaStream_t st, const StereoBatchDev& s, int n_pairs
     stereo_median_kernel<<<n_pairs, 1024, 0, st>>>(s);
 }
 
+// ---- Rectification of stereo pairs: the cv::remap(im, imRect, M1, M2, INTER_LINEAR) that System::TrackStereo runs on both images before
+// GrabImageStereo when Settings::needToRectify() (src/System.cc:251 ff.), for 8UC1 images, two CV_32FC1 maps, BORDER_CONSTANT 0.
+//
+// OpenCV's bilinear remap works in fixed point (imgproc remapBilinear with INTER_BITS = 5): X = cvRound(mapx * 32), Y = cvRound(mapy * 32)
+// (round half to even, saturated to int), source pixel (sx, sy) = (sat16(X >> 5), sat16(Y >> 5)), fraction (ax, ay) = (X & 31, Y & 31),
+// tap weights (32 - ay)(32 - ax) 32, (32 - ay) ax 32, ay (32 - ax) 32, ay ax 32 (their sum is 2^15, so OpenCV's table correction never
+// changes them) and dst = sat_u8((sum of tap * weight + 2^14) >> 15), a tap outside the source contributing 0.  cv::remap with the float
+// maps gives what it gives with convertMaps(..., CV_16SC2) maps, so the maps are converted to that form once, when they are set
+// (launch_rectify_maps); the remap of a batch reads the converted form (launch_rectify).
+
+namespace {
+
+__device__ __forceinline__ int round_fixed5(float v) {        // cvRound(v * 32), saturated
+    const float r = rintf(v * 32.f);
+    if (r >= 2147483648.f) return INT_MAX;
+    if (r < -2147483648.f) return INT_MIN;
+    return (int)r;
+}
+
+__device__ __forceinline__ int sat16(int v) { return v < SHRT_MIN ? SHRT_MIN : (v > SHRT_MAX ? SHRT_MAX : v); }
+
+// one thread per map entry: maps = [m1l | m2l | m1r | m2r], each H x W floats; camera = blockIdx.z (0 left, 1 right)
+__global__ void __launch_bounds__(256) rectify_maps_kernel(const float* maps, int W, int H, uint32_t* xy, uint16_t* a, int pitch) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y, cam = blockIdx.z;
+    if (x >= pitch) return;
+    const size_t o = ((size_t)cam * H + y) * pitch + x;
+    if (x >= W) { xy[o] = 0u; a[o] = 0; return; }           // row padding: read by the last group of a row, never used
+    const size_t i = ((size_t)2 * cam * H + y) * W + x;
+    const int X = round_fixed5(maps[i]), Y = round_fixed5(maps[i + (size_t)H * W]);
+    xy[o] = (uint32_t)(uint16_t)sat16(X >> 5) | ((uint32_t)(uint16_t)sat16(Y >> 5) << 16);
+    a[o] = (uint16_t)((Y & 31) * 32 + (X & 31));
+}
+
+constexpr int kGroup = 4;                  // output pixels per thread: one 32-bit store per row group
+
+// One thread per group of 4 output pixels of row blockIdx.y of camera blockIdx.z: the group's map entries are read once, then the
+// camera's n frames are remapped with them.  Taps outside the source get weight 0 and offset 0, so the frame loop has no branch.
+__global__ void __launch_bounds__(128) rectify_kernel(RectifyDev r, int n) {
+    const int x0 = (blockIdx.x * blockDim.x + threadIdx.x) * kGroup, y = blockIdx.y, cam = blockIdx.z;
+    if (x0 >= r.W) return;
+    const size_t o = ((size_t)cam * r.H + y) * r.map_pitch + x0;
+    const uint4 m = *reinterpret_cast<const uint4*>(r.xy + o);
+    const unsigned long long fr = *reinterpret_cast<const unsigned long long*>(r.a + o);
+    const uint32_t mxy[kGroup] = {m.x, m.y, m.z, m.w};
+    int off[kGroup][4], w[kGroup][4];
+#pragma unroll
+    for (int p = 0; p < kGroup; ++p) {
+        const int sx = (int)(int16_t)(mxy[p] & 0xffffu), sy = (int)(int16_t)(mxy[p] >> 16);
+        const int f = (int)((fr >> (16 * p)) & 0xffffu), ax = f & 31, ay = f >> 5;
+        const int wt[4] = {(32 - ay) * (32 - ax) * 32, (32 - ay) * ax * 32, ay * (32 - ax) * 32, ay * ax * 32};
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+            const int tx = sx + (t & 1), ty = sy + (t >> 1);
+            const bool in = tx >= 0 && tx < r.W && ty >= 0 && ty < r.H;
+            off[p][t] = in ? ty * r.src_pitch + tx : 0;
+            w[p][t] = in ? wt[t] : 0;
+        }
+    }
+    const int n_out = min(kGroup, r.W - x0);
+    for (int f = 0; f < n; ++f) {
+        const int slot = cam * n + f;
+        const uint8_t* src = r.src + (size_t)slot * r.src_stride;
+        uint32_t packed = 0;
+#pragma unroll
+        for (int p = 0; p < kGroup; ++p) {
+            int s = 1 << 14;
+#pragma unroll
+            for (int t = 0; t < 4; ++t) s += (int)__ldg(src + off[p][t]) * w[p][t];
+            packed |= (uint32_t)min(s >> 15, 255) << (8 * p);
+        }
+        uint8_t* dst = r.dst + (size_t)slot * r.dst_stride + r.dst_off + (size_t)y * r.dst_pitch + x0;
+        if (n_out == kGroup) *reinterpret_cast<uint32_t*>(dst) = packed;
+        else for (int p = 0; p < n_out; ++p) dst[p] = (uint8_t)(packed >> (8 * p));     // the row's padding is not written
+    }
+}
+
+}  // namespace
+
+void launch_rectify_maps(cudaStream_t st, const float* maps, int W, int H, uint32_t* xy, uint16_t* a, int pitch) {
+    rectify_maps_kernel<<<dim3((pitch + 255) / 256, H, 2), 256, 0, st>>>(maps, W, H, xy, a, pitch);
+}
+
+void launch_rectify(cudaStream_t st, const RectifyDev& r, int n_pairs) {
+    if (n_pairs < 1) return;
+    const int groups = (r.W + kGroup - 1) / kGroup;
+    rectify_kernel<<<dim3((groups + 127) / 128, r.H, 2), 128, 0, st>>>(r, n_pairs);
+}
+
 }  // namespace rgbl

@@ -59,6 +59,19 @@ class Context:
         check(lib().rgbl_set_camera_distortion(self.handle, fx, fy, cx, cy, ptr(d), len(d), ptr(b)), self.handle)
         return b
 
+    def set_stereo_rectification(self, m1l, m2l, m1r, m2r):
+        """Rectify every later stereo pair on the device (rgbl_set_stereo_rectification): the H x W float32 maps M1l, M2l, M1r, M2r of
+        cv::initUndistortRectifyMap, as Settings holds them; the stereo uploads and runners then take the raw images.  All None: off."""
+        maps = [m1l, m2l, m1r, m2r]
+        if all(m is None for m in maps):
+            check(lib().rgbl_set_stereo_rectification(self.handle, None, None, None, None, 0), self.handle)
+            return
+        arr = [None if m is None else np.ascontiguousarray(m, np.float32) for m in maps]
+        if any(a is not None and a.shape != (self.height, self.width) for a in arr):
+            raise ValueError(f"the maps must be {self.height} x {self.width} (the context's size)")
+        stride = self.width
+        check(lib().rgbl_set_stereo_rectification(self.handle, *[None if a is None else ptr(a) for a in arr], stride), self.handle)
+
     def set_host_quadtree(self, on: bool):
         check(lib().rgbl_set_host_quadtree(self.handle, int(on)), self.handle)
 

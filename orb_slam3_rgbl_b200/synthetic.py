@@ -27,6 +27,11 @@ TUM1_FX, TUM1_FY, TUM1_CX, TUM1_CY = 517.306408, 516.469215, 318.643040, 255.313
 TUM1_DIST = np.array([0.262383, -0.953104, -0.005358, 0.002628, 1.163314], np.float32)      # k1, k2, p1, p2, k3
 TUM1_BF = 40.0
 TUM_DEPTH_FACTOR = 5000.0
+# a EuRoC-like stereo camera (752 x 480, strong barrel distortion) for the rectification path; bf is chosen so that the plane sequences
+# (Z = 20 m) have a whole-pixel disparity of 5 px, not EuRoC's own baseline
+EUROC_W, EUROC_H = 752, 480
+EUROC_CAM = (458.654, 457.296, 367.215, 248.375, 100.0)          # fx, fy, cx, cy, bf
+EUROC_DIST = np.array([-0.28, 0.07, 2e-4, 2e-5], np.float32)      # k1, k2, p1, p2
 
 
 def camera_matrix(fx=KITTI_FX, fy=KITTI_FY, cx=KITTI_CX, cy=KITTI_CY) -> np.ndarray:
@@ -194,11 +199,43 @@ class PlaneSequence:
         bot = tex[y0 + 1, x0] * (1 - fx) + tex[y0 + 1, x0 + 1] * fx
         return np.ascontiguousarray(np.clip(np.rint(top * (1 - fy) + bot * fy), 0, 255).astype(np.uint8))
 
+    def raw_left_image(self, t: int) -> np.ndarray:
+        """Frame t of the left camera of a distorted stereo rig (a sequence built with dist=), before rectification: image(t)."""
+        if self.dist is None:
+            raise ValueError("raw_left_image needs a sequence with a distortion model (dist=)")
+        return self.image(t)
+
+    def raw_right_image(self, t: int) -> np.ndarray:
+        """Frame t of the right camera of a distorted stereo rig (same lens, baseline bf / fx along +x, no rotation), before rectification:
+        the lens sampling of image(t) applied to the pinhole view shifted by the disparity d = bf / Z (right_image of a pinhole sequence).
+        Rectified with rectification_maps(), it becomes that pinhole view."""
+        if self.dist is None:
+            raise ValueError("raw_right_image needs a sequence with a distortion model (dist=)")
+        s, d = self.step_index(t), self._whole_disparity()
+        tex = self.texture.astype(np.float64)
+        xs = self.map_x + (s * self.shift + d + self.margin); ys = self.map_y + self.margin
+        x0 = np.floor(xs).astype(np.int64); y0 = np.floor(ys).astype(np.int64)
+        fx = xs - x0; fy = ys - y0
+        top = tex[y0, x0] * (1 - fx) + tex[y0, x0 + 1] * fx
+        bot = tex[y0 + 1, x0] * (1 - fx) + tex[y0 + 1, x0 + 1] * fx
+        return np.ascontiguousarray(np.clip(np.rint(top * (1 - fy) + bot * fy), 0, 255).astype(np.uint8))
+
+    def rectification_maps(self, R=None):
+        """float32 (map_x, map_y), H x W, of cv::initUndistortRectifyMap(K, dist, R, K, (W, H), CV_32FC1) for this sequence's camera, in
+        closed form: rectified pixel (u, v) -> ray R^-1 K^-1 (u, v, 1) -> distort_normalized -> K.  R = None: the identity (the maps of the
+        raw views above, whose rig needs no rotation)."""
+        if self.dist is None:
+            raise ValueError("rectification_maps needs a sequence with a distortion model (dist=)")
+        return rectification_maps(self.W, self.H, self.cam[:4], self.dist, R)
+
     def disparity_px(self) -> int:
         """Disparity of the plane in a rectified stereo rig with baseline bf / fx: bf / Z pixels (5 at the defaults)."""
-        d = self.cam[4] / self.Z
         if self.dist is not None:
             raise ValueError("right_image needs a pinhole camera: stereo pairs are rectified, this sequence has a distortion model")
+        return self._whole_disparity()
+
+    def _whole_disparity(self) -> int:
+        d = self.cam[4] / self.Z
         if abs(d - round(d)) > 1e-9:
             raise ValueError(f"right_image needs a whole-pixel disparity bf / Z, got {d} px")
         if round(d) > self.shift + 8:
@@ -245,6 +282,18 @@ def distort_normalized(x, y, dist):
     r2 = x * x + y * y
     radial = 1 + r2 * (k1 + r2 * (k2 + r2 * k3))
     return x * radial + 2 * p1 * x * y + p2 * (r2 + 2 * x * x), y * radial + p1 * (r2 + 2 * y * y) + 2 * p2 * x * y
+
+
+def rectification_maps(W: int, H: int, cam, dist, R=None):
+    """float32 (map_x, map_y), H x W, of cv::initUndistortRectifyMap(K, dist, R, K, (W, H), CV_32FC1), K = (fx, fy, cx, cy): for each
+    rectified pixel (u, v) the raw (distorted) pixel it samples.  R = None: the identity."""
+    fx, fy, cx, cy = (float(v) for v in cam)
+    v, u = np.mgrid[0:H, 0:W].astype(np.float64)
+    ray = np.stack([(u - cx) / fx, (v - cy) / fy, np.ones_like(u)])
+    if R is not None:
+        ray = np.tensordot(np.asarray(R, np.float64).T, ray, 1)         # R^-1 = R^T
+    xd, yd = distort_normalized(ray[0] / ray[2], ray[1] / ray[2], np.asarray(dist, np.float64))
+    return (xd * fx + cx).astype(np.float32), (yd * fy + cy).astype(np.float32)
 
 
 def undistorted_pixel_map(W: int, H: int, cam, dist, iterations: int = 100):
