@@ -180,7 +180,7 @@ struct Ctx {
     // rgbl_track_sequence_rgbd, rgbl_resident_stage_stereo / rgbl_track_sequence_stereo): level-0 planes + clouds (RGB-L), uint16 depth
     // planes (RGB-D) or the left then the right level-0 planes (stereo: n_frames pairs, 2 n_frames planes) of whole batches
     static constexpr int kMaxStageSlots = 8;
-    struct StageSlot { DeviceArray<uint8_t> img; DeviceArray<float> pts; DeviceArray<int> n_pts; DeviceArray<uint16_t> depth; std::vector<int> h_n_pts; int n_frames = 0, max_pts = 0; InputKind kind = InputKind::rgbl; };
+    struct StageSlot { DeviceArray<uint8_t> img; DeviceArray<float> pts; DeviceArray<int> n_pts; DeviceArray<uint16_t> depth; int n_frames = 0, max_pts = 0; InputKind kind = InputKind::rgbl; };
     StageSlot stage[kMaxStageSlots];
 
     // camera model of Frame::UndistortKeyPoints / ComputeImageBounds (rgbl_set_camera_distortion): undistort = (k1 != 0); cam_bounds =

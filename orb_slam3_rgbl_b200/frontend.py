@@ -532,15 +532,51 @@ def make_chain_params(pose0, fx, fy, cx, cy, bf, th_last=15.0, mono=False, conti
     return p
 
 
-class RgblBatch:
+class _FrameBatch:
+    """The output buffers of one batch of frame constructions, and the calls that read the batch from the device: download,
+    download_keys_un and the tracking chain.  The input kinds (RgblBatch, RgbdBatch, StereoBatch) add their inputs and upload calls."""
+
+    def __init__(self, ctx: Context, nF: int, W: int, H: int, pinned: bool):
+        self.ctx, self.nF, self.cap, self.W, self.H = ctx, nF, ctx.cap, W, H
+        self._alloc = alloc = _pinned_alloc if pinned else (lambda shape, dt: np.empty(shape, dt))
+        self.kps = alloc((nF, self.cap), KP_DTYPE); self.desc = alloc((nF, self.cap, 32), np.uint8)
+        self.depth = alloc((nF, self.cap), np.float32); self.uright = alloc((nF, self.cap), np.float32)
+        self.n = np.zeros(nF, np.int32)
+
+    def download(self):
+        c = self.ctx
+        check(lib().rgbl_resident_download(c.handle, ptr(self.kps), ptr(self.desc), ptr(self.depth), ptr(self.uright), self.cap, ptr(self.n)), c.handle)
+        return [(self.kps[f, :self.n[f]], self.desc[f, :self.n[f]], self.depth[f, :self.n[f]], self.uright[f, :self.n[f]]) for f in range(self.nF)]
+
+    def download_keys_un(self):
+        """mvKeysUn of the frames of the last batched call (rgbl_resident_download_keys_un): list of keypoint arrays, one per frame"""
+        c = self.ctx
+        kun = np.empty((self.nF, self.cap), KP_DTYPE); n = np.zeros(self.nF, np.int32)
+        check(lib().rgbl_resident_download_keys_un(c.handle, ptr(kun), self.cap, ptr(n)), c.handle)
+        return [kun[f, :n[f]].copy() for f in range(self.nF)]
+
+    def track_begin2(self, prm: ChainParams):
+        """rgbl_resident_track_begin2: TrackWithMotionModel + (local_map_frames > 0) TrackLocalMap per frame; continue_sequence
+        tracks frame 0 of this batch against the last frame of the previous chain of this context."""
+        check(lib().rgbl_resident_track_begin2(self.ctx.handle, C.byref(prm)), self.ctx.handle)
+
+    def track_end2(self):
+        """-> dict(poses[nF,7], n_matches, n_inliers, n_local_matches, n_inliers_first) of the oldest queued chain"""
+        nF = self.nF
+        out = dict(poses=np.empty((nF, 7), np.float32), n_matches=np.zeros(nF, np.int32), n_inliers=np.zeros(nF, np.int32),
+                   n_local_matches=np.zeros(nF, np.int32), n_inliers_first=np.zeros(nF, np.int32))
+        check(lib().rgbl_resident_track_end2(self.ctx.handle, ptr(out["poses"]), ptr(out["n_matches"]), ptr(out["n_inliers"]),
+                                             ptr(out["n_local_matches"]), ptr(out["n_inliers_first"])), self.ctx.handle)
+        return out
+
+
+class RgblBatch(_FrameBatch):
     """Reusable (pinned if torch+CUDA are available) host buffers for rgbl_frame_rgbl_batch / the resident API."""
 
     def __init__(self, ctx: Context, images, clouds, P, depth_params: DepthParams, pinned=True):
-        self.ctx = ctx
-        nF = len(images); cap = ctx.cap
-        self.nF, self.cap = nF, cap
-        alloc = _pinned_alloc if pinned else (lambda shape, dt: np.empty(shape, dt))
         H, W = images[0].shape
+        super().__init__(ctx, len(images), W, H, pinned)
+        nF, alloc = self.nF, self._alloc
         self.img = alloc((nF, H, W), np.uint8)
         maxn = max(p.shape[1] for p in clouds)
         self.pts = alloc((nF, 4 * maxn), np.float32)
@@ -552,10 +588,6 @@ class RgblBatch:
         self.pa = (C.c_void_p * nF)(*[self.pts[f].ctypes.data for f in range(nF)])
         self.P = np.ascontiguousarray(P, np.float32).reshape(12)
         self.prm = depth_params
-        self.kps = alloc((nF, cap), KP_DTYPE); self.desc = alloc((nF, cap, 32), np.uint8)
-        self.depth = alloc((nF, cap), np.float32); self.uright = alloc((nF, cap), np.float32)
-        self.n = np.zeros(nF, np.int32)
-        self.W, self.H = W, H
         self.h2d_bytes = int(nF * W * H + 4 * 4 * int(self.npts.sum()))
 
     def run_e2e(self):
@@ -620,20 +652,6 @@ class RgblBatch:
         check(lib().rgbl_resident_track_end(c.handle, ptr(poses), ptr(nm), ptr(ni)), c.handle)
         return poses, nm, ni
 
-    def track_begin2(self, prm: ChainParams):
-        """rgbl_resident_track_begin2: TrackWithMotionModel + (local_map_frames > 0) TrackLocalMap per frame; continue_sequence
-        tracks frame 0 of this batch against the last frame of the previous chain of this context."""
-        check(lib().rgbl_resident_track_begin2(self.ctx.handle, C.byref(prm)), self.ctx.handle)
-
-    def track_end2(self):
-        """-> dict(poses[nF,7], n_matches, n_inliers, n_local_matches, n_inliers_first) of the oldest queued chain"""
-        nF = self.nF
-        out = dict(poses=np.empty((nF, 7), np.float32), n_matches=np.zeros(nF, np.int32), n_inliers=np.zeros(nF, np.int32),
-                   n_local_matches=np.zeros(nF, np.int32), n_inliers_first=np.zeros(nF, np.int32))
-        check(lib().rgbl_resident_track_end2(self.ctx.handle, ptr(out["poses"]), ptr(out["n_matches"]), ptr(out["n_inliers"]),
-                                             ptr(out["n_local_matches"]), ptr(out["n_inliers_first"])), self.ctx.handle)
-        return out
-
     def set_inputs(self, images, clouds):
         """Refill the (pinned) input buffers with another batch of the same shape."""
         assert len(images) == self.nF
@@ -645,37 +663,19 @@ class RgblBatch:
             self.npts[f] = n
         self.h2d_bytes = int(self.nF * self.W * self.H + 4 * 4 * int(self.npts.sum()))
 
-    def download(self):
-        c = self.ctx
-        check(lib().rgbl_resident_download(c.handle, ptr(self.kps), ptr(self.desc), ptr(self.depth), ptr(self.uright), self.cap, ptr(self.n)), c.handle)
-        return [(self.kps[f, :self.n[f]], self.desc[f, :self.n[f]], self.depth[f, :self.n[f]], self.uright[f, :self.n[f]]) for f in range(self.nF)]
 
-    def download_keys_un(self):
-        """mvKeysUn of the frames of the last batched call (rgbl_resident_download_keys_un): list of keypoint arrays, one per frame"""
-        c = self.ctx
-        kun = np.empty((self.nF, self.cap), KP_DTYPE); n = np.zeros(self.nF, np.int32)
-        check(lib().rgbl_resident_download_keys_un(c.handle, ptr(kun), self.cap, ptr(n)), c.handle)
-        return [kun[f, :n[f]].copy() for f in range(self.nF)]
-
-
-class RgbdBatch:
+class RgbdBatch(_FrameBatch):
     """Host buffers of one batch of RGB-D frames (gray image + CV_16U depth image each) for the resident RGB-D API: the RGB-D Frame
     constructor (src/Frame.cc:200-237) is upload + process_resident; download / track_begin2 / track_end2 as for RgblBatch."""
 
     def __init__(self, ctx: Context, images, depths, pinned=True):
-        self.ctx = ctx
-        nF = len(images); cap = ctx.cap
-        self.nF, self.cap = nF, cap
-        alloc = _pinned_alloc if pinned else (lambda shape, dt: np.empty(shape, dt))
         H, W = images[0].shape
-        self.W, self.H = W, H
+        super().__init__(ctx, len(images), W, H, pinned)
+        nF, alloc = self.nF, self._alloc
         self.img = alloc((nF, H, W), np.uint8); self.dep = alloc((nF, H, W), np.uint16)
         self.set_inputs(images, depths)
         self.ia = (C.c_void_p * nF)(*[self.img[f].ctypes.data for f in range(nF)])
         self.da = (C.c_void_p * nF)(*[self.dep[f].ctypes.data for f in range(nF)])
-        self.kps = alloc((nF, cap), KP_DTYPE); self.desc = alloc((nF, cap, 32), np.uint8)
-        self.depth = alloc((nF, cap), np.float32); self.uright = alloc((nF, cap), np.float32)
-        self.n = np.zeros(nF, np.int32)
 
     def set_inputs(self, images, depths):
         assert len(images) == self.nF and len(depths) == self.nF
@@ -701,31 +701,21 @@ class RgbdBatch:
         check(lib().rgbl_resident_process_rgbd(c.handle, depth_scale, bf, ptr(self.n)), c.handle)
         return self.n
 
-    download = RgblBatch.download
-    download_keys_un = RgblBatch.download_keys_un
-    track_begin2 = RgblBatch.track_begin2
-    track_end2 = RgblBatch.track_end2
 
 
-class StereoBatch:
+class StereoBatch(_FrameBatch):
     """Host buffers of one batch of rectified stereo pairs for the resident stereo API: the stereo Frame constructor (src/Frame.cc:101-197)
     is upload + process_resident (the 2n images extracted as one batch, then ComputeStereoMatches, ctx.max_batch >= 2n); download /
     download_keys_un / track_begin2 / track_end2 then see the left frames, as for RgblBatch."""
 
     def __init__(self, ctx: Context, lefts, rights, pinned=True):
-        self.ctx = ctx
-        nF = len(lefts); cap = ctx.cap
-        self.nF, self.cap = nF, cap
-        alloc = _pinned_alloc if pinned else (lambda shape, dt: np.empty(shape, dt))
         H, W = lefts[0].shape
-        self.W, self.H = W, H
+        super().__init__(ctx, len(lefts), W, H, pinned)
+        nF, alloc = self.nF, self._alloc
         self.left = alloc((nF, H, W), np.uint8); self.right = alloc((nF, H, W), np.uint8)
         self.set_inputs(lefts, rights)
         self.la = (C.c_void_p * nF)(*[self.left[f].ctypes.data for f in range(nF)])
         self.ra = (C.c_void_p * nF)(*[self.right[f].ctypes.data for f in range(nF)])
-        self.kps = alloc((nF, cap), KP_DTYPE); self.desc = alloc((nF, cap, 32), np.uint8)
-        self.depth = alloc((nF, cap), np.float32); self.uright = alloc((nF, cap), np.float32)
-        self.n = np.zeros(nF, np.int32)
 
     def set_inputs(self, lefts, rights):
         assert len(lefts) == self.nF and len(rights) == self.nF
@@ -750,11 +740,6 @@ class StereoBatch:
         check(lib().rgbl_resident_process_stereo(c.handle, mb, mbf, ptr(self.n)), c.handle)
         return self.n
 
-    download = RgblBatch.download
-    download_keys_un = RgblBatch.download_keys_un
-    track_begin2 = RgblBatch.track_begin2
-    track_end2 = RgblBatch.track_end2
-
 
 class SequenceIO(C.Structure):
     """rgbl_sequence_io (include/rgbl_b200.h)."""
@@ -769,29 +754,18 @@ class SequenceRunner:
     Holds M batches of T frames in pinned host buffers (and, after stage(), in device slots); batches are visited round-robin."""
 
     def __init__(self, ctx: Context, P, depth_params: DepthParams, T: int, W: int, H: int, max_points: int, n_host_batches: int, pinned=True):
-        self.ctx, self.T, self.W, self.H, self.M, self.maxn = ctx, T, W, H, n_host_batches, max_points
-        alloc = _pinned_alloc if pinned else (lambda shape, dt: np.empty(shape, dt))
-        self._alloc = alloc
-        self.img = alloc((self.M, T, H, W), np.uint8)
-        self.pts = alloc((self.M, T, 4 * max_points), np.float32)
-        self.npts = np.zeros((self.M, T), np.int32)
+        self._init(ctx, T, W, H, n_host_batches, pinned, "rgbl", (4 * max_points,), np.float32)
+        self.maxn, self.pts, self.npts = max_points, self.second, np.zeros((self.M, T), np.int32)
         self.P = np.ascontiguousarray(P, np.float32).reshape(12)
         self.prm = depth_params
-        self._out = None
-        self.kind = "rgbl"
 
     @classmethod
     def rgbd(cls, ctx: Context, depth_scale: float, bf: float, T: int, W: int, H: int, n_host_batches: int, pinned=True) -> "SequenceRunner":
         """RGB-D mode (rgbl_track_sequence_rgbd, the loop of Examples/RGB-D/rgbd_kitti.cc): batches of gray images + CV_16U depth images;
         set_batch(m, images, depths).  depth_scale = Tracking::mDepthMapFactor, bf = Camera.bf."""
         self = cls.__new__(cls)
-        self.ctx, self.T, self.W, self.H, self.M, self.maxn = ctx, T, W, H, n_host_batches, 0
-        self._alloc = _pinned_alloc if pinned else (lambda shape, dt: np.empty(shape, dt))
-        self.img = self._alloc((self.M, T, H, W), np.uint8)
-        self.dep = self._alloc((self.M, T, H, W), np.uint16)
-        self.depth_scale, self.bf = float(depth_scale), float(bf)
-        self._out = None
-        self.kind = "rgbd"
+        self._init(ctx, T, W, H, n_host_batches, pinned, "rgbd", (H, W), np.uint16)
+        self.dep, self.depth_scale, self.bf = self.second, float(depth_scale), float(bf)
         return self
 
     @classmethod
@@ -799,42 +773,43 @@ class SequenceRunner:
         """Stereo mode (rgbl_track_sequence_stereo, the loop of Examples/Stereo/stereo_kitti.cc): batches of T rectified pairs, extracted as
         batches of 2T frames (ctx.max_batch >= 2T); set_batch(m, lefts, rights).  mb = mbf / fx, mbf = Camera.bf."""
         self = cls.__new__(cls)
-        self.ctx, self.T, self.W, self.H, self.M, self.maxn = ctx, T, W, H, n_host_batches, 0
+        self._init(ctx, T, W, H, n_host_batches, pinned, "stereo", (H, W), np.uint8)
+        self.right, self.mb, self.mbf = self.second, float(mb), float(mbf)
+        return self
+
+    def _init(self, ctx, T, W, H, n_host_batches, pinned, kind, second_shape, second_dtype):
+        """The images of M batches and, per frame, the kind's second input (`second`): a flat cloud, a depth image or a right image."""
+        self.ctx, self.T, self.W, self.H, self.M, self.maxn, self.kind = ctx, T, W, H, n_host_batches, 0, kind
         self._alloc = _pinned_alloc if pinned else (lambda shape, dt: np.empty(shape, dt))
         self.img = self._alloc((self.M, T, H, W), np.uint8)
-        self.right = self._alloc((self.M, T, H, W), np.uint8)
-        self.mb, self.mbf = float(mb), float(mbf)
+        self.second = self._alloc((self.M, T) + second_shape, second_dtype)
         self._out = None
-        self.kind = "stereo"
-        return self
 
     def set_batch(self, m: int, images, clouds):
         """clouds: 4 x N point clouds (RGB-L), the uint16 depth images in RGB-D mode, or the right images in stereo mode."""
-        if self.kind != "rgbl":
-            other = self.dep if self.kind == "rgbd" else self.right
-            for f in range(self.T):
-                self.img[m, f] = images[f]; other[m, f] = np.asarray(clouds[f], other.dtype)
-            return
         for f in range(self.T):
             self.img[m, f] = images[f]
+            if self.kind != "rgbl":
+                self.second[m, f] = np.asarray(clouds[f], self.second.dtype)
+                continue
             n = clouds[f].shape[1]
             self.pts[m, f, :4 * n] = np.ascontiguousarray(clouds[f], np.float32).reshape(-1)
             self.npts[m, f] = n
 
+    def _frames(self, a, batches):
+        """C array of the addresses of the frames of `batches` in a (img or second)"""
+        return (C.c_void_p * (len(batches) * self.T))(*[a[m, f].ctypes.data for m in batches for f in range(self.T)])
+
     def stage(self, slot: int, m: int):
         """Upload host batch m into device slot `slot` (rgbl_resident_stage / _stage_rgbd / _stage_stereo)."""
-        ia = (C.c_void_p * self.T)(*[self.img[m, f].ctypes.data for f in range(self.T)])
+        h, T, W, H = self.ctx.handle, self.T, self.W, self.H
+        ia, sa = self._frames(self.img, [m]), self._frames(self.second, [m])
         if self.kind == "stereo":
-            ra = (C.c_void_p * self.T)(*[self.right[m, f].ctypes.data for f in range(self.T)])
-            check(lib().rgbl_resident_stage_stereo(self.ctx.handle, slot, self.T, ia, ra, self.W, self.H, self.W), self.ctx.handle)
-            return
-        if self.kind == "rgbd":
-            da = (C.c_void_p * self.T)(*[self.dep[m, f].ctypes.data for f in range(self.T)])
-            check(lib().rgbl_resident_stage_rgbd(self.ctx.handle, slot, self.T, ia, self.W, self.H, self.W, da, self.W), self.ctx.handle)
-            return
-        pa = (C.c_void_p * self.T)(*[self.pts[m, f].ctypes.data for f in range(self.T)])
-        n = np.ascontiguousarray(self.npts[m])
-        check(lib().rgbl_resident_stage(self.ctx.handle, slot, self.T, ia, self.W, self.H, self.W, pa, ptr(n)), self.ctx.handle)
+            check(lib().rgbl_resident_stage_stereo(h, slot, T, ia, sa, W, H, W), h)
+        elif self.kind == "rgbd":
+            check(lib().rgbl_resident_stage_rgbd(h, slot, T, ia, W, H, W, sa, W), h)
+        else:
+            check(lib().rgbl_resident_stage(h, slot, T, ia, W, H, W, sa, ptr(np.ascontiguousarray(self.npts[m]))), h)
 
     def _outputs(self, nb, want_frames):
         n = nb * self.T
@@ -860,41 +835,33 @@ class SequenceRunner:
         o = self._outputs(n_batches, want_frames)
         io = SequenceIO()
         io.n_batches, io.frames_per_batch, io.width, io.height, io.stride = n_batches, T, self.W, self.H, self.W
-        keep = []
-        da = None
+        sa = na = None
         if resident_slots > 0:
-            io.gray = None; io.pts4xn = None; io.n_pts = None; io.n_slots = resident_slots; io.first_slot = first % resident_slots
-        elif self.kind != "rgbl":
-            idx = [(first + b) % self.M for b in range(n_batches)]
-            other = self.dep if self.kind == "rgbd" else self.right
-            ga = (C.c_void_p * (n_batches * T))(*[self.img[m, f].ctypes.data for m in idx for f in range(T)])
-            da = (C.c_void_p * (n_batches * T))(*[other[m, f].ctypes.data for m in idx for f in range(T)])
-            keep += [ga, da]
-            io.gray = C.cast(ga, C.c_void_p); io.pts4xn = None; io.n_pts = None
+            io.n_slots = resident_slots; io.first_slot = first % resident_slots
         else:
             idx = [(first + b) % self.M for b in range(n_batches)]
-            ga = (C.c_void_p * (n_batches * T))(*[self.img[m, f].ctypes.data for m in idx for f in range(T)])
-            pa = (C.c_void_p * (n_batches * T))(*[self.pts[m, f].ctypes.data for m in idx for f in range(T)])
-            na = np.ascontiguousarray(np.concatenate([self.npts[m] for m in idx]).astype(np.int32))
-            keep += [ga, pa, na]
-            io.gray = C.cast(ga, C.c_void_p); io.pts4xn = C.cast(pa, C.c_void_p); io.n_pts = na.ctypes.data
+            ga, sa = self._frames(self.img, idx), self._frames(self.second, idx)
+            io.gray = C.cast(ga, C.c_void_p)
+            if self.kind == "rgbl":
+                na = np.ascontiguousarray(np.concatenate([self.npts[m] for m in idx]).astype(np.int32))
+                io.pts4xn = C.cast(sa, C.c_void_p); io.n_pts = na.ctypes.data
         io.poses = o["poses"].ctypes.data; io.n_matches = o["n_matches"].ctypes.data; io.n_inliers = o["n_inliers"].ctypes.data
         io.n_local_matches = o["n_local_matches"].ctypes.data
         if want_frames:
             io.kps = o["kps"].ctypes.data; io.desc = o["desc"].ctypes.data; io.depth = o["depth"].ctypes.data; io.uright = o["uright"].ctypes.data
             io.cap = self.ctx.cap; io.n_kp = o["n_kp"].ctypes.data
+        h = self.ctx.handle
         if self.kind == "stereo":
-            check(lib().rgbl_track_sequence_stereo(self.ctx.handle, self.mb, self.mbf, C.byref(chain), C.byref(io), da), self.ctx.handle)
+            check(lib().rgbl_track_sequence_stereo(h, self.mb, self.mbf, C.byref(chain), C.byref(io), sa), h)
         elif self.kind == "rgbd":
-            check(lib().rgbl_track_sequence_rgbd(self.ctx.handle, self.depth_scale, self.bf, C.byref(chain), C.byref(io), da, self.W), self.ctx.handle)
+            check(lib().rgbl_track_sequence_rgbd(h, self.depth_scale, self.bf, C.byref(chain), C.byref(io), sa, self.W), h)
         else:
-            check(lib().rgbl_track_sequence(self.ctx.handle, ptr(self.P), C.byref(self.prm), C.byref(chain), C.byref(io)), self.ctx.handle)
+            check(lib().rgbl_track_sequence(h, ptr(self.P), C.byref(self.prm), C.byref(chain), C.byref(io)), h)
         return o
 
     def h2d_bytes_per_batch(self) -> float:
-        if self.kind != "rgbl":
-            return float(self.T * self.W * self.H * (3 if self.kind == "rgbd" else 2))
-        return float(self.T * self.W * self.H + 16.0 * self.npts.sum() / self.M)
+        second = 16.0 * self.npts.sum() / self.M if self.kind == "rgbl" else self.T * self.second[0, 0].nbytes
+        return float(self.T * self.W * self.H + second)
 
     def d2h_bytes_per_batch(self, want_frames: bool) -> float:
         b = self.T * (7 * 4 + 3 * 4)
