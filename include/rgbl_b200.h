@@ -461,7 +461,7 @@ int rgbl_set_camera_distortion(rgbl_ctx* ctx, float fx, float fy, float cx, floa
 int rgbl_resident_download_keys_un(rgbl_ctx* ctx, rgbl_keypoint* kps_un, int cap, int* n_out);
 
 /* Keypoint distribution (DistributeOctTree) runs on the device by default (one CTA per (frame, level)); on != 0
- * selects the host implementation instead (also: environment RGBL_HOST_QUADTREE=1).  Both are exact.           */
+ * selects the host implementation instead.  Both are exact.                                                     */
 int rgbl_set_host_quadtree(rgbl_ctx* ctx, int on);
 
 /* CUDA-event stopwatch on the context's main stream: mark(0) ... work ... mark(1); elapsed = device time

@@ -95,9 +95,8 @@ static int create(const rgbl_config* cfg, Ctx** out) {
         }
         int dev_smem = 0;
         cudaDeviceGetAttribute(&dev_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, cfg->device);
-        const char* env = getenv("RGBL_HOST_QUADTREE");
         c->qt_device_ok = fits && dev_smem >= quadtree_smem_bytes();
-        c->device_quadtree = c->qt_device_ok && !(env && env[0] == '1');
+        c->device_quadtree = c->qt_device_ok;
         CUF(c->d_lvl_region.alloc(nl + 1));
         CUF(cudaMemcpy(c->d_lvl_region, region.data(), (nl + 1) * sizeof(int), cudaMemcpyHostToDevice));
         CUF(c->d_sel_lvl.alloc((size_t)B * c->cap_kp));
@@ -108,21 +107,12 @@ static int create(const rgbl_config* cfg, Ctx** out) {
         CUF(c->qt_quad.alloc(c->dense_cap));
         c->qt_scr = QtScratchDev{c->qt_perm_a, c->qt_perm_b, c->qt_node_a, c->qt_node_b, c->qt_scan, c->qt_quad};
     }
-    {   // strip FAST, staged describe, dilation with the empty-tile shortcut: bit-exact twins of the round-1 kernels and
-        // faster, hence the defaults; RGBL_<NAME>=0 selects the round-1 kernel for A/B runs
-        const char* envd = getenv("RGBL_DESCRIBE_STAGED");
-        c->describe_staged = !(envd && envd[0] == '0');
-        const char* envl = getenv("RGBL_DILATE_V2");
-        c->dilate_v2 = !(envl && envl[0] == '0');
+    {   // fused TMA level kernel unless RGBL_LEVEL_TMA=0 or its tensor maps cannot be made; the cell strips of the FAST kernel
         const char* envt = getenv("RGBL_LEVEL_TMA");
         c->level_tma = !(envt && envt[0] == '0') && make_level_tensor_maps(c->d_pyr, c->frame_bytes, B, c->levels.data(), nl, &c->level_tms) == 0;
-        const char* env = getenv("RGBL_FAST_STRIPS");
-        if (!(env && env[0] == '0')) {
-            build_fast_strips(c->cells, 8, 264, c->strips, c->strip_rows_cap, c->strip_list_cap);
-            CUF(c->d_strips.alloc(c->strips.size()));
-            CUF(cudaMemcpy(c->d_strips, c->strips.data(), c->strips.size() * sizeof(StripInfo), cudaMemcpyHostToDevice));
-            c->fast_strips = true;
-        }
+        build_fast_strips(c->cells, 8, 264, c->strips, c->strip_rows_cap, c->strip_list_cap);
+        CUF(c->d_strips.alloc(c->strips.size()));
+        CUF(cudaMemcpy(c->d_strips, c->strips.data(), c->strips.size() * sizeof(StripInfo), cudaMemcpyHostToDevice));
     }
     CUF(c->d_sel.alloc((size_t)B * c->cap_kp));
     CUF(c->d_n_sel.alloc((size_t)B));
@@ -220,15 +210,10 @@ static int run_extract(Ctx* c, int n_frames, const std::function<void()>& aux_wo
     if (!fused_levels) launch_pyramid(c->st, c->d_pyr, c->frame_bytes, c->levels.data(), nl, c->d_coefs, n_frames);
     stage_end(c, ST_PYRAMID, c->st, level0_launches + (fused_levels ? nl : nl - 1));
     stage_begin(c, ST_FAST, c->st);
-    if (c->fast_strips) {
-        if (launch_fast_strips(c->st, c->d_pyr, c->frame_bytes, c->d_levels, c->d_cells, c->n_cells, c->d_strips, (int)c->strips.size(),
-                               c->strip_rows_cap, c->strip_list_cap, c->cfg.orb.ini_th_fast, c->cfg.orb.min_th_fast, c->d_slots,
-                               c->d_counts, c->d_overflow, n_frames) != 0) {
-            c->err = "strip FAST kernel needs more shared memory than this device allows"; return RGBL_E_CUDA;
-        }
-    } else {
-        launch_fast(c->st, c->d_pyr, c->frame_bytes, c->d_levels, c->d_cells, c->n_cells, c->cfg.orb.ini_th_fast,
-                    c->cfg.orb.min_th_fast, c->d_slots, c->d_counts, c->d_overflow, n_frames);
+    if (launch_fast_strips(c->st, c->d_pyr, c->frame_bytes, c->d_levels, c->d_cells, c->n_cells, c->d_strips, (int)c->strips.size(),
+                           c->strip_rows_cap, c->strip_list_cap, c->cfg.orb.ini_th_fast, c->cfg.orb.min_th_fast, c->d_slots,
+                           c->d_counts, c->d_overflow, n_frames) != 0) {
+        c->err = "strip FAST kernel needs more shared memory than this device allows"; return RGBL_E_CUDA;
     }
     stage_end(c, ST_FAST, c->st, 1);
     stage_begin(c, ST_COMPACT, c->st);
@@ -255,9 +240,8 @@ static int run_extract(Ctx* c, int n_frames, const std::function<void()>& aux_wo
         stage_end(c, ST_QUADTREE, c->st, 2);
         CU(cudaStreamWaitEvent(c->st, c->ev_blur, 0));
         stage_begin(c, ST_DESCRIBE, c->st);
-        (c->describe_staged ? launch_describe_staged : launch_describe)(c->st, c->d_pyr, c->d_blur, c->frame_bytes, c->d_levels, c->d_sel,
-                                                                        c->d_n_sel, c->cap_kp, c->cap_kp, c->tab.umax, c->d_kps, c->d_desc,
-                                                                        n_frames);
+        launch_describe_staged(c->st, c->d_pyr, c->d_blur, c->frame_bytes, c->d_levels, c->d_sel, c->d_n_sel, c->cap_kp, c->cap_kp, c->tab.umax,
+                               c->d_kps, c->d_desc, n_frames);
         stage_end(c, ST_DESCRIBE, c->st, 1);
         CU(cudaGetLastError());
         c->last_frames = n_frames;
@@ -341,8 +325,8 @@ static int run_extract(Ctx* c, int n_frames, const std::function<void()>& aux_wo
     CU(cudaMemcpyAsync(c->d_n_sel, c->h_n_sel, (size_t)n_frames * sizeof(int), cudaMemcpyHostToDevice, c->st));
     CU(cudaStreamWaitEvent(c->st, c->ev_blur, 0));
     stage_begin(c, ST_DESCRIBE, c->st);
-    (c->describe_staged ? launch_describe_staged : launch_describe)(c->st, c->d_pyr, c->d_blur, c->frame_bytes, c->d_levels, c->d_sel,
-                                                                    c->d_n_sel, c->cap_kp, max_n, c->tab.umax, c->d_kps, c->d_desc, n_frames);
+    launch_describe_staged(c->st, c->d_pyr, c->d_blur, c->frame_bytes, c->d_levels, c->d_sel, c->d_n_sel, c->cap_kp, max_n, c->tab.umax,
+                           c->d_kps, c->d_desc, n_frames);
     stage_end(c, ST_DESCRIBE, c->st, max_n > 0 ? 1 : 0);
     CU(cudaGetLastError());
     c->last_frames = n_frames;
@@ -360,7 +344,7 @@ static int fetch_counts(Ctx* c, int n_frames) {
     if (c->h_overflow[0] || c->h_overflow[1]) {
         const int a = c->h_overflow[0], b = c->h_overflow[1];
         cudaMemsetAsync(c->d_overflow, 0, 2 * sizeof(int), c->st);
-        c->err = b ? "device quad-tree capacity exceeded (set RGBL_HOST_QUADTREE=1)" : (a == 1 ? "FAST cell slot overflow (>256 survivors in one cell)" : "candidate buffer overflow: raise max_candidates");
+        c->err = b ? "device quad-tree capacity exceeded (select the host quad-tree: rgbl_set_host_quadtree)" : (a == 1 ? "FAST cell slot overflow (>256 survivors in one cell)" : "candidate buffer overflow: raise max_candidates");
         return RGBL_E_CAPACITY;
     }
     return RGBL_OK;
@@ -375,8 +359,8 @@ static void run_depth_maps(Ctx* c, const DepthDev& dd, int n_frames, int max_pts
     stage_begin(c, ST_DEPTH_DILATE, st);
     const bool need_raw = dd.method == RGBL_DEPTH_AVERAGE_FILTERING || dd.method == RGBL_DEPTH_NEAREST_NEIGHBOR_PIXEL;
     float* raw_out = need_raw ? c->d_raw : raw;
-    (c->dilate_v2 ? launch_depth_resolve_dilate_v2 : launch_depth_resolve_dilate)(st, c->d_pts, 4 * c->cfg.max_points, c->d_n_pts, dd, W, H, c->d_idx_map,
-                                                                                  c->stamp, raw_out, c->d_processed, n_frames);
+    launch_depth_resolve_dilate_v2(st, c->d_pts, 4 * c->cfg.max_points, c->d_n_pts, dd, W, H, c->d_idx_map, c->stamp, raw_out, c->d_processed,
+                                   n_frames);
     int launches = 1;
     if (dd.method == RGBL_DEPTH_AVERAGE_FILTERING) { launch_depth_average_filter(st, c->d_raw, W, H, dd.avg_kernel, c->d_processed, n_frames); ++launches; }
     stage_end(c, ST_DEPTH_DILATE, st, launches);

@@ -1,7 +1,7 @@
-// DepthModule::Upsample_InverseDilation (src/DepthModule.cc:230-274): the default kernel since round 2 (RGBL_DILATE_V2=0 selects
-// depth_resolve_dilate_kernel of depth_kernels.cu); validated on the CUDA-on-CPU shim and on the GPU against the oracle.
-//
-// Against that first kernel, results identical by construction (max is exact and order-free):
+// DepthModule::Upsample_InverseDilation (src/DepthModule.cc:230-274); validated on the CUDA-on-CPU shim and on the GPU against the oracle.
+// Per 32 x 32 tile: recompute the winning point's depth of every pixel of the tile and its halo (same arithmetic as depth_project_kernel),
+// build the inverted map t = M - d (zeroed above M-1), take the max over the structuring element, invert back: the exact float pipeline
+// of the reference.  Max is exact and order-free, so the following shortcuts do not change a bit:
 //   * a tile whose staged window holds no LiDAR return skips the structuring-element loop: every in-image value of the inverted
 //     map is 0 there, so the output is 0 whatever the element is (most of the upper half of a KITTI frame);
 //   * the (dy, dx) taps are turned once per CTA into shared-memory offsets, so a tap costs two shared loads and one FMNMX

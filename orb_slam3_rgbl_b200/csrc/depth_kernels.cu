@@ -6,20 +6,15 @@
 //              The reference scatters sequentially, so the LAST point in file order owns a pixel:
 //              atomicMax on (stamp << 22 | point_index+1).  The per-call stamp makes stale entries of
 //              earlier frames lose automatically, so the index map is never cleared on the hot path.
-//   resolve+dilate : per tile, recompute the winning point's depth (same arithmetic), build the
-//              inverted map t = M - d (zeroed above M-1), take the max over the structuring element,
-//              invert back: the exact float pipeline of Upsample_InverseDilation.
+//   resolve+dilate : depth_dilate_v2.cu.
 //   gather   : GetFeatureDepthFromDepthMap (:82-104), and Frame::ComputeStereoFromRGBD (src/Frame.cc:1074-1095) on a uint16 RGB-D plane.
 //   undistort: Frame::UndistortKeyPoints (src/Frame.cc:837-869), mvKeys -> mvKeysUn of a distorted camera, before the gather.
-#include <cfloat>
-
 #include "rgbl_device.cuh"
 #include "rgbl_kernels.h"
 
 namespace rgbl {
 
 constexpr int kStampShift = 22;
-constexpr uint32_t kIdxMask = (1u << kStampShift) - 1u;
 
 __device__ __forceinline__ float project_row(const float* P, float x, float y, float z, float o) {
     double acc = __dmul_rn((double)P[0], (double)x);
@@ -58,63 +53,6 @@ __global__ void __launch_bounds__(256) deinterleave_xyzr_kernel(const float* __r
     const float4 r = __ldg(reinterpret_cast<const float4*>(raw + (size_t)frame * pts_stride) + i);
     float* X = pts + (size_t)frame * pts_stride;
     X[i] = r.x; X[n + i] = r.y; X[2 * (size_t)n + i] = r.z; X[3 * (size_t)n + i] = 1.0f;
-}
-
-struct DilateTaps { int n; int8_t dx[81], dy[81]; };
-
-__global__ void __launch_bounds__(256) depth_resolve_dilate_kernel(const float* __restrict__ pts, int pts_stride,
-                                                                   const int* __restrict__ n_pts, DepthDev prm,
-                                                                   DilateTaps taps, int W, int H,
-                                                                   const uint32_t* __restrict__ idx_map,
-                                                                   uint32_t stamp, float* __restrict__ raw,
-                                                                   float* __restrict__ processed) {
-    constexpr int TW = 32, TH = 32, HALO = 4, SW = TW + 2 * HALO, SH = TH + 2 * HALO;
-    __shared__ float t[SH][SW + 1];
-    const int frame = blockIdx.z, tid = threadIdx.x;
-    const int lx = tid & 31, ly = tid >> 5;
-    const int x0 = blockIdx.x * TW, y0 = blockIdx.y * TH;
-    const int n = n_pts[frame];
-    const float* X = pts + (size_t)frame * pts_stride;
-    const uint32_t* im = idx_map + (size_t)frame * W * H;
-    const float M = prm.inv_scale_m, thr = __fsub_rn(M, 1.0f);
-
-    // rows: warp `ly` handles rows ly, ly+8, ...; lanes cover the 40 columns in two passes
-    for (int r = ly; r < SH; r += 8) {
-        const int gy = y0 + r - HALO;
-#pragma unroll
-        for (int cc = 0; cc < 2; ++cc) {
-            const int c = lx + 32 * cc;
-            if (c >= SW) break;
-            const int gx = x0 + c - HALO;
-            float tv = -FLT_MAX;                      // out-of-image taps are ignored by cv::dilate
-            if (gx >= 0 && gx < W && gy >= 0 && gy < H) {
-                const uint32_t e = __ldg(im + (size_t)gy * W + gx);
-                float d = 0.f;
-                if ((e >> kStampShift) == stamp) {
-                    const int p = (int)(e & kIdxMask) - 1;
-                    d = project_row(prm.P + 8, __ldg(X + p), __ldg(X + n + p), __ldg(X + 2 * (size_t)n + p),
-                                    __ldg(X + 3 * (size_t)n + p));
-                }
-                const bool interior = (r >= HALO && r < HALO + TH && c >= HALO && c < HALO + TW);
-                if (interior && raw) raw[(size_t)frame * W * H + (size_t)gy * W + gx] = d;
-                const float inv = __fsub_rn(M, d);
-                tv = (inv > thr) ? 0.f : inv;         // THRESH_TOZERO_INV at M-1
-            }
-            t[r][c] = tv;
-        }
-    }
-    __syncthreads();
-    const int gx = x0 + lx;
-    if (gx >= W) return;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const int r = ly + 8 * k, gy = y0 + r;
-        if (gy >= H) break;
-        float best = -FLT_MAX;
-        for (int q = 0; q < taps.n; ++q) best = fmaxf(best, t[r + HALO + taps.dy[q]][lx + HALO + taps.dx[q]]);
-        const float o = __fsub_rn(M, best);
-        processed[(size_t)frame * W * H + (size_t)gy * W + gx] = (o > thr) ? 0.f : o;
-    }
 }
 
 // The plane holds metric depth (float: the processed LiDAR depth map, or a scaled RGB-D map) or the raw 16-bit RGB-D samples, scaled here
@@ -274,19 +212,6 @@ void launch_depth_project(cudaStream_t st, const float* pts, int pts_stride, con
 void launch_deinterleave_xyzr(cudaStream_t st, const float* raw, float* pts, int pts_stride, const int* n_pts, int max_n_pts, int n_frames) {
     if (max_n_pts <= 0) return;
     deinterleave_xyzr_kernel<<<dim3((max_n_pts + 255) / 256, n_frames), 256, 0, st>>>(raw, pts, pts_stride, n_pts);
-}
-
-void launch_depth_resolve_dilate(cudaStream_t st, const float* pts, int pts_stride, const int* n_pts,
-                                 const DepthDev& prm, int W, int H, const uint32_t* idx_map, uint32_t stamp,
-                                 float* raw, float* processed, int n_frames) {
-    DilateTaps taps;
-    taps.n = 0;
-    const int ax = prm.ku / 2, ay = prm.kv / 2;
-    for (int j = 0; j < prm.kv; ++j)
-        for (int i = 0; i < prm.ku; ++i)
-            if (prm.mask[j * prm.ku + i]) { taps.dx[taps.n] = (int8_t)(i - ax); taps.dy[taps.n] = (int8_t)(j - ay); ++taps.n; }
-    depth_resolve_dilate_kernel<<<dim3((W + 31) / 32, (H + 31) / 32, n_frames), 256, 0, st>>>(
-        pts, pts_stride, n_pts, prm, taps, W, H, idx_map, stamp, raw, processed);
 }
 
 void launch_depth_gather(cudaStream_t st, const float* processed, int W, int H, const rgbl_keypoint* kps,

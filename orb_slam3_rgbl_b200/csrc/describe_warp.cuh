@@ -1,9 +1,9 @@
 // Warp-per-keypoint orientation + steered BRIEF with the two pixel neighbourhoods staged in shared memory
 // (IC_Angle src/ORBextractor.cc:76-103, computeOrbDescriptor :107-146).
 //
-// Why: describe_kernel (orb_kernels.cu) maps lane <-> ROW of the radius-15 disc and gathers the 512 BRIEF samples straight
-// from global memory, so almost every one of its ~47 load instructions touches ~32 different cache lines (≈ 1.5 k L1
-// wavefronts per keypoint, the bound of that kernel).  Here the 31 x 31 patch of the level and the 37 x 37 window of the
+// Why: a warp that maps lane <-> ROW of the radius-15 disc and gathers the 512 BRIEF samples straight from global memory
+// touches ~32 different cache lines with almost every one of its ~47 load instructions (≈ 1.5 k L1 wavefronts per keypoint,
+// the bound of that formulation).  Here the 31 x 31 patch of the level and the 37 x 37 window of the
 // blurred level (|rotated pattern coordinate| <= round(13 * sqrt 2) = 18) are copied with aligned 32-bit loads of
 // consecutive words (≈ 22 load instructions, 1-2 lines each); the centroid sums then run lane <-> COLUMN (a row of the
 // patch is one shared-memory wavefront) and the BRIEF samples are shared-memory byte reads.  All sums are integer, the

@@ -1,6 +1,5 @@
-// Staged variant of describe_kernel (describe_warp.cuh): kernel, launcher, host twin and its test hook.
-// The default describe kernel since round 2 (RGBL_DESCRIBE_STAGED=0 selects describe_kernel of orb_kernels.cu); host twin checked against the oracle on
-// the CPU (tests/test_host_abi.py), device path on the CUDA-on-CPU shim and on the GPU.
+// Describe kernel (staged formulation, describe_warp.cuh): kernel, launcher, host twin and its test hook.  Host twin checked against
+// the oracle on the CPU (tests/test_host_abi.py), device path on the CUDA-on-CPU shim and on the GPU.
 #include <cmath>
 #include <cstring>
 #include <string>

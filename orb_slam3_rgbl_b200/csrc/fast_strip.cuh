@@ -7,7 +7,7 @@
 //   * non-maximum suppression: neighbours outside the cell's tested region count as 0 (cv::FAST never scores them),
 //   * the iniTh -> minTh fallback, decided per cell ("no keypoint at iniTh in this cell"),
 //   * the output order: row-major inside the cell, cells in table order.
-// So a strip scores every pixel once (the per-cell kernel re-reads the 3 px halo of every cell and pays its fixed costs
+// So a strip scores every pixel once (a CTA per cell would re-read the 3 px halo of every cell and pay its fixed costs
 // per 30 x 30 px), masks the NMS comparisons at the inner cell boundaries, and emits per cell.
 //
 // The body is bulk-synchronous (FS_FOR loops separated by FS_SYNC) and compiles for the host as well, where every phase

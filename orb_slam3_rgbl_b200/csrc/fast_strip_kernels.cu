@@ -1,5 +1,4 @@
-// Strip variant of the per-cell FAST kernel (fast_strip.cuh): kernel wrapper, launcher, host twin and its test hook.
-// The default FAST kernel since round 2 (RGBL_FAST_STRIPS=0 selects the per-cell kernel of orb_kernels.cu); the host twin is checked
+// FAST kernel (strip formulation, fast_strip.cuh): kernel wrapper, launcher, host twin and its test hook.  The host twin is checked
 // against the oracle on the CPU (tests/test_host_abi.py), the device path on the CUDA-on-CPU shim and on the GPU.
 #include <cstring>
 #include <string>

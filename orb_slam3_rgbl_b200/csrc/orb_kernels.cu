@@ -1,5 +1,5 @@
-// ORB extractor kernels for sm_90a: pyramid, per-cell FAST-9/16 + cell-local NMS, candidate
-// compaction, 7x7 Gaussian pre-filter, and the fused orientation + rBRIEF describe kernel.
+// ORB extractor kernels for sm_90a: pyramid, candidate compaction, 7x7 Gaussian pre-filter and the
+// padded copy of a level.
 // Reference semantics: src/ORBextractor.cc (cited per kernel) with the OpenCV primitives restated
 // in integer/fixed-point form (SURVEY.md Appendix A).  Every frame of a batch is processed by the
 // same launch (blockIdx.z / blockIdx.y = frame slot).
@@ -98,162 +98,6 @@ __global__ void __launch_bounds__(256) resize_level_gather_kernel(uint8_t* __res
         }
     }
     *reinterpret_cast<uint32_t*>(d + (size_t)y * dst.pitch + x4) = out;
-}
-
-// ------------------------------------------------------------------------------------------------
-// FAST: one CTA per (cell, frame).  Equivalent of the per-cell cv::FAST(th=iniTh, nms) with the
-// cv::FAST(th=minTh, nms) fallback when the first call returns nothing (src/ORBextractor.cc:805-868).
-//   score(p) = K-1 with K the arc strength (corner at threshold t  <=>  K > t  <=>  score >= t);
-//   NMS survivors at minTh = {s >= minTh, s > all 8 neighbours (non-corners / outside the window = 0)};
-//   survivors at iniTh = survivors at minTh with s >= iniTh (a weaker neighbour never suppresses).
-// Survivors are written in row-major order (the order cv::FAST returns) into the cell's slot array.
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ bool fast_quick_test(const uint8_t* p, int th) {
-    constexpr int P = kFastTilePitch;
-    const int v = p[0];
-    const int r0 = p[3 * P], r4 = p[3], r8 = p[-3 * P], r12 = p[-3];
-    const int hi_t = v + th, lo_t = v - th;
-    const int ndark = (r0 < lo_t) + (r4 < lo_t) + (r8 < lo_t) + (r12 < lo_t);
-    const int nbright = (r0 > hi_t) + (r4 > hi_t) + (r8 > hi_t) + (r12 > hi_t);
-    return ndark >= 2 || nbright >= 2;           // a 9-arc always covers >= 2 of the 4 compass points
-}
-
-__device__ __forceinline__ int fast_score_at(const uint8_t* p, int th) {
-    constexpr int P = kFastTilePitch;
-    const int v = p[0];
-    int r[16];
-    r[0] = p[3 * P]; r[4] = p[3]; r[8] = p[-3 * P]; r[12] = p[-3];
-    r[1] = p[3 * P + 1];  r[2] = p[2 * P + 2];   r[3] = p[P + 3];
-    r[5] = p[-P + 3];     r[6] = p[-2 * P + 2];  r[7] = p[-3 * P + 1];
-    r[9] = p[-3 * P - 1]; r[10] = p[-2 * P - 2]; r[11] = p[-P - 3];
-    r[13] = p[P - 3];     r[14] = p[2 * P - 2];  r[15] = p[3 * P - 1];
-    const int K = fast_arc_strength16(v, r);
-    return (K > th) ? (K - 1) : 0;
-}
-
-// Phases: (1) window -> shared memory with aligned 32-bit loads; (2) high-speed test on every tested pixel,
-// survivors appended (warp ballot) to a shared list; (3) full arc score only for the listed pixels, densely
-// packed across the CTA (the heavy path no longer runs divergently on whole warps); (4) cell-local NMS +
-// threshold fallback + ordered emission.
-__global__ void __launch_bounds__(256) fast_cells_kernel(const uint8_t* __restrict__ pyr, size_t frame_stride,
-                                                         const LevelGeom* __restrict__ levels,
-                                                         const CellInfo* __restrict__ cells, int n_cells,
-                                                         int ini_th, int min_th,
-                                                         uint32_t* __restrict__ slots, int* __restrict__ counts,
-                                                         int* __restrict__ overflow) {
-    constexpr int P = kFastTilePitch;            // 88: 3 alignment bytes + 78-byte window, multiple of 4
-    constexpr int ROWS = kFastTilePitch - 8;     // 80 >= max window height 78
-    __shared__ __align__(16) uint8_t tile[P * ROWS];
-    __shared__ __align__(16) uint8_t sc[P * ROWS];
-    __shared__ uint16_t list[72 * 72 + 32];
-    __shared__ int warp_sums[8];
-    __shared__ int n_list;
-
-    const int cell = blockIdx.x, frame = blockIdx.y, tid = threadIdx.x;
-    const int lane = tid & 31, warp = tid >> 5;
-    const CellInfo ci = cells[cell];
-    const LevelGeom lg = levels[ci.level];
-    const int cw = ci.cw, ch = ci.ch;
-    const int a = ci.x0 & 3;                      // byte offset of the window inside its first aligned word
-    const uint8_t* src = pyr + (size_t)frame * frame_stride + lg.off + (size_t)ci.y0 * lg.pitch + (ci.x0 - a);
-    const int nw = (cw + a + 3) >> 2;             // words per row (<= 21)
-
-    if (tid == 0) n_list = 0;
-    for (int y = warp; y < ch; y += 8) {
-        const uint32_t* g = reinterpret_cast<const uint32_t*>(src + (size_t)y * lg.pitch);
-        uint32_t* t = reinterpret_cast<uint32_t*>(tile + y * P);
-        uint32_t* z = reinterpret_cast<uint32_t*>(sc + y * P);
-        if (lane < nw) { t[lane] = __ldg(g + lane); z[lane] = 0; }
-    }
-    __syncthreads();
-
-    const int tw = cw - 6, th = ch - 6;          // tested region [3, cw-3) x [3, ch-3)
-    const int n_t = (tw > 0 && th > 0) ? tw * th : 0;
-    {
-        // incremental (x, y) of flattened index i = tid + 256*k without per-iteration divisions
-        const int q = (tw > 0) ? 256 / tw : 0, r = (tw > 0) ? 256 - q * tw : 0;
-        int y = (tw > 0) ? tid / tw : 0, x = tid - y * tw;
-        for (int i0 = 0; i0 < n_t; i0 += 256) {
-            const bool valid = (i0 + tid) < n_t;
-            bool pass = false;
-            int pos = 0;
-            if (valid) {
-                pos = (y + 3) * P + x + 3 + a;
-                pass = fast_quick_test(&tile[pos], min_th);
-            }
-            const uint32_t m = __ballot_sync(0xffffffffu, pass);
-            int base = 0;
-            if (lane == 0 && m) base = atomicAdd(&n_list, __popc(m));
-            base = __shfl_sync(0xffffffffu, base, 0);
-            if (pass) list[base + __popc(m & ((1u << lane) - 1u))] = (uint16_t)pos;
-            x += r; y += q;
-            if (x >= tw) { x -= tw; ++y; }
-        }
-    }
-    __syncthreads();
-    const int nl = n_list;
-    for (int j = tid; j < nl; j += 256) {
-        const int pos = list[j];
-        sc[pos] = (uint8_t)fast_score_at(&tile[pos], min_th);
-    }
-    __syncthreads();
-
-    // contiguous row-major chunk per thread -> ordered emission
-    const int per = (n_t + 255) / 256;           // <= 21 for windows <= 78 px
-    const int beg = min(tid * per, n_t), end = min(beg + per, n_t);
-    uint32_t m_min = 0, m_ini = 0;
-    int y0c = (tw > 0) ? beg / tw : 0, x0c = beg - y0c * tw;
-    {
-        int y = y0c, x = x0c;
-        for (int i = beg; i < end; ++i) {
-            const uint8_t* c = &sc[(y + 3) * P + x + 3 + a];
-            const int s = c[0];
-            if (s != 0) {
-                const bool keep = s > c[-1] && s > c[1] && s > c[-P - 1] && s > c[-P] && s > c[-P + 1] &&
-                                  s > c[P - 1] && s > c[P] && s > c[P + 1];
-                if (keep) {
-                    m_min |= 1u << (i - beg);
-                    if (s >= ini_th) m_ini |= 1u << (i - beg);
-                }
-            }
-            if (++x == tw) { x = 0; ++y; }
-        }
-    }
-    const int any_ini = __syncthreads_or(m_ini != 0);
-    const uint32_t m = any_ini ? m_ini : m_min;
-    const int cnt = __popc(m);
-
-    // block-wide exclusive scan of cnt
-    int incl = cnt;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int t = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += t;
-    }
-    if (lane == 31) warp_sums[warp] = incl;
-    __syncthreads();
-    int base = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) {
-        const int ws = warp_sums[w];
-        if (w < warp) base += ws;
-        total += ws;
-    }
-    int pos = base + incl - cnt;
-    uint32_t* out = slots + ((size_t)frame * n_cells + cell) * kCellCap;
-    uint32_t mm = m;
-    while (mm) {
-        const int b = __ffs(mm) - 1;
-        mm &= mm - 1;
-        int x = x0c + b, y = y0c;
-        while (x >= tw) { x -= tw; ++y; }
-        if (pos < kCellCap) out[pos] = pack_cand_dev(x + 3 + ci.off_x, y + 3 + ci.off_y, sc[(y + 3) * P + x + 3 + a]);
-        ++pos;
-    }
-    if (tid == 0) {
-        counts[(size_t)frame * n_cells + cell] = min(total, kCellCap);
-        if (total > kCellCap) atomicExch(overflow, 1);
-    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -409,83 +253,6 @@ __global__ void __launch_bounds__(256) blur_level_kernel(const uint8_t* __restri
     }
 }
 
-// ------------------------------------------------------------------------------------------------
-// Describe: one warp per selected keypoint.  IC_Angle (src/ORBextractor.cc:76-103) on the un-blurred
-// level, then computeOrbDescriptor (:107-146) on the blurred level, then the cv::KeyPoint record with
-// the level->image coordinate scaling of operator() (:1143-1151).
-// ------------------------------------------------------------------------------------------------
-__device__ const int8_t g_pattern[1024] = {
-#include "orb_pattern_31.inc"
-};
-
-struct UmaxTable { int v[16]; };
-
-__global__ void __launch_bounds__(256) describe_kernel(const uint8_t* __restrict__ pyr, const uint8_t* __restrict__ blur,
-                                                       size_t frame_stride, const LevelGeom* __restrict__ levels,
-                                                       const SelKp* __restrict__ sel, const int* __restrict__ n_sel,
-                                                       int cap, UmaxTable umax, rgbl_keypoint* __restrict__ kps,
-                                                       uint8_t* __restrict__ desc) {
-    const int frame = blockIdx.y;
-    const int k = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (k >= n_sel[frame]) return;
-    const SelKp kp = sel[(size_t)frame * cap + k];
-    const LevelGeom lg = levels[kp.level];
-    const uint8_t* img = pyr + (size_t)frame * frame_stride + lg.off;
-    const uint8_t* c = img + (size_t)kp.y * lg.pitch + kp.x;
-
-    // intensity centroid: lane <-> row v = lane-15 of the radius-15 disc (lane 31 idle)
-    int m10 = 0, m01 = 0;
-    if (lane < 31) {
-        const int v = lane - kHalfPatch;
-        const int dmax = umax.v[v < 0 ? -v : v];
-        const uint8_t* row = c + v * lg.pitch;
-        int rs = 0;
-        for (int u = -dmax; u <= dmax; ++u) {
-            const int val = __ldg(row + u);
-            m10 += u * val;
-            rs += val;
-        }
-        m01 = v * rs;
-    }
-    m10 = __reduce_add_sync(0xffffffffu, m10);
-    m01 = __reduce_add_sync(0xffffffffu, m01);
-    const float angle = fast_atan2_deg((float)m01, (float)m10);
-
-    // steered BRIEF: lane i computes descriptor byte i (8 comparisons, 16 samples)
-    const float factor_pi = (float)(3.14159265358979323846 / 180.0);
-    float a, b;
-    glibc_sincosf(__fmul_rn(angle, factor_pi), &b, &a);       // a = cos, b = sin
-    const uint8_t* bc = blur + (size_t)frame * frame_stride + lg.off + (size_t)kp.y * lg.pitch + kp.x;
-    const int8_t* pat = g_pattern + lane * 32;
-    int val = 0;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-        int t[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-            const float px = (float)pat[4 * j + 2 * e], py = (float)pat[4 * j + 2 * e + 1];
-            const int rr = __float2int_rn(__fadd_rn(__fmul_rn(px, b), __fmul_rn(py, a)));
-            const int cc = __float2int_rn(__fsub_rn(__fmul_rn(px, a), __fmul_rn(py, b)));
-            t[e] = __ldg(bc + rr * lg.pitch + cc);
-        }
-        val |= (t[0] < t[1]) << j;
-    }
-    desc[((size_t)frame * cap + k) * 32 + lane] = (uint8_t)val;
-
-    if (lane == 0) {
-        rgbl_keypoint o;
-        const float fx = (float)kp.x, fy = (float)kp.y;
-        o.x = (kp.level != 0) ? __fmul_rn(fx, lg.scale) : fx;
-        o.y = (kp.level != 0) ? __fmul_rn(fy, lg.scale) : fy;
-        o.size = (float)lg.scaled_patch;
-        o.angle = angle;
-        o.response = (float)kp.score;
-        o.octave = kp.level;
-        o.class_id = -1;
-        kps[(size_t)frame * cap + k] = o;
-    }
-}
-
 // mvImagePyramid[level] with its 19 px BORDER_REFLECT_101 frame (src/ORBextractor.cc:1185-1191),
 // synthesised on demand: the hot path itself never reads the border (SURVEY App. C).
 __global__ void padded_level_kernel(const uint8_t* __restrict__ pyr, size_t frame_stride, int frame, LevelGeom lg,
@@ -516,13 +283,6 @@ void launch_pyramid(cudaStream_t st, uint8_t* pyr, size_t frame_stride, const Le
     }
 }
 
-void launch_fast(cudaStream_t st, const uint8_t* pyr, size_t frame_stride, const LevelGeom* d_levels,
-                 const CellInfo* d_cells, int n_cells, int ini_th, int min_th, uint32_t* slots, int* counts,
-                 int* overflow, int n_frames) {
-    fast_cells_kernel<<<dim3(n_cells, n_frames), 256, 0, st>>>(pyr, frame_stride, d_levels, d_cells, n_cells, ini_th,
-                                                             min_th, slots, counts, overflow);
-}
-
 void launch_compact(cudaStream_t st, const LevelGeom* d_levels, int n_levels, int n_cells, const uint32_t* slots,
                     const int* counts, int* cell_off, int* level_cnt, int* frame_total, uint32_t* dense, int dense_cap,
                     int* overflow, int n_frames) {
@@ -539,16 +299,6 @@ void launch_blur(cudaStream_t st, const uint8_t* pyr, uint8_t* blur, size_t fram
         dim3 grd((lg.w + 127) / 128, (lg.h + 31) / 32, n_frames);
         blur_level_kernel<<<grd, 256, 0, st>>>(pyr, blur, frame_stride, lg);
     }
-}
-
-void launch_describe(cudaStream_t st, const uint8_t* pyr, const uint8_t* blur, size_t frame_stride,
-                     const LevelGeom* d_levels, const SelKp* sel, const int* n_sel, int cap, int max_n,
-                     const int umax[16], rgbl_keypoint* kps, uint8_t* desc, int n_frames) {
-    if (max_n <= 0) return;
-    UmaxTable t;
-    for (int i = 0; i < 16; ++i) t.v[i] = umax[i];
-    describe_kernel<<<dim3((max_n + 7) / 8, n_frames), 256, 0, st>>>(pyr, blur, frame_stride, d_levels, sel, n_sel, cap,
-                                                                   t, kps, desc);
 }
 
 void launch_padded_level(cudaStream_t st, const uint8_t* pyr, size_t frame_stride, int frame, const LevelGeom& lg,

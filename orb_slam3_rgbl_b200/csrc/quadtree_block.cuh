@@ -187,7 +187,6 @@ struct SharedT {
     SortItem open[2][MAXN];   // expandable children: [cur] produced by the last pass, [1-cur] being built
     int open_slot[MAXN * 4];  // per push index: position in the next open list, or -1
     int n_nodes, n_open, cur_tab, cur_open, n_div, total_push, n_keep, n_expand, scan_total, flag;
-    int block_sort;                // 1: block_std_sort (the default), 0: one-thread std_sort (RGBL_QT_BLOCK_SORT=0)
     int root_cnt[kMaxRoots + 1];
     unsigned long long scan_carry[1024 + 32];
 };
@@ -539,9 +538,8 @@ QT_BIG int divide_pass(SharedX& s, const unsigned int* cand, int n, Scratch g, i
 // configuration exceeds the on-chip capacities; the caller then uses the host implementation).
 template <class SharedX>
 QT_FN int distribute(SharedX& s, const unsigned int* cand, int n, int width, int height, int N, Scratch g,
-                     unsigned int* out, int out_cap, int block_sort = 0) {
+                     unsigned int* out, int out_cap) {
     if (n <= 0) return 0;
-    QT_SINGLE { s.block_sort = block_sort; }
 #if QT_DEVICE
     const int n_ini = (int)roundf(static_cast<float>(width) / height);
 #else
@@ -602,26 +600,15 @@ QT_FN int distribute(SharedX& s, const unsigned int* cand, int n, int width, int
     // ---- subdivision loop (src/ORBextractor.cc:609-755) ----
     for (;;) {
         const int prev = s.n_nodes;
-        {   // full pass: D = every node with more than one key, processed in list order
+        {   // full pass: D = every node with more than one key, processed in list order (ranks from a block scan of the flags)
             const auto& T = s.tab[s.cur_tab];
-            if (s.block_sort) {              // the same compaction through a block scan of the flags
-                QT_FOR(i, prev) s.pushbase[i] = (T.end[i] - T.beg[i] > 1) ? 1 : 0;
-                QT_SYNC();
-                scan_int(s.pushbase, prev, &s.n_div, s);
-                QT_SYNC();
-                QT_FOR(i, prev) {
-                    if (T.end[i] - T.beg[i] > 1) { const int r = s.pushbase[i]; s.proc[i] = (short)r; s.by_rank[r] = (short)i; }
-                    else s.proc[i] = -1;
-                }
-            } else {
-                QT_SINGLE {
-                    int r = 0;
-                    for (int i = 0; i < prev; ++i) {
-                        if (T.end[i] - T.beg[i] > 1) { s.proc[i] = (short)r; s.by_rank[r] = (short)i; ++r; }
-                        else s.proc[i] = -1;
-                    }
-                    s.n_div = r;
-                }
+            QT_FOR(i, prev) s.pushbase[i] = (T.end[i] - T.beg[i] > 1) ? 1 : 0;
+            QT_SYNC();
+            scan_int(s.pushbase, prev, &s.n_div, s);
+            QT_SYNC();
+            QT_FOR(i, prev) {
+                if (T.end[i] - T.beg[i] > 1) { const int r = s.pushbase[i]; s.proc[i] = (short)r; s.by_rank[r] = (short)i; }
+                else s.proc[i] = -1;
             }
             QT_SYNC();
         }
@@ -634,8 +621,7 @@ QT_FN int distribute(SharedX& s, const unsigned int* cand, int n, int width, int
             while (!done) {
                 const int prev2 = s.n_nodes;
                 const int n_open = s.n_open;
-                if (s.block_sort) block_std_sort(s, s.open[s.cur_open], s.open[s.cur_open ^ 1], n_open, -1);
-                else { QT_SINGLE { std_sort(s.open[s.cur_open], n_open); } }
+                block_std_sort(s, s.open[s.cur_open], s.open[s.cur_open ^ 1], n_open, -1);
                 QT_SYNC();
                 // child counts of every open node (they are all candidates for division)
                 {
@@ -658,37 +644,23 @@ QT_FN int distribute(SharedX& s, const unsigned int* cand, int n, int width, int
                         s.pushes[nd] = (short)(((mask >> 0) & 1) + ((mask >> 1) & 1) + ((mask >> 2) & 1) + ((mask >> 3) & 1));
                     }
                     QT_SYNC();
-                    if (s.block_sort) {
-                        // the list grows by pushes - 1 >= 0 per division: the sequential loop stops after the first rank
-                        // whose running size reaches N, i.e. m = 1 + #{r : size after r < N} (capped at n_open)
-                        QT_FOR(r, n_open) s.keepbase[r] = s.pushes[s.by_rank[r]] - 1;
-                        QT_SINGLE { s.n_div = 0; }
-                        QT_SYNC();
-                        scan_int(s.keepbase, n_open, &s.scan_total, s);
-                        QT_SYNC();
-                        QT_FOR(r, n_open) {
-                            const int incl = prev2 + ((r + 1 < n_open) ? s.keepbase[r + 1] : s.scan_total);
-                            const int incl_next = (r + 1 < n_open) ? prev2 + ((r + 2 < n_open) ? s.keepbase[r + 2] : s.scan_total) : N;
-                            if (r == 0 && incl >= N) s.n_div = 1;
-                            if (incl < N && incl_next >= N) s.n_div = (r + 2 < n_open) ? r + 2 : n_open;
-                        }
-                        QT_SYNC();
-                        {
-                            const int m = s.n_div;
-                            QT_FOR(r, n_open) if (r >= m) s.proc[s.by_rank[r]] = -1;
-                        }
-                    } else {
-                        QT_SINGLE {
-                            int size2 = prev2, m = 0;
-                            for (int r = 0; r < n_open; ++r) {
-                                size2 += s.pushes[s.by_rank[r]] - 1;
-                                ++m;
-                                if (size2 >= N) break;
-                            }
-                            // nodes beyond the break are not divided in this iteration
-                            for (int r = m; r < n_open; ++r) s.proc[s.by_rank[r]] = -1;
-                            s.n_div = m;
-                        }
+                    // the list grows by pushes - 1 >= 0 per division: the sequential loop stops after the first rank
+                    // whose running size reaches N, i.e. m = 1 + #{r : size after r < N} (capped at n_open)
+                    QT_FOR(r, n_open) s.keepbase[r] = s.pushes[s.by_rank[r]] - 1;
+                    QT_SINGLE { s.n_div = 0; }
+                    QT_SYNC();
+                    scan_int(s.keepbase, n_open, &s.scan_total, s);
+                    QT_SYNC();
+                    QT_FOR(r, n_open) {
+                        const int incl = prev2 + ((r + 1 < n_open) ? s.keepbase[r + 1] : s.scan_total);
+                        const int incl_next = (r + 1 < n_open) ? prev2 + ((r + 2 < n_open) ? s.keepbase[r + 2] : s.scan_total) : N;
+                        if (r == 0 && incl >= N) s.n_div = 1;
+                        if (incl < N && incl_next >= N) s.n_div = (r + 2 < n_open) ? r + 2 : n_open;
+                    }
+                    QT_SYNC();
+                    {   // nodes beyond the stopping rank are not divided in this iteration
+                        const int m = s.n_div;
+                        QT_FOR(r, n_open) if (r >= m) s.proc[s.by_rank[r]] = -1;
                     }
                     QT_SYNC();
                 }

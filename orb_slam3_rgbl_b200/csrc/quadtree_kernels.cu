@@ -2,7 +2,6 @@
 // per-frame SelKp list the describe kernel consumes.  Algorithm: quadtree_block.cuh.
 #include <algorithm>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <vector>
 
@@ -19,7 +18,7 @@ __global__ void __launch_bounds__(512, MAXN <= 512 ? 2 : 1) quadtree_kernel(cons
                                                        const int* __restrict__ frame_total, const LevelGeom* __restrict__ levels,
                                                        int n_levels, QtScratchDev scr, uint32_t* __restrict__ sel_lvl,
                                                        int* __restrict__ n_sel_lvl, const int* __restrict__ lvl_region,
-                                                       int cap_kp, int* __restrict__ status, int dyn_bytes, int block_sort) {
+                                                       int cap_kp, int* __restrict__ status, int dyn_bytes) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     typedef qt::SharedT<MAXN> SharedX;
     SharedX& s = *reinterpret_cast<SharedX*>(smem_raw);
@@ -55,7 +54,7 @@ __global__ void __launch_bounds__(512, MAXN <= 512 ? 2 : 1) quadtree_kernel(cons
 #ifdef QT_TIMING
     const long long qt_t0 = clock64();
 #endif
-    const int m = qt::distribute(s, dense + off, n, lg.max_bx - lg.min_bx, lg.max_by - lg.min_by, lg.quota, g, out, region_cap, block_sort);
+    const int m = qt::distribute(s, dense + off, n, lg.max_bx - lg.min_bx, lg.max_by - lg.min_by, lg.quota, g, out, region_cap);
 #ifdef QT_TIMING
     if (threadIdx.x == 0 && f == 0) printf("quadtree level %d: n=%d quota=%d selected=%d keys_on_chip=%d cycles=%lld\n", l, n, lg.quota, m, (int)(sizeof(SharedX) + key_bytes <= (size_t)dyn_bytes), clock64() - qt_t0);
 #endif
@@ -107,34 +106,30 @@ int launch_quadtree(cudaStream_t st, const uint32_t* dense, const int* level_cnt
                     int n_levels, const QtScratchDev& scr, uint32_t* sel_lvl, int* n_sel_lvl, const int* lvl_region, int cap_kp,
                     int* status, SelKp* sel, int* n_sel, int n_frames, int max_nodes) {
     // max_nodes = the largest node list any level of the context needs (max(quota + 3, 4 nIni)): <= 512 selects the half-size tree state
-    // with two CTAs per SM (RGBL_QT_TWO_PER_SM=0: one per SM with all the shared memory, as in round 1)
-    static const int two_per_sm = [] { const char* e = getenv("RGBL_QT_TWO_PER_SM"); return (e && e[0] == '0') ? 0 : 1; }();
+    // with two CTAs per SM
     static int dyn512 = 0, dyn1024 = 0;
     const bool small = max_nodes <= 512;
     int& dyn_bytes = small ? dyn512 : dyn1024;
-    if (!dyn_bytes) dyn_bytes = small ? quadtree_dyn_bytes<512>(two_per_sm ? 2 : 1) : quadtree_dyn_bytes<1024>(1);
+    if (!dyn_bytes) dyn_bytes = small ? quadtree_dyn_bytes<512>(2) : quadtree_dyn_bytes<1024>(1);
     if (dyn_bytes <= 0) return -1;
-    // block-parallel std::sort of the budgeted expansion: the default;
-    // RGBL_QT_BLOCK_SORT=0 selects the one-thread sort
-    static const int block_sort = [] { const char* e = getenv("RGBL_QT_BLOCK_SORT"); return (e && e[0] == '0') ? 0 : 1; }();
     if (small)
         quadtree_kernel<512><<<dim3(n_frames, n_levels), 512, dyn_bytes, st>>>(dense, level_cnt, frame_total, d_levels, n_levels, scr, sel_lvl, n_sel_lvl,
-                                                                             lvl_region, cap_kp, status, dyn_bytes, block_sort);
+                                                                             lvl_region, cap_kp, status, dyn_bytes);
     else
         quadtree_kernel<1024><<<dim3(n_frames, n_levels), 512, dyn_bytes, st>>>(dense, level_cnt, frame_total, d_levels, n_levels, scr, sel_lvl, n_sel_lvl,
-                                                                              lvl_region, cap_kp, status, dyn_bytes, block_sort);
+                                                                              lvl_region, cap_kp, status, dyn_bytes);
     sel_pack_kernel<<<n_frames, 256, 0, st>>>(sel_lvl, n_sel_lvl, lvl_region, n_levels, cap_kp, sel, n_sel);
     return 0;
 }
 
 // Host execution of the SAME block algorithm (phase-sequential): CPU validation of the device logic.
-int quadtree_block_host(const uint32_t* cand, int n, int width, int height, int N, uint32_t* out, int out_cap, int block_sort) {
+int quadtree_block_host(const uint32_t* cand, int n, int width, int height, int N, uint32_t* out, int out_cap) {
     std::vector<qt::KeyIdx> pa(n + 1), pb(n + 1), na(n + 1), nb(n + 1);
     std::vector<unsigned long long> scan(n + 2);
     std::vector<unsigned char> quad(n + 1);
     qt::Scratch g{pa.data(), pb.data(), na.data(), nb.data(), scan.data(), quad.data()};
     qt::Shared* s = new qt::Shared();
-    const int m = qt::distribute(*s, cand, n, width, height, N, g, out, out_cap, block_sort);
+    const int m = qt::distribute(*s, cand, n, width, height, N, g, out, out_cap);
     delete s;
     return m;
 }
@@ -144,15 +139,14 @@ int quadtree_block_host(const uint32_t* cand, int n, int width, int height, int 
 #ifdef RGBL_TESTING_EXPORTS        // test hooks: only in librgbl_b200_testing.so (csrc/rgbl_testing.h)
 extern "C" {
 
-// test hook: the block algorithm run on the host; xys n x 3 (x, y, score) like rgbl_quadtree_select
+// test hook: the block algorithm run on the host; xys n x 3 (x, y, score) like rgbl_quadtree_select.  The budget is |n_desired|: the
+// sign once chose between two sort formulations with the same survivors, and callers that still pass it get the one that remains.
 int rgbl_quadtree_select_block_emulation(const int32_t* xys, int n, int min_x, int max_x, int min_y, int max_y, int n_desired,
                                          int32_t* out_xys, int cap) {
     if (n < 0 || (n > 0 && !xys) || !out_xys) return RGBL_E_INVALID;
     std::vector<uint32_t> c(n), o(cap);
     for (int i = 0; i < n; ++i) c[i] = rgbl::pack_cand(xys[3 * i], xys[3 * i + 1], xys[3 * i + 2]);
-    // n_desired < 0: run the block-parallel std::sort variant with |n_desired|
-    const int m = rgbl::quadtree_block_host(c.data(), n, max_x - min_x, max_y - min_y, n_desired < 0 ? -n_desired : n_desired, o.data(), cap,
-                                            n_desired < 0 ? 1 : 0);
+    const int m = rgbl::quadtree_block_host(c.data(), n, max_x - min_x, max_y - min_y, n_desired < 0 ? -n_desired : n_desired, o.data(), cap);
     if (m < 0) return RGBL_E_UNSUPPORTED;
     if (m > cap) return RGBL_E_CAPACITY;
     for (int i = 0; i < m; ++i) { out_xys[3 * i] = (int)(o[i] & 0xfff); out_xys[3 * i + 1] = (int)((o[i] >> 12) & 0xfff); out_xys[3 * i + 2] = (int)(o[i] >> 24); }

@@ -128,10 +128,9 @@ struct Ctx {
 
     // device quad-tree (quadtree_kernels.cu)
     bool device_quadtree = false, host_counts_valid = false;
-    // strip formulation of the FAST kernel (fast_strip.cuh); selected with RGBL_FAST_STRIPS=1
     LevelTensorMaps level_tms{};                 // level_tma_kernels.cu; level_tma: the fused TMA tile kernel replaces launch_pyramid + launch_blur (RGBL_LEVEL_TMA=0: off)
     bool level_tma = false;
-    bool fast_strips = false, describe_staged = false, dilate_v2 = false;   // RGBL_DESCRIBE_STAGED=1: describe_warp_kernels.cu
+    // cell strips of the FAST kernel (fast_strip.cuh)
     std::vector<StripInfo> strips;
     DeviceArray<StripInfo> d_strips;
     int strip_rows_cap = 0, strip_list_cap = 0;

@@ -18,7 +18,6 @@ constexpr int kFastBorder = 16;      // EDGE_THRESHOLD - 3, src/ORBextractor.cc:
 constexpr int kCellTarget = 35;      // W, src/ORBextractor.cc:785
 constexpr int kCellCap = 256;        // staged FAST survivors per cell (overflow is reported, never dropped)
 constexpr int kGridCols = 64, kGridRows = 48;   // FRAME_GRID_COLS / FRAME_GRID_ROWS, include/Frame.h:46-47
-constexpr int kFastTilePitch = 88;   // shared-memory window pitch: <= 3 alignment bytes + <= 78-byte window rows
 
 // Geometry of one pyramid level (identical for every frame of a context).
 struct LevelGeom {

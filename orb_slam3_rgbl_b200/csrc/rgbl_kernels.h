@@ -17,19 +17,11 @@ struct __align__(8) SelKp {
     uint16_t pad;
 };
 
-#if defined(__CUDACC__)
-__device__ __forceinline__ uint32_t pack_cand_dev(int x, int y, int s) {
-    return (uint32_t)x | ((uint32_t)y << 12) | ((uint32_t)s << 24);
-}
-#endif
-
 // orb_kernels.cu
 void launch_pyramid(cudaStream_t st, uint8_t* pyr, size_t frame_stride, const LevelGeom* h_levels, int n_levels,
                     const LinCoef* d_coefs, int n_frames);
-void launch_fast(cudaStream_t st, const uint8_t* pyr, size_t frame_stride, const LevelGeom* d_levels,
-                 const CellInfo* d_cells, int n_cells, int ini_th, int min_th, uint32_t* slots, int* counts,
-                 int* overflow, int n_frames);
-// fast_strip_kernels.cu: strip formulation of launch_fast (same outputs); returns -1 when the shared-memory request is refused
+// fast_strip_kernels.cu: per-cell FAST with the iniTh -> minTh fallback, one CTA per strip of cells (fast_strip.cuh); survivors in
+// each cell's slot array; returns -1 when the shared-memory request is refused
 int launch_fast_strips(cudaStream_t st, const uint8_t* pyr, size_t frame_stride, const LevelGeom* d_levels, const CellInfo* d_cells,
                        int n_cells, const StripInfo* d_strips, int n_strips, int rows_cap, int list_cap, int ini_th, int min_th,
                        uint32_t* slots, int* counts, int* overflow, int n_frames);
@@ -52,10 +44,8 @@ int launch_level_tiles(cudaStream_t st, const LevelTensorMaps& tms, uint8_t* pyr
                        int n_levels, const LinCoef* d_coefs, int n_frames);
 void launch_blur(cudaStream_t st, const uint8_t* pyr, uint8_t* blur, size_t frame_stride, const LevelGeom* h_levels,
                  int n_levels, int n_frames);
-void launch_describe(cudaStream_t st, const uint8_t* pyr, const uint8_t* blur, size_t frame_stride,
-                     const LevelGeom* d_levels, const SelKp* sel, const int* n_sel, int cap, int max_n,
-                     const int umax[16], rgbl_keypoint* kps, uint8_t* desc, int n_frames);
-// describe_warp_kernels.cu: launch_describe with the pixel neighbourhoods staged in shared memory (same outputs)
+// describe_warp_kernels.cu: orientation + rBRIEF descriptor + keypoint record, one warp per selected keypoint with its pixel
+// neighbourhoods staged in shared memory (describe_warp.cuh)
 void launch_describe_staged(cudaStream_t st, const uint8_t* pyr, const uint8_t* blur, size_t frame_stride, const LevelGeom* d_levels,
                             const SelKp* sel, const int* n_sel, int cap, int max_n, const int umax[16], rgbl_keypoint* kps, uint8_t* desc,
                             int n_frames);
@@ -68,7 +58,7 @@ int quadtree_smem_bytes();
 int launch_quadtree(cudaStream_t st, const uint32_t* dense, const int* level_cnt, const int* frame_total, const LevelGeom* d_levels,
                     int n_levels, const QtScratchDev& scr, uint32_t* sel_lvl, int* n_sel_lvl, const int* lvl_region, int cap_kp,
                     int* status, SelKp* sel, int* n_sel, int n_frames, int max_nodes = 1024);      // max_nodes: largest max(quota + 3, 4 nIni) over the levels
-int quadtree_block_host(const uint32_t* cand, int n, int width, int height, int N, uint32_t* out, int out_cap, int block_sort = 0);
+int quadtree_block_host(const uint32_t* cand, int n, int width, int height, int N, uint32_t* out, int out_cap);
 
 // depth_kernels.cu
 struct DepthDev {
@@ -83,10 +73,8 @@ struct DepthDev {
 void launch_deinterleave_xyzr(cudaStream_t st, const float* raw, float* pts, int pts_stride, const int* n_pts, int max_n_pts, int n_frames);
 void launch_depth_project(cudaStream_t st, const float* pts, int pts_stride, const int* n_pts, int max_n_pts,
                           const DepthDev& prm, int W, int H, uint32_t* idx_map, uint32_t stamp, int n_frames);
-void launch_depth_resolve_dilate(cudaStream_t st, const float* pts, int pts_stride, const int* n_pts,
-                                 const DepthDev& prm, int W, int H, const uint32_t* idx_map, uint32_t stamp,
-                                 float* raw, float* processed, int n_frames);
-// depth_dilate_v2.cu: same outputs; empty tiles skip the structuring-element loop, taps as shared-memory offsets
+// depth_dilate_v2.cu: depth of each pixel's winning point (raw, nullable) and its inverse dilation by the structuring element of prm
+// (processed); empty tiles skip the structuring-element loop, taps as shared-memory offsets
 void launch_depth_resolve_dilate_v2(cudaStream_t st, const float* pts, int pts_stride, const int* n_pts, const DepthDev& prm, int W, int H,
                                     const uint32_t* idx_map, uint32_t stamp, float* raw, float* processed, int n_frames);
 void launch_depth_average_filter(cudaStream_t st, const float* raw, int W, int H, int k, float* processed, int n_frames);

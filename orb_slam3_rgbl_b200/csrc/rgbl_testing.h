@@ -15,14 +15,13 @@ extern "C" {
 int rgbl_quadtree_select(const int32_t* xys, int n, int min_x, int max_x, int min_y, int max_y, int n_desired,
                          int32_t* out_idx, int cap);
 
-/* Test hooks (host-only): the device quad-tree's block algorithm executed phase-sequentially on the host, and the
- * restated libstdc++ std::sort it uses.  out_xys: n x 3 survivors in the reference's output order.              */
+/* Test hooks (host-only): the device quad-tree's block algorithm executed phase-sequentially on the host (budget |n_desired|), and
+ * the restated libstdc++ std::sort it falls back to.  out_xys: n x 3 survivors in the reference's output order.              */
 int rgbl_quadtree_select_block_emulation(const int32_t* xys, int n, int min_x, int max_x, int min_y, int max_y, int n_desired,
                                          int32_t* out_xys, int cap);
 int rgbl_std_sort_emulation(const int32_t* size_ulx, int n, int32_t* perm_out);
 /* The block-parallel formulation of that sort (mode 0; mode > 0: depth limit mode - 1, which forces the heapsort fallback) or,
- * as ground truth, the C++ library's own std::sort with the reference's comparator (mode < 0).  n <= 1024.
- * rgbl_quadtree_select_block_emulation runs its budgeted expansion with the block-parallel sort when n_desired < 0.       */
+ * as ground truth, the C++ library's own std::sort with the reference's comparator (mode < 0).  n <= 1024.                */
 int rgbl_std_sort_block_emulation(const int32_t* size_ulx, int n, int mode, int32_t* perm_out);
 
 /* Test hook (host-only): the strip formulation of the per-cell FAST detection (fast_strip.cuh; src/ORBextractor.cc:805-868)

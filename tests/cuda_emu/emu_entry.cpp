@@ -65,7 +65,7 @@ int emu_describe_staged(const rgbl_orb_params* orb, const uint8_t* level_img, co
 }
 
 // xys: n x 3 candidates (x, y relative to the FAST window origin, score) in the reference's order; out_xys: survivors in level
-// coordinates (+16) in the reference's output order.  The block-parallel sort is selected by RGBL_QT_BLOCK_SORT (read once).
+// coordinates (+16) in the reference's output order.
 int emu_quadtree(const int32_t* xys, int n, int w, int h, int n_desired, int32_t* out_xys, int cap) {
     LevelGeom lg{};
     lg.w = w; lg.h = h; lg.min_bx = kFastBorder; lg.min_by = kFastBorder; lg.max_bx = w - kFastBorder; lg.max_by = h - kFastBorder;
@@ -87,10 +87,9 @@ int emu_quadtree(const int32_t* xys, int n, int w, int h, int n_desired, int32_t
 }
 
 // ORBextractor::operator() for one image through the device pipeline of api.cu's run_extract (device quad-tree mode):
-// pyramid -> FAST (per cell, or strips) -> compaction -> blur -> quad-tree -> describe (gathering, or staged).
-// variants: bit 0 = strip FAST, bit 1 = staged describe (the block-parallel quad-tree sort follows RGBL_QT_BLOCK_SORT).
-int emu_extract(const rgbl_orb_params* orb, const uint8_t* img, int width, int height, int stride, int variants, rgbl_keypoint* kps_out,
-                uint8_t* desc_out, int cap) {
+// pyramid -> FAST -> compaction -> blur -> quad-tree -> describe.
+int emu_extract(const rgbl_orb_params* orb, const uint8_t* img, int width, int height, int stride, rgbl_keypoint* kps_out, uint8_t* desc_out,
+                int cap) {
     OrbTables tab;
     int rc = compute_orb_tables(*orb, tab);
     if (rc) return rc;
@@ -105,15 +104,10 @@ int emu_extract(const rgbl_orb_params* orb, const uint8_t* img, int width, int h
     std::vector<uint32_t> slots((size_t)n_cells * kCellCap);
     std::vector<int> counts(n_cells, 0), cell_off(n_cells + 1, 0);
     int level_cnt[RGBL_MAX_LEVELS] = {0}, frame_total = 0, overflow[4] = {0, 0, 0, 0};
-    if (variants & 1) {
-        std::vector<StripInfo> strips; int rows_cap = 0, list_cap = 0;
-        build_fast_strips(cells, 8, 264, strips, rows_cap, list_cap);
-        if (launch_fast_strips(nullptr, pyr.data(), fb, levels.data(), cells.data(), n_cells, strips.data(), (int)strips.size(), rows_cap, list_cap,
-                               orb->ini_th_fast, orb->min_th_fast, slots.data(), counts.data(), overflow, 1) != 0) return -100;
-    } else {
-        launch_fast(nullptr, pyr.data(), fb, levels.data(), cells.data(), n_cells, orb->ini_th_fast, orb->min_th_fast, slots.data(), counts.data(),
-                    overflow, 1);
-    }
+    std::vector<StripInfo> strips; int rows_cap = 0, list_cap = 0;
+    build_fast_strips(cells, 8, 264, strips, rows_cap, list_cap);
+    if (launch_fast_strips(nullptr, pyr.data(), fb, levels.data(), cells.data(), n_cells, strips.data(), (int)strips.size(), rows_cap, list_cap,
+                           orb->ini_th_fast, orb->min_th_fast, slots.data(), counts.data(), overflow, 1) != 0) return -100;
     const int dense_cap = std::max(32768, width * height / 8);
     std::vector<uint32_t> dense(dense_cap + 8);
     launch_compact(nullptr, levels.data(), nl, n_cells, slots.data(), counts.data(), cell_off.data(), level_cnt, &frame_total, dense.data(), dense_cap,
@@ -139,15 +133,14 @@ int emu_extract(const rgbl_orb_params* orb, const uint8_t* img, int width, int h
                         &status, sel.data(), &n_sel, 1) != 0) return -100;
     if (status) return RGBL_E_CAPACITY;
     if (n_sel > cap) return RGBL_E_CAPACITY;
-    ((variants & 2) ? launch_describe_staged : launch_describe)(nullptr, pyr.data(), blur.data(), fb, levels.data(), sel.data(), &n_sel, cap_kp, n_sel,
-                                                               tab.umax, kps_out, desc_out, 1);
+    launch_describe_staged(nullptr, pyr.data(), blur.data(), fb, levels.data(), sel.data(), &n_sel, cap_kp, n_sel, tab.umax, kps_out, desc_out, 1);
     return n_sel;
 }
 
-// ProjectPointcloudToImage + Upsample_InverseDilation: depth_project_kernel, then depth_resolve_dilate_kernel (v2 == 0) or
-// depth_resolve_dilate_v2_kernel.  pts: 4 x n planar (x | y | z | 1), mask ku x kv, outputs W x H floats.
+// ProjectPointcloudToImage + Upsample_InverseDilation: depth_project_kernel, then depth_resolve_dilate_v2_kernel.
+// pts: 4 x n planar (x | y | z | 1), mask ku x kv, outputs W x H floats.
 int emu_depth_dilate(const float* pts, int n, const float P[12], int W, int H, const uint8_t* mask, int ku, int kv, float min_d, float max_d,
-                     float inv_scale, int v2, float* raw_out, float* processed_out) {
+                     float inv_scale, float* raw_out, float* processed_out) {
     DepthDev dd{};
     std::memcpy(dd.P, P, 12 * sizeof(float));
     dd.min_dist = min_d; dd.max_dist = max_d; dd.bf = 0; dd.inv_scale_m = max_d * inv_scale; dd.ku = ku; dd.kv = kv;
@@ -155,7 +148,7 @@ int emu_depth_dilate(const float* pts, int n, const float P[12], int W, int H, c
     dd.method = RGBL_DEPTH_INVERSE_DILATION;
     std::vector<uint32_t> idx((size_t)W * H, 0u);
     launch_depth_project(nullptr, pts, 4 * n, &n, n, dd, W, H, idx.data(), 1u, 1);
-    (v2 ? launch_depth_resolve_dilate_v2 : launch_depth_resolve_dilate)(nullptr, pts, 4 * n, &n, dd, W, H, idx.data(), 1u, raw_out, processed_out, 1);
+    launch_depth_resolve_dilate_v2(nullptr, pts, 4 * n, &n, dd, W, H, idx.data(), 1u, raw_out, processed_out, 1);
     return 0;
 }
 

@@ -4,7 +4,6 @@ The host twins (tests/test_host_abi.py) check the algorithms; this checks the de
 shared-memory atomics, warp reductions, dynamic shared-memory carving and the launch geometry."""
 import ctypes as C
 import importlib.util
-import os
 from pathlib import Path
 
 import numpy as np
@@ -19,7 +18,6 @@ HERE = Path(__file__).resolve().parent
 
 @pytest.fixture(scope="module")
 def emu():
-    os.environ["RGBL_QT_BLOCK_SORT"] = "1"          # read once by the emulated launch_quadtree
     spec = importlib.util.spec_from_file_location("cuda_emu_build", HERE / "cuda_emu" / "build.py")
     mod = importlib.util.module_from_spec(spec); spec.loader.exec_module(mod)
     lib = C.CDLL(str(mod.build()))
@@ -80,7 +78,7 @@ def test_staged_describe_kernel_device_path(emu):
 def test_quadtree_kernel_with_block_sort_device_path(emu):
     img = S.make_image(79, 700, 260)
     ex = oracle.Extractor(1000); ex(img)
-    for l in (0, 4):
+    for l in (0, 4, 5):
         cand = np.ascontiguousarray(ex.level_candidates(l), np.int32)
         hh, ww = ex.level_image(l).shape
         nd = int(ex.features_per_level[l])
@@ -91,44 +89,15 @@ def test_quadtree_kernel_with_block_sort_device_path(emu):
         assert (out[:m, 0] == ref["x"]).all() and (out[:m, 1] == ref["y"]).all() and (out[:m, 2] == ref["response"]).all()
 
 
-def test_default_quadtree_kernel_device_path_in_a_fresh_process(emu):
-    """The shipped configuration (one-thread std::sort; RGBL_QT_BLOCK_SORT unset, which launch_quadtree reads once per process):
-    same emulated kernel, default mode.  Guards the default path against the edits made for the block mode."""
-    import subprocess, sys
-    code = r'''
-import ctypes as C, sys, numpy as np
-sys.path.insert(0, %r); sys.path.insert(0, %r)
-import oracle
-from orb_slam3_rgbl_b200 import _lib as L, synthetic as S
-lib = C.CDLL(%r)
-lib.emu_quadtree.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int]
-img = S.make_image(79, 700, 260)
-ex = oracle.Extractor(1000); ex(img)
-for l in (0, 5):
-    cand = np.ascontiguousarray(ex.level_candidates(l), np.int32)
-    hh, ww = ex.level_image(l).shape
-    nd = int(ex.features_per_level[l])
-    out = np.empty((nd + 64, 3), np.int32)
-    m = lib.emu_quadtree(L.ptr(cand), len(cand), ww, hh, nd, L.ptr(out), len(out))
-    ref = ex.level_keypoints(l)
-    assert m == len(ref) and (out[:m, 0] == ref["x"]).all() and (out[:m, 1] == ref["y"]).all() and (out[:m, 2] == ref["response"]).all()
-print("default-ok")
-''' % (str(HERE.parent), str(HERE), str(HERE / "cuda_emu" / "build" / "libcuda_emu.so"))
-    env = {k: v for k, v in os.environ.items() if k != "RGBL_QT_BLOCK_SORT"}
-    r = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "default-ok" in r.stdout, r.stderr[-2000:]
-
-
-@pytest.mark.parametrize("v2", [0, 1])
-def test_depth_dilate_kernels_device_path(emu, v2):
-    """depth_project + depth_resolve_dilate (shipped, v2 = 0) and the variant with the empty-tile shortcut and shared-memory tap
-    offsets (v2 = 1) against the oracle's ProjectPointcloudToImage + Upsample_InverseDilation, bit for bit; the cloud covers
-    only the lower part of the image so that whole tiles are empty."""
+def test_depth_dilate_kernels_device_path(emu):
+    """depth_project + depth_resolve_dilate_v2 (empty-tile shortcut, shared-memory tap offsets, the 5x5 diamond compiled in) against
+    the oracle's ProjectPointcloudToImage + Upsample_InverseDilation, bit for bit; the cloud covers only the lower part of the image
+    so that whole tiles are empty."""
     W, H = 333, 150
     P = S.lidar_projection_matrix().astype(np.float32)
     pts = S.make_pointcloud(3, n_azimuth=500)
     emu.emu_depth_dilate.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float,
-                                     C.c_float, C.c_int, C.c_void_p, C.c_void_p]
+                                     C.c_float, C.c_void_p, C.c_void_p]
     # shift the projection so that the returns land inside this small image
     P2 = P.copy(); P2[0, :] *= W / S.KITTI_W; P2[1, :] *= H / S.KITTI_H
     for kind, k in (("diamond", 5), ("rectangle", 3), ("cross", 7)):
@@ -139,24 +108,22 @@ def test_depth_dilate_kernels_device_path(emu, v2):
         raw = np.empty((H, W), np.float32); out = np.empty((H, W), np.float32)
         m = np.ascontiguousarray(mask, np.uint8)
         emu.emu_depth_dilate(L.ptr(p), p.shape[1], L.ptr(np.ascontiguousarray(P2.reshape(12))), W, H, L.ptr(m), m.shape[1], m.shape[0], 5.0, 200.0, 1.0,
-                             v2, L.ptr(raw), L.ptr(out))
+                             L.ptr(raw), L.ptr(out))
         assert (raw.view(np.uint32) == raw_ref.view(np.uint32)).all()
         assert (out.view(np.uint32) == ref.view(np.uint32)).all(), kind
         assert (raw_ref > 0).sum() > 200 and (raw_ref[: H // 4] > 0).sum() == 0
 
 
-@pytest.mark.parametrize("variants", [0, 3])
-def test_whole_extraction_pipeline_device_path(emu, variants):
-    """pyramid -> FAST -> compaction -> blur -> quad-tree -> describe through the real launchers on the emulator, shipped kernels
-    (variants = 0) and strip FAST + staged describe (variants = 3; the quad-tree runs its block-parallel sort in this process):
-    keypoints and descriptors equal the oracle's ORBextractor::operator() bit for bit."""
+def test_whole_extraction_pipeline_device_path(emu):
+    """pyramid -> FAST -> compaction -> blur -> quad-tree -> describe through the real launchers on the emulator: keypoints and
+    descriptors equal the oracle's ORBextractor::operator() bit for bit."""
     w, h = 260, 200
     img = S.make_image(81, w, h)
     prm = L.OrbParams(400, 1.2, 4, 12, 7)
     ok, od, _ = oracle.Extractor(400, 1.2, 4, 12, 7)(img)
-    emu.emu_extract.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
+    emu.emu_extract.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
     kps = np.empty(1024, oracle.KP_DTYPE); desc = np.empty((1024, 32), np.uint8)
-    n = emu.emu_extract(C.byref(prm), L.ptr(img), w, h, img.strides[0], variants, L.ptr(kps), L.ptr(desc), len(kps))
+    n = emu.emu_extract(C.byref(prm), L.ptr(img), w, h, img.strides[0], L.ptr(kps), L.ptr(desc), len(kps))
     assert n == len(ok) > 150
     for f in ok.dtype.names:
         assert (kps[:n][f].view(np.uint32) == ok[f].view(np.uint32)).all(), f

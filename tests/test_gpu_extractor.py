@@ -191,27 +191,23 @@ def test_fused_tma_level_kernel_equals_oracle_and_two_pass_kernels(W, H, scale, 
             assert (a == b).all() and (ab == bb).all()
 
 
-def test_first_formulation_kernels_behind_their_switches(monkeypatch):
-    """The kernels that were the defaults in round 1 stay in the library as exact twins behind RGBL_FAST_STRIPS=0 (per-cell FAST),
-    RGBL_DESCRIBE_STAGED=0 (gathering describe), RGBL_DILATE_V2=0 (first dilation kernel), RGBL_LEVEL_TMA=0 (two-pass pyramid + blur) and
-    RGBL_HOST_QUADTREE=1 (host quad-tree): one RGB-L frame construction with all of them selected equals the oracle bit for bit, like the
-    default kernels do."""
+def test_two_pass_levels_and_host_quadtree_frames_equal_the_oracle(monkeypatch):
+    """The paths besides the defaults that a context can take: the two-pass pyramid + blur (RGBL_LEVEL_TMA=0, also the path of level
+    ratios the fused tile kernel cannot hold) and the host quad-tree (rgbl_set_host_quadtree, also the path of level geometries the device
+    quad-tree cannot hold).  One RGB-L frame construction with each equals the oracle bit for bit, like the default kernels do."""
     W, H = S.KITTI_W, S.KITTI_H
     img = S.make_image(77, W, H)
     pts = S.make_pointcloud(77)
     P = S.lidar_projection_matrix()
     rk, rd, _ = oracle.Extractor(2000)(img)
     rdep, rur, _, _ = oracle.depth_from_pcd(pts, P, W, H, S.structuring_element("diamond", 5), S.KITTI_BF, rk, rk)
-    for env in ({"RGBL_FAST_STRIPS": "0", "RGBL_DESCRIBE_STAGED": "0", "RGBL_DILATE_V2": "0", "RGBL_LEVEL_TMA": "0"},
-                {"RGBL_HOST_QUADTREE": "1"}):
-        for k_ in ("RGBL_FAST_STRIPS", "RGBL_DESCRIBE_STAGED", "RGBL_DILATE_V2", "RGBL_LEVEL_TMA", "RGBL_HOST_QUADTREE"):
-            monkeypatch.delenv(k_, raising=False)
-        for k_, v_ in env.items():
-            monkeypatch.setenv(k_, v_)
-        ctx = F.Context(W, H, 2000, max_batch=1, max_points=pts.shape[1])          # the switches are read by rgbl_create
+    for level_tma, host_quadtree in (("0", False), ("1", True)):
+        monkeypatch.setenv("RGBL_LEVEL_TMA", level_tma)                # read by rgbl_create
+        ctx = F.Context(W, H, 2000, max_batch=1, max_points=pts.shape[1])
         try:
+            ctx.set_host_quadtree(host_quadtree)
             (k, d, dep, ur), = F.frame_rgbl_batch(ctx, [img], [pts], P, F.make_depth_params(bf=S.KITTI_BF))
         finally:
             ctx.close()
         _cmp_kps(k, rk)
-        assert (d == rd).all() and (dep == rdep).all() and (ur == rur).all(), env
+        assert (d == rd).all() and (dep == rdep).all() and (ur == rur).all(), (level_tma, host_quadtree)

@@ -1,8 +1,6 @@
 """rgbl_frame_rgbl_batch (extraction + LiDAR depth of a 2-frame batch) through the real C ABI of the EMULATED library
-(tests/cuda_emu, `build.py full`), compared bit for bit with the oracle.  Run it once with the default kernels and once with every
-prepared variant selected by its environment variable (this is what exercises the selection code of api.cu without a GPU):
+(tests/cuda_emu, `build.py full`), compared bit for bit with the oracle, without a GPU:
     python tests/tools/emu_abi_variants.py
-    RGBL_FAST_STRIPS=1 RGBL_DESCRIBE_STAGED=1 RGBL_QT_BLOCK_SORT=1 RGBL_DILATE_V2=1 python tests/tools/emu_abi_variants.py
 """
 import sys, os
 ROOT = __import__('pathlib').Path(__file__).resolve().parent.parent.parent
