@@ -386,6 +386,37 @@ def pose_optimize(pose, xw, obs, inv_sigma2, stereo, fx, fy, cx, cy, bf):
     return r, out, outlier
 
 
+class PoseTraceC(C.Structure):
+    """PoseTrace (oracle/pose_oracle.cpp)."""
+    _fields_ = [("rounds", C.c_int), ("iters", C.c_int * 4), ("rejected", C.c_int), ("max_reject_run", C.c_int),
+                ("term_qmax", C.c_int), ("term_rho0", C.c_int), ("term_nbad", C.c_int), ("term_iters", C.c_int),
+                ("any_sincos", C.c_int), ("empty_rounds", C.c_int), ("max_accepted_trial", C.c_int),
+                ("min_rho_margin", C.c_double), ("min_stop_margin", C.c_double), ("min_chi2_margin", C.c_double)]
+
+
+def pose_optimize_trace(pose, xw, obs, inv_sigma2, stereo, fx, fy, cx, cy, bf):
+    """pose_optimize with the same outputs plus a dict of what the call did: rounds and LM iterations per round, rejected trials and the
+    longest run of them in one iteration, how often each termination ended a round (term_qmax / term_rho0 / term_nbad / term_iters),
+    whether a step had theta^2 >= 0.25 (any_sincos), rounds that began with no active edge, the highest trial index of an iteration that
+    was accepted (max_accepted_trial: the damping of trial w is lambda nu^w 2^(w(w-1)/2)), and the smallest relative margins of the
+    accept / reject test, the stop test and the chi2 classification (inf when no such decision depended on rounding).
+    -> (n_inliers, pose_out[7], outlier[n], trace)"""
+    _late(lib())
+    L = lib()
+    if L.orc_pose_optimize_trace.argtypes is None:
+        L.orc_pose_optimize_trace.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 4 + [C.c_float] * 5 + [C.c_void_p, C.c_void_p, C.POINTER(PoseTraceC)]
+        L.orc_pose_optimize_trace.restype = C.c_int
+    pose = np.ascontiguousarray(pose, np.float32); xw = np.ascontiguousarray(xw, np.float32).reshape(-1, 3)
+    obs = np.ascontiguousarray(obs, np.float32).reshape(-1, 3); inv_sigma2 = np.ascontiguousarray(inv_sigma2, np.float32)
+    stereo = np.ascontiguousarray(stereo, np.uint8)
+    n = len(xw)
+    out = np.empty(7, np.float32); outlier = np.zeros(n, np.uint8); tr = PoseTraceC()
+    r = L.orc_pose_optimize_trace(_p(pose), n, _p(xw), _p(obs), _p(inv_sigma2), _p(stereo), fx, fy, cx, cy, bf, _p(out), _p(outlier), C.byref(tr))
+    trace = {name: (list(getattr(tr, name)) if name == "iters" else getattr(tr, name)) for name, _ in PoseTraceC._fields_}
+    trace["iters"] = trace["iters"][:tr.rounds]
+    return r, out, outlier, trace
+
+
 def _csr(node_ids, node_start, node_feat):
     return (np.ascontiguousarray(node_ids, np.uint32), np.ascontiguousarray(node_start, np.int32), np.ascontiguousarray(node_feat, np.int32))
 

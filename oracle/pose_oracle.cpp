@@ -93,6 +93,8 @@ inline void edge_jacobian(const Edge& e, const SE3& T, const Cam& c, double J[3]
 }
 
 // Dense LDL^T solve of the 6x6 system (Eigen::LDLT with its diagonal pivoting), isPositive() check.
+// A NaN pivot (an edge on the camera plane makes H NaN) is neither positive nor negative for Eigen's sign tracking: isPositive() stays
+// true and the step comes out NaN (Eigen zeroes that row of D^-1, the triangular solves with NaN in L still spread it).
 bool solve6(const double Hin[6][6], const double bin[6], double x[6]) {
     double A[6][6]; int perm[6];
     for (int i = 0; i < 6; ++i) { perm[i] = i; for (int j = 0; j < 6; ++j) A[i][j] = Hin[i][j]; }
@@ -128,12 +130,30 @@ void study_build_system(LM& lm, double H[6][6], double b[6]);
 bool study_solve6(const double H[6][6], const double b[6], double x[6]);
 #endif
 
+// What one call did (orc_pose_optimize_trace): the paths it took and how close each discrete decision came to going the other way.
+// Margins: |rho| for the accept / reject test (rho is already a ratio), |(ini - cur) * 1e3 - ini| / |ini| for the stop test and
+// |chi2 - threshold| / threshold for the outlier classification.  Decisions that do not depend on rounding (no active edge, a failed
+// solve, a non-finite value) are not counted.
+struct PoseTrace {
+    int rounds, iters[4];                                   // rounds run, LM iterations of each round
+    int rejected, max_reject_run;                           // rejected trials in all; most consecutive rejections in one iteration
+    int term_qmax, term_rho0, term_nbad, term_iters;        // how each round's optimize() ended: qmax == 10, rho == 0, n_bad >= 3, 10 iterations
+    int any_sincos, empty_rounds;                           // a trial step with theta^2 >= 0.25; rounds that began with no active edge
+    int max_accepted_trial;                                 // highest trial index (0-based, within an iteration) that was accepted
+    double min_rho_margin, min_stop_margin, min_chi2_margin;
+};
+
+inline void margin(double& m, double dist, double scale) {
+    if (std::isfinite(dist) && std::isfinite(scale) && scale != 0) m = std::min(m, std::fabs(dist) / std::fabs(scale));
+}
+
 struct LM {
     std::vector<Edge>& edges;
     const Cam& cam;
     double delta_mono, delta_stereo; float dsqr_mono, dsqr_stereo;
     SE3 est;
     double lambda = -1, ni = 2; int n_bad = 0;
+    PoseTrace* tr = nullptr;
 
     void compute_active_errors() { for (Edge& e : edges) if (e.level == 0) edge_error(e, est, cam); }
     double active_robust_chi2() const {
@@ -182,7 +202,7 @@ struct LM {
             for (int j = 0; j < 6; ++j) mx = std::max(std::fabs(H[j][j]), mx);
             lambda = 1e-5 * mx; ni = 2; n_bad = 0;
         }
-        double rho = 0; int qmax = 0;
+        double rho = 0; int qmax = 0, run = 0;
         do {
             const SE3 backup = est;
             double Hl[6][6];
@@ -193,6 +213,7 @@ struct LM {
 #else
             const bool ok2 = solve6(Hl, b, x);
 #endif
+            if (tr && x[0] * x[0] + x[1] * x[1] + x[2] * x[2] >= 0.25) tr->any_sincos = 1;
             est = se3_mul(se3_exp(x), est);
             compute_active_errors();
             temp = active_robust_chi2();
@@ -202,40 +223,46 @@ struct LM {
             for (int j = 0; j < 6; ++j) scale += x[j] * (lambda * x[j] + b[j]);
             scale += 1e-3;
             rho /= scale;
+            if (tr && ok2 && !(current == 0 && temp == 0) && std::isfinite(rho)) tr->min_rho_margin = std::min(tr->min_rho_margin, std::fabs(rho));
             if (rho > 0 && std::isfinite(temp)) {
                 double alpha = 1. - std::pow((2 * rho - 1), 3);
                 alpha = std::min(alpha, 2. / 3.);
                 const double sf = std::max(1. / 3., alpha);
                 lambda *= sf; ni = 2; current = temp;
+                if (tr) { tr->max_reject_run = std::max(tr->max_reject_run, run); tr->max_accepted_trial = std::max(tr->max_accepted_trial, qmax); }
+                run = 0;
             } else {
                 lambda *= ni; ni *= 2; est = backup;
+                if (tr) { tr->rejected += 1; tr->max_reject_run = std::max(tr->max_reject_run, ++run); }
             }
             ++qmax;
         } while (rho < 0 && qmax < 10);
-        if (qmax == 10 || rho == 0) return false;
+        if (qmax == 10 || rho == 0) {
+            if (tr) (qmax == 10 ? tr->term_qmax : tr->term_rho0) += 1;
+            return false;
+        }
+        if (tr && ini != 0) margin(tr->min_stop_margin, (ini - current) * 1e3 - ini, ini);
         if ((ini - current) * 1e3 < ini) ++n_bad; else n_bad = 0;
-        if (n_bad >= 3) return false;
+        if (n_bad >= 3) {
+            if (tr) tr->term_nbad += 1;
+            return false;
+        }
         return true;
     }
-    void optimize(int iterations) {
+    int optimize(int iterations) {
         bool any = false;
         for (const Edge& e : edges) if (e.level == 0) { any = true; break; }
-        (void)any;    // g2o keeps the vertex active even with no active edges; H = 0 -> LDLT not positive -> rho = 0 path
+        if (tr && !any) tr->empty_rounds += 1;      // g2o keeps the vertex active even with no active edges; H = 0 -> LDLT not positive -> rho = 0 path
         bool ok = true;
-        for (int i = 0; i < iterations && ok; ++i) ok = solve_iteration(i);
+        int i = 0;
+        for (; i < iterations && ok; ++i) ok = solve_iteration(i);
+        if (tr && ok) tr->term_iters += 1;
+        return i;
     }
 };
 
-}  // namespace
-
-extern "C" {
-
-// pose = (qx, qy, qz, qw, tx, ty, tz) float (Sophus::SE3f of Frame::GetPose()).  Edges in keypoint order i:
-// xw (3 floats, MapPoint::GetWorldPos()), obs = (kpUn.x, kpUn.y, uRight) floats, inv_sigma2 float, stereo = (uRight >= 0).
-// outlier[i] written like pFrame->mvbOutlier.  Returns nInitialCorrespondences - nBad (0 if < 3 correspondences).
-int orc_pose_optimize(const float pose_in[7], int n, const float* xw, const float* obs, const float* inv_sigma2,
-                      const uint8_t* stereo, float fx, float fy, float cx, float cy, float bf,
-                      float pose_out[7], uint8_t* outlier) {
+int pose_optimize(const float pose_in[7], int n, const float* xw, const float* obs, const float* inv_sigma2, const uint8_t* stereo,
+                  float fx, float fy, float cx, float cy, float bf, float pose_out[7], uint8_t* outlier, PoseTrace* tr) {
     for (int i = 0; i < 7; ++i) pose_out[i] = pose_in[i];
     if (n < 3) return 0;
     std::vector<Edge> edges(n);
@@ -248,6 +275,7 @@ int orc_pose_optimize(const float pose_in[7], int n, const float* xw, const floa
     const Cam cam = {fx, fy, cx, cy, bf};
     const float delta_mono = std::sqrt(5.991), delta_stereo = std::sqrt(7.815);      // src/Optimizer.cc:852-853
     LM lm{edges, cam, delta_mono, delta_stereo, (float)((double)delta_mono * delta_mono), (float)((double)delta_stereo * delta_stereo)};
+    lm.tr = tr;
     SE3 init;
     init.r = {pose_in[0], pose_in[1], pose_in[2], pose_in[3]};
     init.t[0] = pose_in[4]; init.t[1] = pose_in[5]; init.t[2] = pose_in[6];
@@ -257,13 +285,16 @@ int orc_pose_optimize(const float pose_in[7], int n, const float* xw, const floa
     int n_bad = 0;
     for (int it = 0; it < 4; ++it) {
         lm.est = init;
-        lm.optimize(10);
+        const int iters = lm.optimize(10);
+        if (tr) { tr->iters[it] = iters; tr->rounds = it + 1; }
         n_bad = 0;
         for (int i = 0; i < n; ++i) {
             Edge& e = edges[i];
             if (outlier[i]) edge_error(e, lm.est, cam);
             const float chi2 = (float)edge_chi2(e);
-            if (chi2 > (e.stereo ? chi2_stereo : chi2_mono)) { outlier[i] = 1; e.level = 1; ++n_bad; }
+            const float thr = e.stereo ? chi2_stereo : chi2_mono;
+            if (tr) margin(tr->min_chi2_margin, (double)chi2 - thr, thr);
+            if (chi2 > thr) { outlier[i] = 1; e.level = 1; ++n_bad; }
             else { outlier[i] = 0; e.level = 0; }
             if (it == 2) e.robust = false;
         }
@@ -276,6 +307,28 @@ int orc_pose_optimize(const float pose_in[7], int n, const float* xw, const floa
     for (int i = 0; i < 4; ++i) pose_out[i] = qf[i] / length;
     pose_out[4] = (float)lm.est.t[0]; pose_out[5] = (float)lm.est.t[1]; pose_out[6] = (float)lm.est.t[2];
     return n - n_bad;
+}
+
+}  // namespace
+
+extern "C" {
+
+// pose = (qx, qy, qz, qw, tx, ty, tz) float (Sophus::SE3f of Frame::GetPose()).  Edges in keypoint order i:
+// xw (3 floats, MapPoint::GetWorldPos()), obs = (kpUn.x, kpUn.y, uRight) floats, inv_sigma2 float, stereo = (uRight >= 0).
+// outlier[i] written like pFrame->mvbOutlier.  Returns nInitialCorrespondences - nBad (0 if < 3 correspondences).
+int orc_pose_optimize(const float pose_in[7], int n, const float* xw, const float* obs, const float* inv_sigma2,
+                      const uint8_t* stereo, float fx, float fy, float cx, float cy, float bf,
+                      float pose_out[7], uint8_t* outlier) {
+    return pose_optimize(pose_in, n, xw, obs, inv_sigma2, stereo, fx, fy, cx, cy, bf, pose_out, outlier, nullptr);
+}
+
+// orc_pose_optimize with the same arithmetic and outputs, plus what the call did (PoseTrace above)
+int orc_pose_optimize_trace(const float pose_in[7], int n, const float* xw, const float* obs, const float* inv_sigma2,
+                            const uint8_t* stereo, float fx, float fy, float cx, float cy, float bf,
+                            float pose_out[7], uint8_t* outlier, PoseTrace* tr) {
+    *tr = PoseTrace{};
+    tr->min_rho_margin = tr->min_stop_margin = tr->min_chi2_margin = std::numeric_limits<double>::infinity();
+    return pose_optimize(pose_in, n, xw, obs, inv_sigma2, stereo, fx, fy, cx, cy, bf, pose_out, outlier, tr);
 }
 
 }  // extern "C"

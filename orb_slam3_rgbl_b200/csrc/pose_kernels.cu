@@ -136,9 +136,10 @@ __device__ __forceinline__ double rcp_newton(double d) {
 // rounding only (covered by the 1e-5 pose tolerance of the parity tests; the oracle keeps the pivoted form).  This runs on
 // ONE thread and is bound by the latency of dependent FP64 operations (~36 cycles each, measured), so it is written for a
 // short dependency chain: compile-time indices (registers), b eliminated alongside the columns, one Newton reciprocal per
-// pivot, column-oriented back substitution.  Returns false when a pivot is negative or not finite (Eigen's isPositive() ==
-// false -> g2o treats the trial as failed); an exactly zero pivot (no active edge and lambda == 0) leaves that unknown at 0
-// like Eigen's solve does.
+// pivot, column-oriented back substitution.  Returns false when a pivot is negative (Eigen's isPositive() == false -> g2o treats
+// the trial as failed); an exactly zero pivot (no active edge and lambda == 0) leaves that unknown at 0 like Eigen's solve does.
+// A NaN pivot (an edge exactly on the camera plane makes H NaN) is neither positive nor negative for Eigen's sign tracking, so the
+// solve "succeeds" with a NaN step, the trial is rejected and its NaN errors are what the classification reads, as in g2o.
 __device__ __forceinline__ bool solve6(const double* Hsym /*21 upper*/, double lambda, const double* b, double* x) {
     double L[6][6], dinv[6], y[6];
     // every loop has the constant trip count 6 with compile-time guards: triangular bounds defeat the unroller, and one
@@ -154,7 +155,7 @@ __device__ __forceinline__ bool solve6(const double* Hsym /*21 upper*/, double l
 #pragma unroll
     for (int k = 0; k < 6; ++k) {
         const double d = L[k][k];
-        positive = positive && (d >= 0) && (d <= DBL_MAX);
+        positive = positive && !(d < 0);
         dinv[k] = (d >= DBL_MIN && d <= DBL_MAX) ? rcp_newton(d) : 0.0;
 #pragma unroll
         for (int i = 0; i < 6; ++i) {

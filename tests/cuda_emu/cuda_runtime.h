@@ -2,17 +2,23 @@
 // library's .cu files with g++ against this header so that the DEVICE branches of those kernels (__CUDA_ARCH__ code paths:
 // shuffle scans, shared-memory atomics, warp collectives, launch geometry) execute on the CPU: every CTA of a launch runs
 // with one OS thread per CUDA thread, __syncthreads is a real barrier, warp collectives rendezvous the 32 lanes of a warp.
+// A kernel declared with __cluster_dims__ runs its CTAs cluster by cluster, all CTAs of a cluster at once, with per-CTA shared
+// memory in an emulated shared window (build.py rewrites that kernel's __shared__ declarations and its DSMEM / mbarrier PTX).
 // Only what those kernels use is provided.
 #pragma once
 #include <algorithm>
 #include <atomic>
 #include <barrier>
+#include <chrono>
 #include <cmath>
+#include <condition_variable>
 #include <cstdint>
+#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <functional>
 #include <memory>
+#include <mutex>
 #include <thread>
 #include <vector>
 
@@ -27,8 +33,9 @@
 #define __restrict__
 #define __launch_bounds__(...)
 #define __align__(n) __attribute__((aligned(n)))
-#define __shared__ static                 /* one CTA runs at a time */
+#define __shared__ static                 /* one CTA runs at a time (cluster kernels: see emu::cluster_shared) */
 #define __constant__ static
+#define __cluster_dims__(...)
 
 struct uint3 { unsigned x, y, z; };
 struct dim3 { unsigned x, y, z; dim3(unsigned a = 1, unsigned b = 1, unsigned c = 1) : x(a), y(b), z(c) {} };
@@ -37,7 +44,7 @@ struct alignas(16) uint4 { unsigned x, y, z, w; };
 typedef int cudaError_t;
 typedef void* cudaStream_t;
 enum { cudaSuccess = 0 };
-enum cudaFuncAttribute { cudaFuncAttributeMaxDynamicSharedMemorySize = 8 };
+enum cudaFuncAttribute { cudaFuncAttributeMaxDynamicSharedMemorySize = 8, cudaFuncAttributeNonPortableClusterSizeAllowed = 11 };
 enum cudaDeviceAttr { cudaDevAttrMaxSharedMemoryPerBlockOptin = 97, cudaDevAttrMaxSharedMemoryPerMultiprocessor = 81 };
 struct cudaFuncAttributes { size_t sharedSizeBytes = 0; };
 template <class F> inline cudaError_t cudaFuncSetAttribute(F, cudaFuncAttribute, int) { return cudaSuccess; }
@@ -53,11 +60,91 @@ struct Cta {
     std::vector<std::array<unsigned long long, 32>> slot;
     std::atomic<int> nb_count{0}, nb_gen{0};      // named barrier of a subset of the CTA's threads (team_sync)
 };
-extern Cta* g_cta;
+extern thread_local Cta* g_cta;
 extern thread_local int t_warp, t_lane;
 struct Cfg { dim3 grid, block; size_t smem; };
 inline Cfg cfg(dim3 g, dim3 b, size_t smem = 0, cudaStream_t = nullptr) { return Cfg{g, b, smem}; }
 void run(const Cfg& c, const std::function<void()>& body);
+[[noreturn]] inline void fail(const char* what) { std::fprintf(stderr, "cuda_emu: %s\n", what); std::fflush(stderr); std::abort(); }
+
+// ---- thread-block clusters ---------------------------------------------------------------------------------------------------------
+// next_launch_cluster(n): the next launch runs as clusters of n CTAs (build.py inserts it before the launch of a __cluster_dims__ kernel).
+// All n x blockDim threads of a cluster are OS threads at once; cluster.sync() is a barrier over all of them.
+struct Cluster { std::unique_ptr<std::barrier<>> bar; unsigned size = 1; };
+extern thread_local Cluster* t_cluster;
+extern thread_local unsigned t_rank;              // rank of this thread's CTA in its cluster
+void next_launch_cluster(unsigned n);
+inline void cluster_sync() { t_cluster->bar->arrive_and_wait(); }
+
+// Shared memory of a cluster kernel: a window of kMaxClusterCtas slots of kCtaWindow bytes, slot r = CTA rank r.  A 32-bit shared
+// address is an offset into the window (so mapa is slot arithmetic); build.py turns each `__shared__ T x[..];` of such a kernel into
+// `auto& x = emu::cluster_shared<T[..], id>();`, a fixed offset in the slot of the calling thread's CTA.
+constexpr unsigned kMaxClusterCtas = 16;
+constexpr size_t kCtaWindow = 1 << 16;
+extern unsigned char g_window[kMaxClusterCtas][kCtaWindow];
+size_t window_reserve(size_t size, size_t align);
+template <class T, int Id> inline T& cluster_shared() {
+    static const size_t off = window_reserve(sizeof(T), alignof(T) < 16 ? 16 : alignof(T));
+    return *reinterpret_cast<T*>(&g_window[t_rank][off]);
+}
+inline uint32_t window_addr(const void* p) {
+    const auto* c = static_cast<const unsigned char*>(p);
+    if (c < &g_window[0][0] || c >= &g_window[0][0] + sizeof(g_window)) fail("shared address of a variable outside the cluster shared window");
+    return (uint32_t)(c - &g_window[0][0]);
+}
+inline unsigned char* window_ptr(uint32_t a) { return &g_window[0][0] + a; }
+inline uint32_t mapa(uint32_t a, uint32_t rank) {          // mapa.shared::cluster: the same variable in CTA `rank`
+    if (rank >= t_cluster->size) fail("mapa: rank outside the cluster");
+    return (uint32_t)(a % kCtaWindow + rank * kCtaWindow);
+}
+
+// mbarrier (PTX ISA "mbarrier"): one 64-bit word in shared memory holding the phase parity, the arrival count, the pending arrivals and
+// the tx-count of the current phase.  The phase completes when the pending arrivals AND the tx-count are both zero; a complete_tx that
+// runs ahead of the expect_tx makes the tx-count negative for a while, as on the device.  A wrong byte count therefore never completes
+// (try_wait times out below) or completes early.
+struct Mbar { unsigned phase, count, pending; int32_t tx; };
+inline Mbar mbar_unpack(uint64_t w) { return Mbar{(unsigned)(w >> 63), (unsigned)(w >> 48) & 0x7fff, (unsigned)(w >> 32) & 0xffff, (int32_t)(uint32_t)w}; }
+inline uint64_t mbar_pack(const Mbar& m) { return (uint64_t)m.phase << 63 | (uint64_t)m.count << 48 | (uint64_t)m.pending << 32 | (uint32_t)m.tx; }
+inline std::atomic_ref<uint64_t> mbar_word(uint32_t a) {
+    if (a % 8) fail("mbarrier not 8-byte aligned");
+    return std::atomic_ref<uint64_t>(*reinterpret_cast<uint64_t*>(window_ptr(a)));
+}
+extern std::mutex g_mbar_mu;
+extern std::condition_variable g_mbar_cv;
+inline void mbar_init(uint32_t a, unsigned count) { mbar_word(a).store(mbar_pack(Mbar{0, count, count, 0}), std::memory_order_release); }
+inline void mbar_update(uint32_t a, unsigned arrivals, int32_t tx) {
+    auto w = mbar_word(a);
+    uint64_t o = w.load(std::memory_order_relaxed), n;
+    bool flipped;
+    do {
+        Mbar m = mbar_unpack(o);
+        if (m.count == 0) fail("mbarrier used before mbarrier.init");
+        if (m.pending < arrivals) fail("mbarrier: more arrivals than its count in one phase");
+        m.pending -= arrivals; m.tx += tx;
+        flipped = m.pending == 0 && m.tx == 0;
+        if (flipped) { m.phase ^= 1; m.pending = m.count; }
+        n = mbar_pack(m);
+    } while (!w.compare_exchange_weak(o, n, std::memory_order_acq_rel, std::memory_order_relaxed));
+    if (flipped) { { std::lock_guard<std::mutex> lk(g_mbar_mu); } g_mbar_cv.notify_all(); }
+}
+inline void mbar_arrive_expect_tx(uint32_t a, unsigned bytes) { mbar_update(a, 1, (int32_t)bytes); }
+// st.async.shared::cluster.mbarrier::complete_tx::bytes.b64: store 8 bytes into (possibly another CTA's) shared memory, then signal
+// the mbarrier of the CTA that owns it
+inline void st_async_b64(uint32_t dst, unsigned long long v, uint32_t mbar) {
+    if (dst / kCtaWindow != mbar / kCtaWindow) fail("st.async: data and mbarrier in different CTAs");
+    std::memcpy(window_ptr(dst), &v, 8);
+    mbar_update(mbar, 0, -8);
+}
+// mbarrier.try_wait.parity: true once the phase of that parity has completed.  It blocks here (a device try_wait returns false after a
+// while and the caller spins); a phase that does not complete within a minute is a lost exchange and aborts the process.
+inline uint32_t mbar_try_wait_parity(uint32_t a, unsigned parity) {
+    auto w = mbar_word(a);
+    auto done = [&] { return mbar_unpack(w.load(std::memory_order_acquire)).phase != (parity & 1); };
+    if (done()) return 1;
+    std::unique_lock<std::mutex> lk(g_mbar_mu);
+    if (!g_mbar_cv.wait_for(lk, std::chrono::seconds(60), done)) fail("mbarrier.try_wait: the phase never completed (lost exchange: wrong tx byte count or parity)");
+    return 1;
+}
 inline double approx64(double v) { unsigned long long u; std::memcpy(&u, &v, 8); u &= 0xffffffff00000000ull; std::memcpy(&v, &u, 8); return v; }
 inline void warp_sync() { g_cta->warp_bar[t_warp]->arrive_and_wait(); }
 inline void named_barrier(int n) {
@@ -80,8 +167,10 @@ template <class T> inline T exchange(T v, int src_lane) {       // every lane pu
 }  // namespace emu
 
 extern thread_local uint3 threadIdx;
-extern uint3 blockIdx;
+extern thread_local uint3 blockIdx;
 extern dim3 blockDim, gridDim;
+inline size_t __cvta_generic_to_shared(const void* p) { return emu::window_addr(p); }
+[[noreturn]] inline void __trap() { emu::fail("__trap() in a kernel"); }
 
 inline void __syncthreads() { emu::g_cta->bar->arrive_and_wait(); }
 inline void __syncwarp(unsigned = 0xffffffffu) { emu::warp_sync(); }
@@ -155,6 +244,7 @@ inline int __float2int_rn(float v) { return (int)lrintf(v); }
 inline float __fmaf_rn(float a, float b, float c) { return fmaf(a, b, c); }
 inline float __uint_as_float(unsigned u) { float f; std::memcpy(&f, &u, 4); return f; }
 inline unsigned __float_as_uint(float f) { unsigned u; std::memcpy(&u, &f, 4); return u; }
+inline long long __double_as_longlong(double d) { long long u; std::memcpy(&u, &d, 8); return u; }
 inline double rsqrt(double x) { return 1.0 / std::sqrt(x); }
 inline void sincos(double x, double* s, double* c) { *s = std::sin(x); *c = std::cos(x); }
 using std::isfinite;
@@ -215,6 +305,7 @@ inline cudaError_t cudaLaunchKernelEx(const cudaLaunchConfig_t* cfg, void (*kern
     emu::run(emu::Cfg{cfg->gridDim, cfg->blockDim, cfg->dynamicSmemBytes}, [&]() { kernel(args...); });
     return cudaSuccess;
 }
+template <class F> inline cudaError_t cudaOccupancyMaxActiveClusters(int* n, F, const cudaLaunchConfig_t*) { *n = 1; return cudaSuccess; }
 // CUDA graphs are not emulated: capture is refused (the library replays the chain launch by launch when RGBL_CHAIN_GRAPH=0)
 inline cudaError_t cudaStreamBeginCapture(cudaStream_t, cudaStreamCaptureMode) { return cudaErrorNotSupported; }
 inline cudaError_t cudaStreamEndCapture(cudaStream_t, cudaGraph_t* g) { *g = nullptr; return cudaErrorNotSupported; }

@@ -1,16 +1,8 @@
-// TEST INFRASTRUCTURE (emulated library only): pose_kernels.cu is a thread-block-cluster kernel (DSMEM st.async + mbarrier) that the
-// CUDA-on-CPU shim does not model, so the emulated library refuses PoseOptimization loudly instead of computing it some other way.
-#include <cstdio>
-#include <cstdlib>
+// TEST INFRASTRUCTURE (emulated library only): level_tma_kernels.cu builds TMA tensor maps, which the CUDA-on-CPU shim does not
+// model; without tensor maps the library uses resize_level_kernel + blur_level_kernel.
 #include "rgbl_kernels.h"
 
 namespace rgbl {
-const char* pose_cluster_unsupported(int) { return nullptr; }     // reaches launch_pose_optimize below, which refuses loudly
-void launch_pose_optimize(cudaStream_t, const PoseProblemDev&, double*, uint8_t*, uint8_t*, float*, int*, const ChainPrepDev*) {
-    std::fprintf(stderr, "librgbl_b200_emu: PoseOptimization (pose_kernels.cu, 4-CTA cluster) is not emulated; run it on the GPU\n");
-    std::abort();
-}
-// level_tma_kernels.cu (TMA tensor maps) is not emulated either: no tensor maps -> the library uses resize_level_kernel + blur_level_kernel
 int make_level_tensor_maps(uint8_t*, size_t, int, const LevelGeom*, int, LevelTensorMaps* out) { out->n_levels = 0; return -1; }
 int launch_level_tiles(cudaStream_t, const LevelTensorMaps&, uint8_t*, uint8_t*, size_t, const LevelGeom*, int, const LinCoef*, int) { return -1; }
 }  // namespace rgbl

@@ -2,8 +2,8 @@
  * Creates and destroys contexts and runs every lazily allocating entry point.  For rgbl_create and the PNG, RGB-D, stage, tracking,
  * BoW and mapping paths it fails the k-th allocation for each k (emu_fail_allocation, cuda_runtime.h in this directory) and checks
  * that the failed call reports RGBL_E_CUDA and that a retry on the same context succeeds with the outputs of a fresh context.
- * LeakSanitizer checks at exit that nothing leaks.  PoseOptimization and the tracking chain are not emulated, so nothing here
- * reaches them.  Frame construction is slow under emulation: the RGB-D path is the one that runs it.
+ * LeakSanitizer checks at exit that nothing leaks.  PoseOptimization and the tracking chain are not called here (the emulated pose
+ * kernel is tests/test_cuda_emu_pose.py's).  Frame construction is slow under emulation: the RGB-D path is the one that runs it.
  * Exit 0: every check passed.                                                                                                   */
 #include <math.h>
 #include <stdio.h>

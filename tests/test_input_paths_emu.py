@@ -1,8 +1,8 @@
 """Input paths of frame construction: every upload, PNG upload, stage, process and sequence-runner entry point of each input kind
 (RGB-L, RGB-D, stereo) called with inputs that have one fault each, against the whole library compiled over the CUDA-on-CPU shim
 (tests/cuda_emu).  Each case asserts its status code.  After each refused call the same context must still build frames: one valid
-batch of the case's kind is uploaded, processed and downloaded, and must equal a fresh context's outputs bit for bit.  PoseOptimization
-is not emulated, so every runner case fails before the tracking chain starts."""
+batch of the case's kind is uploaded, processed and downloaded, and must equal a fresh context's outputs bit for bit.  Every runner
+case is refused before its tracking chain starts."""
 import ctypes as C
 import importlib.util
 from pathlib import Path
