@@ -449,6 +449,29 @@ int rgbl_track_sequence_stereo(rgbl_ctx* ctx, float mb, float mbf, const rgbl_ch
  * rectified ones (Settings: P1's intrinsics, bf = b * P1(0,0)).  Setting or clearing the maps discards a pending stereo upload (the process
  * call then reports "nothing uploaded"); staged slots stay valid.                                                                       */
 int rgbl_set_stereo_rectification(rgbl_ctx* ctx, const float* m1l, const float* m2l, const float* m1r, const float* m2r, int map_stride);
+/* Input resize on the device: the cv::resize(im, im, newImSize, INTER_LINEAR) that System::TrackRGBD and System::TrackStereo run on every
+ * image when Settings::needToResize() (Camera.newWidth / Camera.newHeight), and TrackRGBD on the CV_16U depth image too.  The context's
+ * width x height is Settings::newImSize(); src_width x src_height is the camera's original size.  Everything downstream sees the
+ * context's size: the extractor, the camera model, the chain and the rectification maps.  The caller passes the intrinsics Settings scaled
+ * (fx, cx by newWidth / width, fy, cy by newHeight / height; mb / mbf) as it does without the resize.
+ * (0, 0) or the context's own size turns the resize off (the default).  A chain in flight, a negative size, or only one of the two sizes
+ * zero is RGBL_E_INVALID; an input size smaller than the context's in either axis (upscaling) is RGBL_E_UNSUPPORTED.  A refused call leaves
+ * the previous setting in place.  Setting or clearing the resize discards a pending upload of any kind.
+ * While the resize is on:
+ *   - the RGB-D and stereo uploads, PNG uploads, stage calls and sequence runners take images (and depth images, and PNG streams) at the
+ *     input size; the resize writes level 0 of the frame slots (one launch per batch, billed to the `pyramid` stage) and, for RGB-D, the
+ *     context-size depth plane of the gather (on the aux stream, billed to `depth_gather`).  Both are bit-exact with OpenCV;
+ *   - RGB-D needs integer factors (src_width % width == 0 and src_height % height == 0; else RGBL_E_UNSUPPORTED), the case OpenCV's
+ *     16-bit linear resize is restated for; stereo and 8-bit images take any downscale;
+ *   - image PNG streams must be 8-bit gray (colour: RGBL_E_UNSUPPORTED: the reference resizes before its conversion to gray);
+ *   - a staged slot holds input-size planes and records the input size: a runner given a slot staged at another size returns
+ *     RGBL_E_INVALID;
+ *   - every RGB-L entry point (uploads, _kitti, _kitti_png, stage, process, rgbl_track_sequence, rgbl_frame_rgbl_batch) returns
+ *     RGBL_E_UNSUPPORTED: the reference never resizes RGB-L input and the LiDAR projection P describes the original image;
+ *   - with rectification on too, stereo pairs go through the remap alone, as in TrackStereo: the maps keep the context's size and their
+ *     coordinates index the input-size images (Settings builds them for newImSize);
+ *   - rgbl_decode_png_gray / rgbl_decode_png_depth16, rgbl_orb_extract* and the depth-from-map / point-cloud calls keep the context's size. */
+int rgbl_set_input_resize(rgbl_ctx* ctx, int src_width, int src_height);
 
 /* ---- Camera model of Frame::UndistortKeyPoints / ComputeImageBounds (src/Frame.cc:837-899) for every later batched frame construction
  * (rgbl_frame_rgbl_batch, rgbl_resident_process, rgbl_resident_process_rgbd, both sequence runners) and tracking chain of this context:

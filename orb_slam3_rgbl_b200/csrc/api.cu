@@ -27,9 +27,10 @@ static void release(Ctx* c) {
     delete c;
 }
 
-// a lazily allocated array: allocated by the first call that needs it (and retried by the next call if that allocation failed)
+// a lazily allocated array of at least n elements: allocated by the first call that needs it, reallocated (contents not kept) by a call
+// that needs more (the input planes after a larger rgbl_set_input_resize), and retried by the next call if that allocation failed
 template <class A>
-static bool ensure(A& a, size_t n) { return a || a.alloc(n) == cudaSuccess; }
+static bool ensure(A& a, size_t n) { return a.size() >= n || a.alloc(n) == cudaSuccess; }
 
 static int create(const rgbl_config* cfg, Ctx** out) {
     Ctx* c = new Ctx();
@@ -42,6 +43,7 @@ static int create(const rgbl_config* cfg, Ctx** out) {
     rc = build_geometry(cfg->width, cfg->height, c->tab, c->levels, c->cells, c->coefs, c->frame_bytes, c->err);
     if (rc) return fail(rc);
     c->n_cells = (int)c->cells.size();
+    c->in_w = cfg->width; c->in_h = cfg->height; c->in_pitch = c->levels[0].pitch;      // no input resize
     // DistributeOctTree returns at most max(quota + 2, 4 * nIni) keypoints per level (SURVEY App. C: the very
     // first subdivision pass is unguarded, later ones stop within +3 of the budget).
     c->cap_kp = 0;
@@ -172,6 +174,9 @@ void prof_collect(Ctx* c) {
         c->st_used[i] = false;
         c->st_pending_launches[i] = 0;
     }
+    float ms = 0.f;
+    if (c->prof_on && c->rsd_used && cudaEventElapsedTime(&ms, c->ev_rsd_b, c->ev_rsd_e) == cudaSuccess) c->st_ms[ST_DEPTH_GATHER] += ms;
+    c->rsd_used = false;
 }
 
 // ---- extraction pipeline -----------------------------------------------------------------------
@@ -180,24 +185,26 @@ void prof_collect(Ctx* c) {
 // Stage 2 (host):   quad-tree per (frame, level) on worker threads -> SelKp lists.
 // Stage 3 (device): describe.  Results stay in d_kps / d_desc (copied out by the callers).
 
-// The image planes of a batch: plane f at base + f * stride + off, rows pitch bytes apart.  raw: the planes are the remap's source
-// (stereo pairs with rectification on), not level 0.
+// The image planes of a batch: plane f at base + f * stride + off, rows pitch bytes apart, w x h pixels.  raw: the planes are the source of
+// the kernel that writes level 0 (the remap of stereo pairs with rectification on, or the input resize), not level 0.
 struct Planes {
-    uint8_t* base; size_t stride, off; int pitch; bool raw;
+    uint8_t* base; size_t stride, off; int pitch; bool raw; int w, h;
     uint8_t* at(int f) const { return base + (size_t)f * stride + off; }
 };
 
-static Planes level0_planes(const Ctx* c) { return {c->d_pyr, c->frame_bytes, (size_t)c->levels[0].off, c->levels[0].pitch, false}; }
+static Planes level0_planes(const Ctx* c) {
+    return {c->d_pyr, c->frame_bytes, (size_t)c->levels[0].off, c->levels[0].pitch, false, c->cfg.width, c->cfg.height};
+}
 
 // H2D of n host images into planes [first, first + n) of dst, on stream st
 static int upload_planes(Ctx* c, const Planes& dst, int first, int n, const uint8_t* const* img, int stride, cudaStream_t st) {
     for (int f = 0; f < n; ++f)
-        CU(cudaMemcpy2DAsync(dst.at(first + f), dst.pitch, img[f], stride, c->cfg.width, c->cfg.height, cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpy2DAsync(dst.at(first + f), dst.pitch, img[f], stride, dst.w, dst.h, cudaMemcpyHostToDevice, st));
     return RGBL_OK;
 }
 
-// level0: if set, enqueues the kernels that write level 0 on the main stream (rectification of stereo pairs) and returns their count;
-// billed to the pyramid stage.
+// level0: if set, enqueues the kernels that write level 0 on the main stream (rectification of stereo pairs, the input resize) and returns
+// their count; billed to the pyramid stage.
 static int run_extract(Ctx* c, int n_frames, const std::function<void()>& aux_work = nullptr, const std::function<int()>& level0 = nullptr) {
     const int nl = c->tab.nlevels;
     // new frames: mvKeysUn == mvKeys and image bounds until undistort_keypoints says otherwise
@@ -683,9 +690,13 @@ int rgbl_depth_from_map(rgbl_ctx* ctx, const float* depth_map, int width, int he
     return RGBL_OK;
 }
 
-static int check_batch_args(Ctx* c, int n_frames, int width, int height, int stride) {
+// input_size: the images are camera input (the input size, rgbl_set_input_resize), else they have the context's size
+static int check_batch_args(Ctx* c, int n_frames, int width, int height, int stride, bool input_size = true) {
     if (width <= 0 || height <= 0) { c->err = "empty image"; return RGBL_E_EMPTY; }
-    if (width != c->cfg.width || height != c->cfg.height || stride < width) { c->err = "image size does not match the context"; return RGBL_E_INVALID; }
+    const bool rs = input_size && c->resize;
+    if (width != (rs ? c->in_w : c->cfg.width) || height != (rs ? c->in_h : c->cfg.height) || stride < width) {
+        c->err = rs ? "image size does not match the input size (rgbl_set_input_resize)" : "image size does not match the context"; return RGBL_E_INVALID;
+    }
     if (n_frames < 1) { c->err = "n_frames < 1"; return RGBL_E_INVALID; }
     if (n_frames > c->cfg.max_batch) { c->err = "n_frames exceeds max_batch"; return RGBL_E_CAPACITY; }
     return RGBL_OK;
@@ -753,7 +764,7 @@ static int check_inputs(Ctx* c, const HostInputs& in, int* max_pts) {
     for (int f = 0; f < in.n; ++f)
         if (!in.gray[f] || (in.right && !in.right[f])) { c->err = "empty image"; return RGBL_E_EMPTY; }
     if (in.kind == InputKind::rgbd) {
-        if (!in.depth || in.depth_stride < c->cfg.width) { c->err = !in.depth ? "null argument" : "depth_stride < width"; return RGBL_E_INVALID; }
+        if (!in.depth || in.depth_stride < c->in_w) { c->err = !in.depth ? "null argument" : "depth_stride < width"; return RGBL_E_INVALID; }
         for (int f = 0; f < in.n; ++f) if (!in.depth[f]) { c->err = "empty depth image"; return RGBL_E_EMPTY; }
     }
     return RGBL_OK;
@@ -761,9 +772,9 @@ static int check_inputs(Ctx* c, const HostInputs& in, int* max_pts) {
 
 // cv::imread(PNG, IMREAD_UNCHANGED) + cvtColor to gray (Examples/RGB-L/rgbl_kitti.cc:87, src/Tracking.cc:1567-1580) into the image planes
 // of the batch: host inflate into pinned staging, H2D of the filtered scanlines, reconstruction + gray on the device.
-static int ensure_png_staging(Ctx* c) {
-    const size_t w = c->cfg.width, B = c->cfg.max_batch;
-    c->png_raw_stride = ((w * 4 + 1) * c->cfg.height + 255) & ~(size_t)255;
+static int ensure_png_staging(Ctx* c, int width, int height) {
+    const size_t w = width, B = c->cfg.max_batch;
+    c->png_raw_stride = ((w * 4 + 1) * height + 255) & ~(size_t)255;
     if (!c->d_png_status) {          // allocated and zeroed, or not at all
         if (c->d_png_status.alloc(1) != cudaSuccess) { c->err = "allocation of the PNG staging buffers failed"; return RGBL_E_CUDA; }
         if (cudaMemset(c->d_png_status, 0, sizeof(int)) != cudaSuccess) { c->d_png_status.reset(); c->err = "cudaMemset failed (PNG status word)"; return RGBL_E_CUDA; }
@@ -775,21 +786,17 @@ static int ensure_png_staging(Ctx* c) {
     return RGBL_OK;
 }
 
-// host inflate of n PNG streams into the pinned staging buffer + H2D of the filtered scanlines -> bytes per pixel (or < 0).
-// gray_only: a colour stream is RGBL_E_UNSUPPORTED, refused before anything is copied.
-static int inflate_png_batch(Ctx* c, int n_frames, const uint8_t* const* png, const size_t* png_bytes, bool depth16, cudaStream_t st, bool gray_only = false) {
-    const int w = c->cfg.width, h = c->cfg.height;
-    int rc = ensure_png_staging(c); if (rc) return rc;
+// host inflate of n PNG streams of w x h pixels into the pinned staging buffer + H2D of the filtered scanlines -> bytes per pixel (or < 0).
+// gray_only: if given, a colour stream is RGBL_E_UNSUPPORTED with this message, refused before anything is copied.
+static int inflate_png_batch(Ctx* c, int n_frames, const uint8_t* const* png, const size_t* png_bytes, int w, int h, bool depth16, cudaStream_t st,
+                             const char* gray_only = nullptr) {
+    int rc = ensure_png_staging(c, w, h); if (rc) return rc;
     for (int f = 0; f < n_frames; ++f) if (!png[f] || !png_bytes[f]) { c->err = "empty image"; return RGBL_E_EMPTY; }
     int ch = 0;
     std::string perr;
     const int prc = png_inflate_batch(n_frames, png, png_bytes, w, h, c->h_png_raw, c->png_raw_stride, &ch, perr, depth16);
     if (prc) { c->err = perr; return prc == -2 ? RGBL_E_UNSUPPORTED : RGBL_E_INVALID; }
-    if (gray_only && ch != 1) {
-        // the reference remaps the image imread returned and converts it to gray afterwards, which differs for colour images
-        c->err = "rectified stereo takes 8-bit gray PNGs only (the reference remaps colour images before their conversion to gray)";
-        return RGBL_E_UNSUPPORTED;
-    }
+    if (gray_only && ch != 1) { c->err = gray_only; return RGBL_E_UNSUPPORTED; }
     const size_t used = ((size_t)w * ch + 1) * h;
     for (int f = 0; f < n_frames; ++f)
         CU(cudaMemcpyAsync(c->d_png_raw + (size_t)f * c->png_raw_stride, c->h_png_raw + (size_t)f * c->png_raw_stride, used, cudaMemcpyHostToDevice, st));
@@ -807,60 +814,74 @@ static int png_status(Ctx* c, cudaStream_t st) {
     return RGBL_OK;
 }
 
-// one raw plane of a stereo pair awaiting rectification: level 0's layout without the frame slot around it
-static size_t raw_plane_bytes(const Ctx* c) { return (size_t)c->levels[0].pitch * c->cfg.height; }
+// one raw image plane: level 0's layout at the input size (in_w x in_h, row pitch in_pitch) without the frame slot around it
+static size_t raw_plane_bytes(const Ctx* c) { return (size_t)c->in_pitch * c->in_h; }
 
 // Where the image planes of the batch being loaded go: into stage slot `slot` if given, else level 0 of the frame slots.  With
-// rectification on, stereo pairs are remapped into level 0 by process_stereo and nothing else writes it: their raw planes (rect_src)
-// are the planes of the slot `staged` that already holds them (base == nullptr: nothing to copy), or else the raw planes d_rect_raw.
+// rectification on (stereo pairs) or the input resize on (RGB-D frames, stereo pairs), process_stereo / process_rgbd write level 0 from
+// raw planes and nothing else writes it: the raw planes (raw_src) are the planes of the slot `staged` that already holds them (base ==
+// nullptr: nothing to copy), or else d_raw_img.
 static int image_planes(Ctx* c, InputKind kind, Ctx::StageSlot* slot, const Ctx::StageSlot* staged, Planes* p) {
-    const bool raw = kind == InputKind::stereo && c->rectify;
-    if (slot) { *p = {slot->img, raw_plane_bytes(c), 0, c->levels[0].pitch, raw}; return RGBL_OK; }
+    const bool raw = (kind == InputKind::stereo && c->rectify) || (kind != InputKind::rgbl && c->resize);
+    if (slot) { *p = {slot->img, raw_plane_bytes(c), 0, c->in_pitch, raw, c->in_w, c->in_h}; return RGBL_OK; }
     if (!raw) { *p = level0_planes(c); return RGBL_OK; }
-    if (staged) { c->rect_src = staged->img; *p = {nullptr, 0, 0, 0, true}; return RGBL_OK; }
-    if (!ensure(c->d_rect_raw, c->cfg.max_batch * raw_plane_bytes(c))) { c->err = "device allocation failed (raw stereo planes)"; return RGBL_E_CUDA; }
-    c->rect_src = c->d_rect_raw;
-    *p = {c->d_rect_raw, raw_plane_bytes(c), 0, c->levels[0].pitch, true};
+    if (staged) { c->raw_src = staged->img; *p = {nullptr, 0, 0, 0, true, 0, 0}; return RGBL_OK; }
+    if (!ensure(c->d_raw_img, c->cfg.max_batch * raw_plane_bytes(c))) { c->err = "device allocation failed (raw image planes)"; return RGBL_E_CUDA; }
+    c->raw_src = c->d_raw_img;
+    *p = {c->d_raw_img, raw_plane_bytes(c), 0, c->in_pitch, true, c->in_w, c->in_h};
     return RGBL_OK;
 }
 
-// n PNG streams into the image planes of the batch being loaded (image_planes); raw planes take 8-bit gray streams only
+// n PNG streams into the image planes of the batch being loaded (image_planes); raw planes take 8-bit gray streams only, since the
+// reference remaps or resizes the image imread returned and converts it to gray afterwards, which differs for colour images
 static int decode_png_gray(Ctx* c, InputKind kind, int n_frames, const uint8_t* const* png, const size_t* png_bytes, int camera_rgb, cudaStream_t st) {
     Planes p;
     int rc = image_planes(c, kind, nullptr, nullptr, &p); if (rc) return rc;
-    const int ch = inflate_png_batch(c, n_frames, png, png_bytes, false, st, p.raw);
+    const char* gray_only = !p.raw ? nullptr
+                          : kind == InputKind::stereo && c->rectify ? "rectified stereo takes 8-bit gray PNGs only (the reference remaps colour images before their conversion to gray)"
+                                                                    : "with the input resize on, image PNGs must be 8-bit gray (the reference resizes colour images before their conversion to gray)";
+    const int ch = inflate_png_batch(c, n_frames, png, png_bytes, p.w, p.h, false, st, gray_only);
     if (ch < 0) return ch;
     LevelGeom g = c->levels[0];
-    g.off = p.off;
-    launch_png_unfilter_gray(st, c->d_png_raw, c->png_raw_stride, c->cfg.width, c->cfg.height, ch, p.raw ? 0 : camera_rgb, p.base, p.stride, g,
+    g.off = p.off; g.pitch = p.pitch;
+    launch_png_unfilter_gray(st, c->d_png_raw, c->png_raw_stride, p.w, p.h, ch, p.raw ? 0 : camera_rgb, p.base, p.stride, g,
                              c->d_png_band, c->d_png_status, n_frames);
     return png_status(c, st);
 }
 
 static size_t depth16_frame_elems(const Ctx* c) { return c->depth16_pitch * c->cfg.height; }
+// the depth planes RGB-D input lands in (d_depth16_raw with the resize on, else d_depth16; a stage slot's planes): pitch and frame size
+static size_t depth16_in_pitch(const Ctx* c) { return c->resize ? c->depth16_raw_pitch : c->depth16_pitch; }
+static size_t depth16_in_frame_elems(const Ctx* c) { return depth16_in_pitch(c) * c->in_h; }
 
 static int ensure_depth16(Ctx* c) {
     c->depth16_pitch = ((size_t)c->cfg.width * sizeof(uint16_t) + 63) / 64 * 32;
     if (!ensure(c->d_depth16, c->depth16_pitch * c->cfg.height * c->cfg.max_batch)) { c->err = "device allocation failed (RGB-D depth planes)"; return RGBL_E_CUDA; }
+    if (c->resize && !ensure(c->d_depth16_raw, depth16_in_frame_elems(c) * c->cfg.max_batch)) { c->err = "device allocation failed (RGB-D input-size depth planes)"; return RGBL_E_CUDA; }
     return RGBL_OK;
 }
 
 // cv::imread(depth PNG, IMREAD_UNCHANGED) of Examples/RGB-D/rgbd_kitti.cc into the uint16 depth planes of frame slots 0..n_frames-1
-// (16-bit gray only); shares the staging buffer with the image decode, one after the other.
-static int decode_png_to_depth16(Ctx* c, int n_frames, const uint8_t* const* png, const size_t* png_bytes, cudaStream_t st) {
+// (16-bit gray only); shares the staging buffer with the image decode, one after the other.  input_size: the streams are camera input,
+// decoded at the input size (into d_depth16_raw, the depth resize's source, while the resize is on); else at the context's size.
+static int decode_png_to_depth16(Ctx* c, int n_frames, const uint8_t* const* png, const size_t* png_bytes, cudaStream_t st, bool input_size) {
     int rc = ensure_depth16(c); if (rc) return rc;
-    const int ch = inflate_png_batch(c, n_frames, png, png_bytes, true, st);
+    const bool rs = input_size && c->resize;
+    const int w = rs ? c->in_w : c->cfg.width, h = rs ? c->in_h : c->cfg.height;
+    const int ch = inflate_png_batch(c, n_frames, png, png_bytes, w, h, true, st);
     if (ch < 0) return ch;
-    launch_png_unfilter_depth16(st, c->d_png_raw, c->png_raw_stride, c->cfg.width, c->cfg.height, c->d_depth16, depth16_frame_elems(c), c->depth16_pitch,
-                                c->d_png_band, c->d_png_status, n_frames);
+    uint16_t* dst = rs ? c->d_depth16_raw.get() : c->d_depth16.get();
+    launch_png_unfilter_depth16(st, c->d_png_raw, c->png_raw_stride, w, h, dst, rs ? depth16_in_frame_elems(c) : depth16_frame_elems(c),
+                                rs ? c->depth16_raw_pitch : c->depth16_pitch, c->d_png_band, c->d_png_status, n_frames);
+    if (rs) c->depth_src = dst;
     return png_status(c, st);
 }
 
-// device buffers of a stage slot (allocated on first use; a slot can hold batches of each kind in turn)
+// device buffers of a stage slot (allocated on first use, grown for a larger input size; a slot can hold batches of each kind in turn)
 static int stage_slot_alloc(Ctx* c, Ctx::StageSlot& sl, InputKind kind) {
     const size_t B = c->cfg.max_batch;
     bool ok = ensure(sl.img, B * raw_plane_bytes(c));         // stereo: the left and the right planes, 2 n_pairs <= max_batch
-    if (ok && kind == InputKind::rgbd) ok = ensure(sl.depth, B * depth16_frame_elems(c));
+    if (ok && kind == InputKind::rgbd) ok = ensure(sl.depth, B * depth16_in_frame_elems(c));
     if (ok && kind == InputKind::rgbl) ok = ensure(sl.pts, B * 4 * c->cfg.max_points) && ensure(sl.n_pts, B);
     if (!ok) { c->err = "device allocation failed (stage slot)"; return RGBL_E_CUDA; }
     return RGBL_OK;
@@ -869,7 +890,6 @@ static int stage_slot_alloc(Ctx* c, Ctx::StageSlot& sl, InputKind kind) {
 // H2D of a checked host batch into stage slot `slot`, or (nullptr) into the working buffers: the image planes (image_planes), d_pts (or
 // d_pts_raw, de-interleaved into d_pts) and d_n_pts, d_depth16.  Clouds and depth images go on the aux stream, images on the main one.
 static int copy_inputs(Ctx* c, const HostInputs& in, int max_pts, Ctx::StageSlot* slot) {
-    const size_t W = c->cfg.width, H = c->cfg.height;
     const bool kitti = in.kind == InputKind::rgbl && in.layout == 1;
     if (in.kind == InputKind::rgbd) { int rc = ensure_depth16(c); if (rc) return rc; }
     if (kitti && !ensure(c->d_pts_raw, (size_t)c->cfg.max_batch * 4 * c->cfg.max_points)) { c->err = "device allocation failed (raw point records)"; return RGBL_E_CUDA; }
@@ -883,10 +903,11 @@ static int copy_inputs(Ctx* c, const HostInputs& in, int max_pts, Ctx::StageSlot
         CU(cudaMemcpyAsync(slot ? slot->n_pts.get() : c->d_n_pts.get(), c->h_n_pts, (size_t)in.n * sizeof(int), cudaMemcpyHostToDevice, c->st_aux));
         if (kitti && max_pts > 0) launch_deinterleave_xyzr(c->st_aux, c->d_pts_raw, c->d_pts, 4 * c->cfg.max_points, c->d_n_pts, max_pts, in.n);
     } else if (in.kind == InputKind::rgbd) {
-        uint16_t* depth = slot ? slot->depth.get() : c->d_depth16.get();
+        uint16_t* depth = slot ? slot->depth.get() : c->resize ? c->d_depth16_raw.get() : c->d_depth16.get();
+        if (!slot && c->resize) c->depth_src = depth;
         for (int f = 0; f < in.n; ++f)
-            CU(cudaMemcpy2DAsync(depth + (size_t)f * depth16_frame_elems(c), c->depth16_pitch * sizeof(uint16_t), in.depth[f], (size_t)in.depth_stride * sizeof(uint16_t),
-                                 W * sizeof(uint16_t), H, cudaMemcpyHostToDevice, c->st_aux));
+            CU(cudaMemcpy2DAsync(depth + (size_t)f * depth16_in_frame_elems(c), depth16_in_pitch(c) * sizeof(uint16_t), in.depth[f],
+                                 (size_t)in.depth_stride * sizeof(uint16_t), (size_t)c->in_w * sizeof(uint16_t), c->in_h, cudaMemcpyHostToDevice, c->st_aux));
     }
     if (!in.gray) return RGBL_OK;          // level 0 was written by a PNG decode
     Planes p;
@@ -920,7 +941,7 @@ static int stage_inputs(Ctx* c, int slot, const HostInputs& in) {
     rc = copy_inputs(c, in, max_pts, &sl); if (rc) return rc;
     CU(cudaStreamSynchronize(c->st));
     CU(cudaStreamSynchronize(c->st_aux));
-    sl.n_frames = in.n; sl.max_pts = max_pts; sl.kind = in.kind;
+    sl.n_frames = in.n; sl.max_pts = max_pts; sl.kind = in.kind; sl.in_w = c->in_w; sl.in_h = c->in_h;
     return RGBL_OK;
 }
 
@@ -936,11 +957,37 @@ static int process_rgbl(Ctx* c, int n_frames, int max_pts, const float P[12], co
     return max_n;
 }
 
+// System::TrackStereo's / TrackRGBD's cv::resize(im, im, newImSize) of the n raw planes (raw_src, in_w x in_h) into level 0 of frame slots
+// [0, n), on the main stream (a level0 step of run_extract) -> its launch count
+static int resize_images(Ctx* c, int n) {
+    LevelGeom src{};
+    src.w = c->in_w; src.h = c->in_h; src.pitch = c->in_pitch;
+    launch_resize_planes(c->st, c->raw_src, raw_plane_bytes(c), src, c->d_pyr, c->frame_bytes, c->levels[0], c->d_resize_coefs,
+                         c->d_resize_coefs + c->cfg.width, n);
+    return 1;
+}
+
 // Everything of the RGB-D Frame constructor (src/Frame.cc:200-237) after the inputs are in HBM: extraction, UndistortKeyPoints (context's
 // camera, rgbl_set_camera_distortion), then ComputeStereoFromRGBD as the gather of the uint16 depth plane, scaled per pixel like
-// GrabImageRGBD's convertTo.
+// GrabImageRGBD's convertTo.  With the input resize on, System::TrackRGBD's two cv::resize run first (src/System.cc, TrackRGBD): the images
+// into level 0 (main stream, billed to the pyramid stage), the depth images into d_depth16 (aux stream, behind the blur and overlapping the
+// quad-tree, billed to the depth_gather stage); the gather waits for both through run_extract's ev_blur.
 static int process_rgbd(Ctx* c, int n_frames, float depth_scale, float bf) {
-    const int max_n = run_extract(c, n_frames);
+    std::function<int()> level0;
+    std::function<void()> depth_resize;
+    if (c->resize) {
+        if (!c->raw_src || !c->depth_src) { c->err = "no input-size planes to resize"; return RGBL_E_INVALID; }
+        level0 = [&]() { return resize_images(c, n_frames); };
+        depth_resize = [&]() {
+            if (c->prof_on) cudaEventRecord(c->ev_rsd_b, c->st_aux);
+            launch_resize_depth16(c->st_aux, c->depth_src, depth16_in_frame_elems(c), c->depth16_raw_pitch, c->resize_kx, c->resize_ky, c->d_depth16,
+                                  depth16_frame_elems(c), c->depth16_pitch, c->cfg.width, c->cfg.height, n_frames);
+            if (c->prof_on) { cudaEventRecord(c->ev_rsd_e, c->st_aux); c->rsd_used = true; }
+            c->total_launches += 1;
+            c->st_pending_launches[ST_DEPTH_GATHER] += 1;
+        };
+    }
+    const int max_n = run_extract(c, n_frames, depth_resize, level0);
     if (max_n < 0) return max_n;
     int launches = max_n > 0 ? 1 : 0;
     stage_begin(c, ST_DEPTH_GATHER, c->st);
@@ -961,24 +1008,28 @@ static int check_rgbd_params(Ctx* c, float depth_scale, float bf) {
 // both extracted as one batch of 2n frames (the reference's two ORBextractor threads), then ComputeStereoMatches.  The left frames are
 // then the batch (last_frames = n) for download, ComputeBoW and the tracking chain.  The capacity-overflow flags cover all 2n frames,
 // so an overflow in a right frame, which changes the left frame's depths, fails the chain's _end2 like a left-frame overflow.
-// With rectification on, the raw planes of the pairs (rect_src) are first remapped into level 0 of the slots, in one launch billed to the
-// pyramid stage: System::TrackStereo's cv::remap of both images (src/System.cc:251 ff.).
+// With rectification on, the raw planes of the pairs (raw_src) are first remapped into level 0 of the slots, in one launch billed to the
+// pyramid stage: System::TrackStereo's cv::remap of both images (src/System.cc:251 ff.).  Else, with the input resize on, they are resized
+// into level 0 in the same way (TrackStereo's cv::resize, the branch after the rectification's).  With both on, the remap alone reads the
+// input-size planes: the maps have the context's size and their coordinates index the input-size images (Settings builds them with
+// initUndistortRectifyMap(..., newImSize_, ...)).
 static int process_stereo(Ctx* c, int n_pairs, float mb, float mbf) {
-    std::function<int()> rectify;
-    if (c->rectify) {
-        if (!c->rect_src) { c->err = "no raw stereo planes to rectify"; return RGBL_E_INVALID; }
-        rectify = [&]() {
+    std::function<int()> level0;
+    if (c->rectify || c->resize) {
+        if (!c->raw_src) { c->err = c->rectify ? "no raw stereo planes to rectify" : "no input-size planes to resize"; return RGBL_E_INVALID; }
+        if (!c->rectify) level0 = [&]() { return resize_images(c, 2 * n_pairs); };
+        else level0 = [&]() {
             const LevelGeom& l0 = c->levels[0];
             RectifyDev r{};
             r.xy = c->d_rect_xy; r.a = c->d_rect_a; r.map_pitch = c->rect_pitch;
-            r.W = c->cfg.width; r.H = c->cfg.height;
-            r.src = c->rect_src; r.src_stride = raw_plane_bytes(c); r.src_pitch = l0.pitch;
+            r.W = c->cfg.width; r.H = c->cfg.height; r.src_W = c->in_w; r.src_H = c->in_h;
+            r.src = c->raw_src; r.src_stride = raw_plane_bytes(c); r.src_pitch = c->in_pitch;
             r.dst = c->d_pyr; r.dst_stride = c->frame_bytes; r.dst_off = l0.off; r.dst_pitch = l0.pitch;
             launch_rectify(c->st, r, n_pairs);
             return 1;
         };
     }
-    const int max_n = run_extract(c, 2 * n_pairs, nullptr, rectify);
+    const int max_n = run_extract(c, 2 * n_pairs, nullptr, level0);
     if (max_n < 0) return max_n;
     int rc = stereo_matches(c, 0, n_pairs, n_pairs, mb, mbf); if (rc) return rc;
     c->last_frames = n_pairs;
@@ -990,6 +1041,21 @@ static int process_stereo(Ctx* c, int n_pairs, float mb, float mbf) {
 static int check_stereo(Ctx* c, int n_pairs) {
     if (2 * n_pairs > c->cfg.max_batch) { c->err = "a stereo batch of n pairs takes 2 n frame slots: 2 n_pairs exceeds max_batch"; return RGBL_E_INVALID; }
     if (c->undistort) { c->err = "stereo needs rectified images: this context's camera has k1 != 0 (rgbl_set_camera_distortion)"; return RGBL_E_UNSUPPORTED; }
+    return RGBL_OK;
+}
+
+// RGB-L input is never resized: the reference's Settings do not handle RGB-L (System::TrackRGBL's resize branch never runs), and the LiDAR
+// projection P describes the original image
+static int check_rgbl_input(Ctx* c) {
+    if (c->resize) { c->err = "RGB-L input is never resized: clear the input resize (rgbl_set_input_resize(ctx, 0, 0))"; return RGBL_E_UNSUPPORTED; }
+    return RGBL_OK;
+}
+
+// RGB-D input with the resize on: the depth resize restates OpenCV's 16-bit INTER_LINEAR at integer factors only
+static int check_rgbd_input(Ctx* c) {
+    if (c->resize && !(c->resize_kx && c->resize_ky)) {
+        c->err = "RGB-D input resize needs integer factors (input width / width and input height / height)"; return RGBL_E_UNSUPPORTED;
+    }
     return RGBL_OK;
 }
 
@@ -1041,7 +1107,8 @@ int rgbl_frame_rgbl_batch(rgbl_ctx* ctx, int n_frames, const uint8_t* const* gra
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
     if (!gray || !pts4xn || !n_pts || !P || !prm || !kps || !desc || !depth || !uright || !n_out) { c->err = "null argument"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
+    int rc = check_rgbl_input(c); if (rc) return rc;
+    rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     rc = upload_inputs(c, HostInputs::rgbl(n_frames, gray, stride, pts4xn, n_pts)); if (rc) return rc;
     rc = process_rgbl(c, n_frames, c->resident_max_pts, P, prm); if (rc < 0) return rc;
@@ -1055,7 +1122,8 @@ int rgbl_resident_upload(rgbl_ctx* ctx, int n_frames, const uint8_t* const* gray
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
     if (!gray || !pts4xn || !n_pts) { c->err = "null argument"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
+    int rc = check_rgbl_input(c); if (rc) return rc;
+    rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     return upload_inputs_sync(c, HostInputs::rgbl(n_frames, gray, stride, pts4xn, n_pts));
 }
@@ -1065,7 +1133,8 @@ int rgbl_resident_upload_kitti(rgbl_ctx* ctx, int n_frames, const uint8_t* const
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
     if (!gray || !xyzr || !n_pts) { c->err = "null argument"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
+    int rc = check_rgbl_input(c); if (rc) return rc;
+    rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     return upload_inputs_sync(c, HostInputs::rgbl(n_frames, gray, stride, xyzr, n_pts, 1));
 }
@@ -1075,7 +1144,8 @@ int rgbl_resident_upload_kitti_png(rgbl_ctx* ctx, int n_frames, const uint8_t* c
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
     if (!png || !png_bytes || !xyzr || !n_pts) { c->err = "null argument"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_frames, c->cfg.width, c->cfg.height, c->cfg.width); if (rc) return rc;
+    int rc = check_rgbl_input(c); if (rc) return rc;
+    rc = check_batch_args(c, n_frames, c->cfg.width, c->cfg.height, c->cfg.width); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     rc = decode_png_gray(c, InputKind::rgbl, n_frames, png, png_bytes, camera_rgb, c->st); if (rc) return rc;
     return upload_inputs_sync(c, HostInputs::rgbl(n_frames, nullptr, 0, xyzr, n_pts, 1));
@@ -1086,7 +1156,7 @@ int rgbl_decode_png_gray(rgbl_ctx* ctx, int n_frames, const uint8_t* const* png,
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
     if (!png || !png_bytes || !gray_out) { c->err = "null argument"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_frames, c->cfg.width, c->cfg.height, stride); if (rc) return rc;
+    int rc = check_batch_args(c, n_frames, c->cfg.width, c->cfg.height, stride, false); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     rc = decode_png_gray(c, InputKind::rgbl, n_frames, png, png_bytes, camera_rgb, c->st); if (rc) return rc;
     const Planes l0 = level0_planes(c);
@@ -1102,7 +1172,8 @@ int rgbl_resident_process(rgbl_ctx* ctx, const float P[12], const rgbl_depth_par
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
     if (!P || !prm) { c->err = "null argument"; return RGBL_E_INVALID; }
-    int rc = check_resident_kind(c, InputKind::rgbl); if (rc) return rc;
+    int rc = check_rgbl_input(c); if (rc) return rc;
+    rc = check_resident_kind(c, InputKind::rgbl); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     rc = process_rgbl(c, c->resident_frames, c->resident_max_pts, P, prm); if (rc < 0) return rc;
     return finish_process(c, n_out);
@@ -1121,7 +1192,8 @@ int rgbl_resident_stage(rgbl_ctx* ctx, int slot, int n_frames, const uint8_t* co
     if (!gray || !pts4xn || !n_pts) { c->err = "null argument"; return RGBL_E_INVALID; }
     if (slot < 0 || slot >= Ctx::kMaxStageSlots) { c->err = "stage slot out of range"; return RGBL_E_INVALID; }
     if (!c->d_pts) { c->err = "context was created with max_points == 0"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
+    int rc = check_rgbl_input(c); if (rc) return rc;
+    rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     return stage_inputs(c, slot, HostInputs::rgbl(n_frames, gray, stride, pts4xn, n_pts));
 }
@@ -1132,7 +1204,8 @@ int rgbl_resident_stage_rgbd(rgbl_ctx* ctx, int slot, int n_frames, const uint8_
     if (!c) return RGBL_E_INVALID;
     if (!gray || !depth) { c->err = "null argument"; return RGBL_E_INVALID; }
     if (slot < 0 || slot >= Ctx::kMaxStageSlots) { c->err = "stage slot out of range"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
+    int rc = check_rgbd_input(c); if (rc) return rc;
+    rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
     if (depth_stride < width) { c->err = "depth_stride < width"; return RGBL_E_INVALID; }
     CU(cudaSetDevice(c->cfg.device));
     return stage_inputs(c, slot, HostInputs::rgbd(n_frames, gray, stride, depth, depth_stride));
@@ -1160,13 +1233,16 @@ static int restage(Ctx* c, int slot, InputKind kind) {
         c->err = std::string("stage slot holds ") + k.what + " (" + k.runner + ")";
         return RGBL_E_INVALID;
     }
+    if (sl.in_w != c->in_w || sl.in_h != c->in_h) { c->err = "stage slot was staged at another input size (rgbl_set_input_resize)"; return RGBL_E_INVALID; }
     Planes dst;
     int rc = image_planes(c, kind, nullptr, &sl, &dst); if (rc) return rc;
     const size_t img_bytes = raw_plane_bytes(c);
     const int n_img = kind == InputKind::stereo ? 2 * sl.n_frames : sl.n_frames;
     if (dst.base)
         for (int f = 0; f < n_img; ++f) CU(cudaMemcpyAsync(dst.at(f), sl.img + (size_t)f * img_bytes, img_bytes, cudaMemcpyDeviceToDevice, c->st));
-    if (kind == InputKind::rgbd) {
+    if (kind == InputKind::rgbd && c->resize) {
+        c->depth_src = sl.depth;          // read in place by the depth resize
+    } else if (kind == InputKind::rgbd) {
         CU(cudaMemcpyAsync(c->d_depth16, sl.depth, (size_t)sl.n_frames * depth16_frame_elems(c) * sizeof(uint16_t), cudaMemcpyDeviceToDevice, c->st_aux));
     } else if (kind == InputKind::rgbl) {
         CU(cudaMemcpyAsync(c->d_pts, sl.pts, (size_t)sl.n_frames * 4 * c->cfg.max_points * sizeof(float), cudaMemcpyDeviceToDevice, c->st_aux));
@@ -1245,7 +1321,8 @@ int rgbl_track_sequence(rgbl_ctx* ctx, const float P[12], const rgbl_depth_param
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
     if (!P || !prm) { c->err = "null argument"; return RGBL_E_INVALID; }
-    int rc = check_sequence_io(c, chain, io); if (rc) return rc;
+    int rc = check_rgbl_input(c); if (rc) return rc;
+    rc = check_sequence_io(c, chain, io); if (rc) return rc;
     if (io->gray && (!io->pts4xn || !io->n_pts)) { c->err = "null argument"; return RGBL_E_INVALID; }
     CU(cudaSetDevice(c->cfg.device));
     const int T = io->frames_per_batch;
@@ -1259,6 +1336,7 @@ int rgbl_track_sequence_rgbd(rgbl_ctx* ctx, float depth_scale, float bf, const r
     if (!c) return RGBL_E_INVALID;
     int rc = check_sequence_io(c, chain, io); if (rc) return rc;
     rc = check_rgbd_params(c, depth_scale, bf); if (rc) return rc;
+    rc = check_rgbd_input(c); if (rc) return rc;
     if (io->pts4xn || io->n_pts) { c->err = "RGB-D sequences take depth images, not point clouds (pts4xn / n_pts must be NULL)"; return RGBL_E_INVALID; }
     if (io->gray && (!depth || depth_stride < io->width)) { c->err = "host mode needs one depth image per frame and depth_stride >= width"; return RGBL_E_INVALID; }
     CU(cudaSetDevice(c->cfg.device));
@@ -1287,7 +1365,8 @@ int rgbl_resident_upload_rgbd(rgbl_ctx* ctx, int n_frames, const uint8_t* const*
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
     if (!gray || !depth) { c->err = "null argument"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
+    int rc = check_rgbd_input(c); if (rc) return rc;
+    rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     return upload_inputs_sync(c, HostInputs::rgbd(n_frames, gray, stride, depth, depth_stride));
 }
@@ -1297,10 +1376,11 @@ int rgbl_resident_upload_rgbd_png(rgbl_ctx* ctx, int n_frames, const uint8_t* co
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
     if (!png || !png_bytes || !depth_png || !depth_png_bytes) { c->err = "null argument"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_frames, c->cfg.width, c->cfg.height, c->cfg.width); if (rc) return rc;
+    int rc = check_rgbd_input(c); if (rc) return rc;
+    rc = check_batch_args(c, n_frames, c->in_w, c->in_h, c->in_w); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     rc = decode_png_gray(c, InputKind::rgbd, n_frames, png, png_bytes, camera_rgb, c->st); if (rc) return rc;
-    rc = decode_png_to_depth16(c, n_frames, depth_png, depth_png_bytes, c->st); if (rc) return rc;
+    rc = decode_png_to_depth16(c, n_frames, depth_png, depth_png_bytes, c->st, true); if (rc) return rc;
     set_resident(c, InputKind::rgbd, n_frames, 0);
     return RGBL_OK;
 }
@@ -1309,10 +1389,10 @@ int rgbl_decode_png_depth16(rgbl_ctx* ctx, int n_frames, const uint8_t* const* p
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
     if (!png || !png_bytes || !depth_out) { c->err = "null argument"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_frames, c->cfg.width, c->cfg.height, stride); if (rc) return rc;
+    int rc = check_batch_args(c, n_frames, c->cfg.width, c->cfg.height, stride, false); if (rc) return rc;
     for (int f = 0; f < n_frames; ++f) if (!depth_out[f]) { c->err = "null output image"; return RGBL_E_INVALID; }
     CU(cudaSetDevice(c->cfg.device));
-    rc = decode_png_to_depth16(c, n_frames, png, png_bytes, c->st); if (rc) return rc;
+    rc = decode_png_to_depth16(c, n_frames, png, png_bytes, c->st, false); if (rc) return rc;
     for (int f = 0; f < n_frames; ++f)
         CU(cudaMemcpy2DAsync(depth_out[f], (size_t)stride * sizeof(uint16_t), c->d_depth16 + (size_t)f * depth16_frame_elems(c), c->depth16_pitch * sizeof(uint16_t),
                              (size_t)c->cfg.width * sizeof(uint16_t), c->cfg.height, cudaMemcpyDeviceToHost, c->st));
@@ -1346,10 +1426,10 @@ int rgbl_resident_upload_stereo_png(rgbl_ctx* ctx, int n_pairs, const uint8_t* c
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
     if (!left_png || !left_bytes || !right_png || !right_bytes) { c->err = "null argument"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_pairs, c->cfg.width, c->cfg.height, c->cfg.width); if (rc) return rc;
+    int rc = check_batch_args(c, n_pairs, c->in_w, c->in_h, c->in_w); if (rc) return rc;
     rc = check_stereo(c, n_pairs); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
-    // one decode of 2n streams: every stream must have the context's size, so left and right sizes that differ are an error
+    // one decode of 2n streams: every stream must have the input size, so left and right sizes that differ are an error
     std::vector<const uint8_t*> png(left_png, left_png + n_pairs);
     std::vector<size_t> bytes(left_bytes, left_bytes + n_pairs);
     png.insert(png.end(), right_png, right_png + n_pairs);
@@ -1404,6 +1484,42 @@ int rgbl_set_stereo_rectification(rgbl_ctx* ctx, const float* m1l, const float* 
     CU(cudaStreamSynchronize(c->st));
     c->rectify = true;
     if (c->resident_kind == InputKind::stereo) c->resident_frames = 0;
+    return RGBL_OK;
+}
+
+// Settings::needToResize(): camera images of src_width x src_height resized to the context's size before frame construction (System::TrackRGBD,
+// System::TrackStereo).  Every check runs before anything is changed, so a refused setting leaves the previous one in place.
+int rgbl_set_input_resize(rgbl_ctx* ctx, int src_width, int src_height) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return RGBL_E_INVALID;
+    if (c->chain_pending) { c->err = "a tracking chain is in flight (rgbl_resident_track_end not called)"; return RGBL_E_INVALID; }
+    if (src_width < 0 || src_height < 0 || (src_width == 0) != (src_height == 0)) {
+        c->err = "the input size is (0, 0) (no resize) or two positive sizes"; return RGBL_E_INVALID;
+    }
+    const int W = c->cfg.width, H = c->cfg.height;
+    const bool on = src_width != 0 && (src_width != W || src_height != H);
+    if (on && (src_width < W || src_height < H)) {
+        c->err = "the input resize only downscales (input size >= the context's size in both axes)"; return RGBL_E_UNSUPPORTED;
+    }
+    if (on && (src_width > 32767 || src_height > 32767)) { c->err = "input sizes above 32767 px are not supported"; return RGBL_E_UNSUPPORTED; }
+    if (on) {
+        CU(cudaSetDevice(c->cfg.device));
+        std::vector<LinCoef> tab((size_t)W + H);
+        linear_coefs(src_width, W, tab.data());
+        linear_coefs(src_height, H, tab.data() + W);
+        if (!ensure(c->d_resize_coefs, tab.size())) { c->err = "device allocation failed (input resize tables)"; return RGBL_E_CUDA; }
+        if (!c->ev_rsd_b) CU(c->ev_rsd_b.create());
+        if (!c->ev_rsd_e) CU(c->ev_rsd_e.create());
+        CU(cudaStreamSynchronize(c->st));         // a batch in flight may still read the previous tables
+        CU(cudaMemcpy(c->d_resize_coefs, tab.data(), tab.size() * sizeof(LinCoef), cudaMemcpyHostToDevice));
+    }
+    c->resize = on;
+    c->in_w = on ? src_width : W; c->in_h = on ? src_height : H;
+    c->in_pitch = (c->in_w + 63) & ~63;
+    c->resize_kx = c->in_w % W == 0 ? c->in_w / W : 0;
+    c->resize_ky = c->in_h % H == 0 ? c->in_h / H : 0;
+    c->depth16_raw_pitch = ((size_t)c->in_w * sizeof(uint16_t) + 63) / 64 * 32;
+    c->resident_frames = 0;                   // the uploaded batch was loaded for the other setting
     return RGBL_OK;
 }
 

@@ -9,6 +9,7 @@
 //   resolve+dilate : depth_dilate_v2.cu.
 //   gather   : GetFeatureDepthFromDepthMap (:82-104), and Frame::ComputeStereoFromRGBD (src/Frame.cc:1074-1095) on a uint16 RGB-D plane.
 //   undistort: Frame::UndistortKeyPoints (src/Frame.cc:837-869), mvKeys -> mvKeysUn of a distorted camera, before the gather.
+//   resize   : System::TrackRGBD's cv::resize of the CV_16U depth image to Settings' new image size (integer factors), before the gather.
 #include "rgbl_device.cuh"
 #include "rgbl_kernels.h"
 
@@ -190,6 +191,35 @@ __global__ void __launch_bounds__(256) depth_nn_pixel_kernel(const float* __rest
         }
     }
     if (lane == 0) { depth[o] = dd; uright[o] = ur; }
+}
+
+// System::TrackRGBD's cv::resize(imDepth, imDepth, newImSize) of a CV_16U depth image (INTER_LINEAR, before GrabImageRGBD's convertTo) at an
+// integer factor per axis.  OpenCV's 16U linear resize runs in float32: per axis the source index s = floor((d + 0.5) k - 0.5) and the
+// weights 1 - f, f, horizontal pass then vertical pass, each a sum of two products, then saturate_cast<ushort> (round half to even).  At an
+// integer factor k, (d + 0.5) k - 0.5 = d k + (k - 1) / 2: f = 1/2 for even k and 0 for odd k, s + 1 stays inside the image and every product
+// is exact.  One thread per output sample; blockIdx.z = frame.
+__global__ void __launch_bounds__(256) resize_depth16_kernel(const uint16_t* __restrict__ src, size_t src_frame_elems, size_t src_pitch, int kx,
+                                                             int ky, uint16_t* __restrict__ dst, size_t dst_frame_elems, size_t dst_pitch, int W,
+                                                             int H) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x >= W || y >= H) return;
+    const float ax = (kx & 1) ? 0.f : 0.5f, ay = (ky & 1) ? 0.f : 0.5f;
+    const int sx = x * kx + (kx - 1) / 2, sy = y * ky + (ky - 1) / 2;
+    const int sx1 = sx + (ax != 0.f), sy1 = sy + (ay != 0.f);
+    const uint16_t* s = src + (size_t)blockIdx.z * src_frame_elems;
+    auto hpass = [&](int row) {
+        const uint16_t* r = s + (size_t)row * src_pitch;
+        return __fadd_rn(__fmul_rn((float)__ldg(r + sx), 1.f - ax), __fmul_rn((float)__ldg(r + sx1), ax));
+    };
+    const float v = __fadd_rn(__fmul_rn(hpass(sy), 1.f - ay), __fmul_rn(hpass(sy1), ay));
+    dst[(size_t)blockIdx.z * dst_frame_elems + (size_t)y * dst_pitch + x] = (uint16_t)__float2int_rn(v);     // 0 <= v <= 65535: no saturation
+}
+
+void launch_resize_depth16(cudaStream_t st, const uint16_t* src, size_t src_frame_elems, size_t src_pitch, int kx, int ky, uint16_t* dst,
+                           size_t dst_frame_elems, size_t dst_pitch, int dst_w, int dst_h, int n_frames) {
+    if (n_frames < 1) return;
+    resize_depth16_kernel<<<dim3((dst_w + 31) / 32, (dst_h + 7) / 8, n_frames), dim3(32, 8), 0, st>>>(src, src_frame_elems, src_pitch, kx, ky, dst,
+                                                                                                     dst_frame_elems, dst_pitch, dst_w, dst_h);
 }
 
 void launch_depth_average_filter(cudaStream_t st, const float* raw, int W, int H, int k, float* processed, int n_frames) {

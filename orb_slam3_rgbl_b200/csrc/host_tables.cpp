@@ -49,7 +49,7 @@ int compute_orb_tables(const rgbl_orb_params& p, OrbTables& t) {
     return RGBL_OK;
 }
 
-static void linear_coefs(int src_n, int dst_n, LinCoef* out) {
+void linear_coefs(int src_n, int dst_n, LinCoef* out) {
     const double scale = (double)src_n / (double)dst_n;
     for (int d = 0; d < dst_n; ++d) {
         float f = (float)((d + 0.5) * scale - 0.5);
@@ -180,7 +180,7 @@ int structuring_element(const char* kind, int ku, int kv, uint8_t* mask) {
 
 extern "C" {
 
-int rgbl_abi_version(void) { return 1; }
+int rgbl_abi_version(void) { return 2; }
 
 int rgbl_orb_tables(const rgbl_orb_params* p, float* scale, float* inv_scale, float* sigma2, float* inv_sigma2,
                     int32_t* features_per_level, int32_t* umax16) {

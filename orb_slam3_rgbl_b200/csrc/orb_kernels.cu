@@ -16,16 +16,18 @@ namespace rgbl {
 // memory with 16-byte loads (rows are 64-byte aligned); every thread then produces 4 adjacent outputs in two rows from
 // shared-memory bytes.  (The first version gathered 16 single bytes per thread straight from global memory and was bound by
 // the number of load instructions, not by HBM.)
+// Both kernels read plane z at src_base + z * src_stride + src.off and write plane z at dst_base + z * dst_stride + dst.off: the pyramid
+// passes its frame slots twice (level l-1 -> level l), the input resize the source-size raw planes and level 0 (launch_resize_planes).
 constexpr int kRzTW = 128, kRzTH = 16, kRzSrcRows = 24, kRzSrcVec = 12;     // staged source: 24 rows x 192 bytes max
-__global__ void __launch_bounds__(256) resize_level_kernel(uint8_t* __restrict__ pyr, size_t frame_stride,
-                                                           LevelGeom src, LevelGeom dst,
+__global__ void __launch_bounds__(256) resize_level_kernel(const uint8_t* __restrict__ src_base, size_t src_stride, LevelGeom src,
+                                                           uint8_t* __restrict__ dst_base, size_t dst_stride, LevelGeom dst,
                                                            const LinCoef* __restrict__ tabx,
                                                            const LinCoef* __restrict__ taby) {
     __shared__ uint4 tile[kRzSrcRows][kRzSrcVec];
     const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
     const int x0 = blockIdx.x * kRzTW, y0 = blockIdx.y * kRzTH;
-    const uint8_t* s = pyr + (size_t)blockIdx.z * frame_stride + src.off;
-    uint8_t* d = pyr + (size_t)blockIdx.z * frame_stride + dst.off;
+    const uint8_t* s = src_base + (size_t)blockIdx.z * src_stride + src.off;
+    uint8_t* d = dst_base + (size_t)blockIdx.z * dst_stride + dst.off;
     // source rectangle of this tile (tables are monotone)
     const int xl = min(x0 + kRzTW - 1, dst.w - 1), yl = min(y0 + kRzTH - 1, dst.h - 1);
     const int sx_lo = tabx[x0].s & ~15, sx_hi = min(tabx[xl].s + 1, src.w - 1);
@@ -71,15 +73,15 @@ __global__ void __launch_bounds__(256) resize_level_kernel(uint8_t* __restrict__
 
 // Fallback for level ratios whose source rectangle does not fit the staged tile (scale factors above ~1.35): one thread
 // gathers the 16 source bytes of 4 adjacent outputs directly from global memory.
-__global__ void __launch_bounds__(256) resize_level_gather_kernel(uint8_t* __restrict__ pyr, size_t frame_stride,
-                                                                  LevelGeom src, LevelGeom dst,
+__global__ void __launch_bounds__(256) resize_level_gather_kernel(const uint8_t* __restrict__ src_base, size_t src_stride, LevelGeom src,
+                                                                  uint8_t* __restrict__ dst_base, size_t dst_stride, LevelGeom dst,
                                                                   const LinCoef* __restrict__ tabx,
                                                                   const LinCoef* __restrict__ taby) {
     const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
     const int y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x4 >= dst.w || y >= dst.h) return;
-    const uint8_t* s = pyr + (size_t)blockIdx.z * frame_stride + src.off;
-    uint8_t* d = pyr + (size_t)blockIdx.z * frame_stride + dst.off;
+    const uint8_t* s = src_base + (size_t)blockIdx.z * src_stride + src.off;
+    uint8_t* d = dst_base + (size_t)blockIdx.z * dst_stride + dst.off;
     const LinCoef cy = taby[y];
     const uint8_t* r0 = s + (size_t)cy.s * src.pitch;
     const uint8_t* r1 = s + (size_t)min(cy.s + 1, src.h - 1) * src.pitch;
@@ -267,19 +269,24 @@ __global__ void padded_level_kernel(const uint8_t* __restrict__ pyr, size_t fram
 // ------------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------------
+void launch_resize_planes(cudaStream_t st, const uint8_t* src_base, size_t src_stride, const LevelGeom& src, uint8_t* dst_base, size_t dst_stride,
+                          const LevelGeom& dst, const LinCoef* tabx, const LinCoef* taby, int n_planes) {
+    if (n_planes < 1) return;
+    const double rx = (double)src.w / dst.w, ry = (double)src.h / dst.h;
+    if (rx * (kRzTW - 1) + 18.0 <= kRzSrcVec * 16 - 1 && ry * (kRzTH - 1) + 3.0 <= kRzSrcRows) {
+        dim3 grd((dst.w + kRzTW - 1) / kRzTW, (dst.h + kRzTH - 1) / kRzTH, n_planes);
+        resize_level_kernel<<<grd, 256, 0, st>>>(src_base, src_stride, src, dst_base, dst_stride, dst, tabx, taby);
+    } else {
+        dim3 blk(32, 8), grd(((dst.w + 3) / 4 + 31) / 32, (dst.h + 7) / 8, n_planes);
+        resize_level_gather_kernel<<<grd, blk, 0, st>>>(src_base, src_stride, src, dst_base, dst_stride, dst, tabx, taby);
+    }
+}
+
 void launch_pyramid(cudaStream_t st, uint8_t* pyr, size_t frame_stride, const LevelGeom* h_levels, int n_levels,
                     const LinCoef* d_coefs, int n_frames) {
     for (int l = 1; l < n_levels; ++l) {
-        const LevelGeom& src = h_levels[l - 1];
         const LevelGeom& dst = h_levels[l];
-        const double rx = (double)src.w / dst.w, ry = (double)src.h / dst.h;
-        if (rx * (kRzTW - 1) + 18.0 <= kRzSrcVec * 16 - 1 && ry * (kRzTH - 1) + 3.0 <= kRzSrcRows) {
-            dim3 grd((dst.w + kRzTW - 1) / kRzTW, (dst.h + kRzTH - 1) / kRzTH, n_frames);
-            resize_level_kernel<<<grd, 256, 0, st>>>(pyr, frame_stride, src, dst, d_coefs + dst.tabx_off, d_coefs + dst.taby_off);
-        } else {
-            dim3 blk(32, 8), grd(((dst.w + 3) / 4 + 31) / 32, (dst.h + 7) / 8, n_frames);
-            resize_level_gather_kernel<<<grd, blk, 0, st>>>(pyr, frame_stride, src, dst, d_coefs + dst.tabx_off, d_coefs + dst.taby_off);
-        }
+        launch_resize_planes(st, pyr, frame_stride, h_levels[l - 1], pyr, frame_stride, dst, d_coefs + dst.tabx_off, d_coefs + dst.taby_off, n_frames);
     }
 }
 

@@ -94,15 +94,27 @@ struct Ctx {
     DeviceArray<int> d_stereo_row_start, d_stereo_row_idx, d_stereo_sad;
     int stereo_idx_cap = 0;
     // stereo rectification (rgbl_set_stereo_rectification, stereo_kernels.cu).  d_rect_xy / d_rect_a: OpenCV's fixed-point form of the
-    // left and right maps, H rows of rect_pitch entries per camera, allocated by the first setting and never reallocated.  d_rect_raw:
-    // max_batch raw planes in level 0's layout (row pitch levels[0].pitch), allocated by the first stereo upload with rectification on;
-    // host uploads and PNG decodes of pairs write there instead of level 0.  rect_src: the raw planes of the uploaded pairs (d_rect_raw,
-    // or a staged slot's planes).  No chain graph references these buffers, so they need no scratch_generation bump.
+    // left and right maps, H rows of rect_pitch entries per camera, allocated by the first setting and never reallocated.
     bool rectify = false;
     DeviceArray<uint32_t> d_rect_xy; DeviceArray<uint16_t> d_rect_a;
     int rect_pitch = 0;
-    DeviceArray<uint8_t> d_rect_raw;
-    const uint8_t* rect_src = nullptr;
+    // input resize (rgbl_set_input_resize): RGB-D and stereo images (and RGB-D depth images) arrive at in_w x in_h, Settings' original
+    // camera size, and are resized to the context's size before the extraction.  in_w / in_h / in_pitch are the context's width, height
+    // and level 0's pitch while the resize is off.  d_resize_coefs: the cv::resize tables of the two axes (x: W entries, then y: H entries).
+    // resize_kx / resize_ky: the integer factors of the depth resize (0: not an integer, refused for RGB-D).
+    bool resize = false;
+    int in_w = 0, in_h = 0, in_pitch = 0, resize_kx = 0, resize_ky = 0;
+    DeviceArray<LinCoef> d_resize_coefs;
+    // Raw image planes: the images of the uploaded batch before the conditioning kernel (rectification or resize) writes level 0 of the frame
+    // slots.  d_raw_img: max_batch planes of in_pitch x in_h bytes, allocated by the first upload that needs them (and reallocated when the
+    // input size grows); host uploads and PNG decodes write there instead of level 0.  raw_src: the raw planes of the uploaded batch
+    // (d_raw_img, or a staged slot's planes).  d_depth16_raw / depth_src: the same for RGB-D depth images with the resize on (row pitch
+    // depth16_raw_pitch elements).  No chain graph references these buffers, so they need no scratch_generation bump.
+    DeviceArray<uint8_t> d_raw_img;
+    const uint8_t* raw_src = nullptr;
+    DeviceArray<uint16_t> d_depth16_raw;
+    size_t depth16_raw_pitch = 0;
+    const uint16_t* depth_src = nullptr;
     DeviceArray<int> d_n_pts;
     DeviceArray<uint32_t> d_idx_map;
     DeviceArray<float> d_raw, d_processed, d_depth, d_uright;
@@ -119,6 +131,7 @@ struct Ctx {
     bool prof_on = false, prof_serial = false;   // prof_serial: stage timings without stream overlap (the aux-stream work is joined before the quad-tree)
     Event ev_b[kNumStages], ev_e[kNumStages];
     bool st_used[kNumStages] = {};
+    Event ev_rsd_b, ev_rsd_e; bool rsd_used = false;   // the depth resize on the aux stream, billed to depth_gather besides the gather itself
     int st_pending_launches[kNumStages] = {};
     double st_ms[kNumStages] = {};
     long st_launches[kNumStages] = {};
@@ -179,7 +192,11 @@ struct Ctx {
     // rgbl_track_sequence_rgbd, rgbl_resident_stage_stereo / rgbl_track_sequence_stereo): level-0 planes + clouds (RGB-L), uint16 depth
     // planes (RGB-D) or the left then the right level-0 planes (stereo: n_frames pairs, 2 n_frames planes) of whole batches
     static constexpr int kMaxStageSlots = 8;
-    struct StageSlot { DeviceArray<uint8_t> img; DeviceArray<float> pts; DeviceArray<int> n_pts; DeviceArray<uint16_t> depth; int n_frames = 0, max_pts = 0; InputKind kind = InputKind::rgbl; };
+    // (in_w x in_h: the input size the slot was staged at)
+    struct StageSlot {
+        DeviceArray<uint8_t> img; DeviceArray<float> pts; DeviceArray<int> n_pts; DeviceArray<uint16_t> depth;
+        int n_frames = 0, max_pts = 0, in_w = 0, in_h = 0; InputKind kind = InputKind::rgbl;
+    };
     StageSlot stage[kMaxStageSlots];
 
     // camera model of Frame::UndistortKeyPoints / ComputeImageBounds (rgbl_set_camera_distortion): undistort = (k1 != 0); cam_bounds =

@@ -74,6 +74,8 @@ struct OrbTables {
 int compute_orb_tables(const rgbl_orb_params& p, OrbTables& t);
 int build_geometry(int width, int height, const OrbTables& t, std::vector<LevelGeom>& levels,
                    std::vector<CellInfo>& cells, std::vector<LinCoef>& coefs, size_t& frame_bytes, std::string& err);
+// cv::resize INTER_LINEAR coefficients of one axis, src_n -> dst_n samples (SURVEY A.1): the pyramid's level tables and the input resize's
+void linear_coefs(int src_n, int dst_n, LinCoef* out);
 // cells -> strips of at most max_cells cells and max_width px; returns the largest window height and tested-pixel count
 void build_fast_strips(const std::vector<CellInfo>& cells, int max_cells, int max_width, std::vector<StripInfo>& strips, int& rows_max,
                        int& tested_max);

@@ -20,6 +20,10 @@ struct __align__(8) SelKp {
 // orb_kernels.cu
 void launch_pyramid(cudaStream_t st, uint8_t* pyr, size_t frame_stride, const LevelGeom* h_levels, int n_levels,
                     const LinCoef* d_coefs, int n_frames);
+// cv::resize(INTER_LINEAR) of n_planes 8-bit planes, src.w x src.h -> dst.w x dst.h with the tables tabx / taby (linear_coefs): plane z at
+// src_base + z * src_stride + src.off -> dst_base + z * dst_stride + dst.off; both rows 64-byte aligned (pitch % 64 == 0, 16-byte aligned bases)
+void launch_resize_planes(cudaStream_t st, const uint8_t* src_base, size_t src_stride, const LevelGeom& src, uint8_t* dst_base, size_t dst_stride,
+                          const LevelGeom& dst, const LinCoef* tabx, const LinCoef* taby, int n_planes);
 // fast_strip_kernels.cu: per-cell FAST with the iniTh -> minTh fallback, one CTA per strip of cells (fast_strip.cuh); survivors in
 // each cell's slot array; returns -1 when the shared-memory request is refused
 int launch_fast_strips(cudaStream_t st, const uint8_t* pyr, size_t frame_stride, const LevelGeom* d_levels, const CellInfo* d_cells,
@@ -90,6 +94,11 @@ void launch_undistort_keypoints(cudaStream_t st, const UndistortDev& cam, const 
 // the same gather on uint16 RGB-D depth planes, metric depth = (float)sample * scale (Tracking::mDepthMapFactor)
 void launch_depth_gather_u16(cudaStream_t st, const uint16_t* plane, size_t frame_elems, size_t pitch_elems, float scale, const rgbl_keypoint* kps,
                              const rgbl_keypoint* kps_un, const int* n_kp, int cap, int max_n, float bf, float* depth, float* uright, int n_frames);
+// cv::resize(INTER_LINEAR) of n_frames CV_16U depth planes by integer factors kx = src_w / dst_w, ky = src_h / dst_h (OpenCV's float path:
+// weights 1 - f, f with f in {0, 1/2}, horizontal then vertical in float32, rounded half to even): src plane f at src + f * src_frame_elems with
+// row pitch src_pitch elements -> dst + f * dst_frame_elems, row pitch dst_pitch elements
+void launch_resize_depth16(cudaStream_t st, const uint16_t* src, size_t src_frame_elems, size_t src_pitch, int kx, int ky, uint16_t* dst,
+                           size_t dst_frame_elems, size_t dst_pitch, int dst_w, int dst_h, int n_frames);
 
 
 // match_kernels.cu ---------------------------------------------------------------------------------
@@ -216,7 +225,8 @@ void launch_stereo_matches(cudaStream_t st, const StereoBatchDev& s, int n_pairs
 void launch_rectify_maps(cudaStream_t st, const float* maps, int W, int H, uint32_t* xy, uint16_t* a, int pitch);
 struct RectifyDev {
     const uint32_t* xy; const uint16_t* a; int map_pitch;
-    int W, H;
+    int W, H;                                                        // output (and map) size: the context's
+    int src_W, src_H;                                                // raw plane size: the input resize's source size (0, 0: W x H)
     const uint8_t* src; size_t src_stride; int src_pitch;            // raw plane of slot s at src + s * src_stride
     uint8_t* dst; size_t dst_stride; int dst_off, dst_pitch;         // rectified plane of slot s at dst + s * dst_stride + dst_off (4-byte aligned rows)
 };

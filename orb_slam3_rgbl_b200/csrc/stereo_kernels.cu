@@ -274,7 +274,7 @@ __global__ void __launch_bounds__(128) rectify_kernel(RectifyDev r, int n) {
 #pragma unroll
         for (int t = 0; t < 4; ++t) {
             const int tx = sx + (t & 1), ty = sy + (t >> 1);
-            const bool in = tx >= 0 && tx < r.W && ty >= 0 && ty < r.H;
+            const bool in = tx >= 0 && tx < r.src_W && ty >= 0 && ty < r.src_H;
             off[p][t] = in ? ty * r.src_pitch + tx : 0;
             w[p][t] = in ? wt[t] : 0;
         }
@@ -305,8 +305,10 @@ void launch_rectify_maps(cudaStream_t st, const float* maps, int W, int H, uint3
 
 void launch_rectify(cudaStream_t st, const RectifyDev& r, int n_pairs) {
     if (n_pairs < 1) return;
-    const int groups = (r.W + kGroup - 1) / kGroup;
-    rectify_kernel<<<dim3((groups + 127) / 128, r.H, 2), 128, 0, st>>>(r, n_pairs);
+    RectifyDev k = r;
+    if (!k.src_W) { k.src_W = k.W; k.src_H = k.H; }
+    const int groups = (k.W + kGroup - 1) / kGroup;
+    rectify_kernel<<<dim3((groups + 127) / 128, k.H, 2), 128, 0, st>>>(k, n_pairs);
 }
 
 }  // namespace rgbl

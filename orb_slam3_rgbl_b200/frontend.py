@@ -72,6 +72,12 @@ class Context:
         stride = self.width
         check(lib().rgbl_set_stereo_rectification(self.handle, *[None if a is None else ptr(a) for a in arr], stride), self.handle)
 
+    def set_input_resize(self, src_width: int = 0, src_height: int = 0):
+        """Resize every later RGB-D and stereo input on the device (rgbl_set_input_resize, Settings::needToResize): the uploads, stage
+        calls and runners then take images (and depth images) of src_width x src_height, Settings' original camera size, and the context's
+        width x height is Camera.newWidth x Camera.newHeight.  (0, 0) or the context's size: off."""
+        check(lib().rgbl_set_input_resize(self.handle, int(src_width), int(src_height)), self.handle)
+
     def set_host_quadtree(self, on: bool):
         check(lib().rgbl_set_host_quadtree(self.handle, int(on)), self.handle)
 
