@@ -3,9 +3,11 @@
 // The ~500-800 edges of a frame are strided over the 16 x 64 threads of the cluster (one pass; the per-edge Jacobian / J^T W J work
 // is bound by the FP64 issue rate of an SM, so sixteen SMs cut it sixteen ways).  J^T W J (21 unique entries), J^T W r (6) and the robust
 // chi2 are reduced inside each CTA with warp shuffles + a fixed shared-memory tree, the partial sums of the CTAs are exchanged through
-// distributed shared memory (each CTA stores its 28 sums into every CTA's exchange slot, one barrier.cluster) and added in rank order
-// by every CTA, so all of them hold bit-identical systems and take the LM decisions redundantly: no broadcast, two cluster barriers per
-// LM trial.  In each CTA, lane 0 of warp w solves the damped 6x6 system of trial w (LDL^T), applies the SE3 exponential update.
+// distributed shared memory (each CTA pushes its sums into every CTA's exchange slot with st.async, no cluster barrier) and added in
+// rank order by every CTA, so all of them hold bit-identical systems and take the LM decisions redundantly: no broadcast.  One exchange
+// per evaluated trial: the pass that evaluates a trial also builds the system at the trial's pose, which is the next iteration's
+// system when the trial is accepted, and the classification pass at the end of a round builds the next round's first system.  In each
+// CTA, lane 0 of warp w solves the damped 6x6 system of trial w (LDL^T), applies the SE3 exponential update.
 // g2o semantics reproduced (Thirdparty/g2o/g2o/: core/optimization_algorithm_levenberg.cpp:61-185,
 // core/base_unary_edge.hpp:43-72, core/robust_kernel_impl.cpp:65-91, types/se3quat.h:104-110,214-254,280-285,
 // types/types_six_dof_expmap.cpp:339-404; src/OptimizableTypes.cpp:49-63):
@@ -215,6 +217,7 @@ __device__ __forceinline__ void huber(double e2, double delta, float dsqr, doubl
 }
 
 constexpr int kAcc = 28;      // 21 H + 6 b + 1 chi
+constexpr int kXchg = kAcc + 1;   // + the trial's chi2 in evaluation order, or the classification's outlier count
 // Cluster shape, measured on an H100 SXM (700 W) through the whole resident chain (tools/pose_variants.sh, bench.py config B,
 // us per tracked frame incl. both searches): 4 x 256: 324   8 x 128: 257   8 x 256: 328   16 x 64: 239   16 x 128: 269.
 // The build / evaluation passes are bound by one SM's FP64 issue rate (~400 DFMA per edge), so more SMs with fewer threads each
@@ -227,7 +230,6 @@ constexpr int kPoseCtas = POSE_CTAS;      // CTAs (SMs) of the cluster that opti
 constexpr int kPoseThreads = POSE_THREADS, kPoseWarps = kPoseThreads / 32, kPoseStride = kPoseCtas * kPoseThreads;
 constexpr int kMaxTrials = 10;    // g2o _maxTrialsAfterFailure (lane l of warp w solves trial w + kPoseWarps * l)
 constexpr int kSolveLanes = (kMaxTrials + kPoseWarps - 1) / kPoseWarps;
-constexpr int kCacheEdges = 512;  // edges PER CTA whose camera-frame point is cached in shared memory (16 KB)
 
 // ---- cluster-wide sums without a cluster barrier ----------------------------------------------------------------------------------
 // barrier.cluster costs ~1.3k cycles here (measured with clock64: arrival skew of four SMs + the L1 invalidation its acquire implies),
@@ -289,35 +291,45 @@ struct ClusterXchg {
     }
 };
 
-// cluster-wide sum of kAcc doubles.  Inside a warp the 28 sums are folded with a halving butterfly: at distance h every lane
-// keeps one half of its slots and ships the other half to its partner, so 16+8+4+2+1 = 31 exchanges replace 28 x 5 and
-// lane L ends up with the warp total of slot L.  The warp totals are added in warp order, the CTA totals go through ClusterXchg.
-__device__ __forceinline__ void cluster_reduce(ClusterXchg& xc, double* v /* 32 slots, 28..31 zero */, double* smem /* warps*kAcc */, double* out /* kAcc, shared */) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+// one level of the halving butterfly below.  The distance is a template argument so that every loop is unrolled and v[] stays in
+// registers (with the distance as a loop variable the inner loop was unrolled before the distance was known: v[] in local memory)
+template <int H>
+__device__ __forceinline__ void butterfly_step(double* v, int lane) {
+    const bool up = (lane & H) != 0;
 #pragma unroll
-    for (int h = 16; h >= 1; h >>= 1) {
-        const bool up = (lane & h) != 0;
-#pragma unroll
-        for (int k = 0; k < h; ++k) {
-            const double send = up ? v[k] : v[k + h];
-            const double keep = up ? v[k + h] : v[k];
-            v[k] = keep + __shfl_xor_sync(0xffffffffu, send, h);
-        }
+    for (int k = 0; k < H; ++k) {
+        const double send = up ? v[k] : v[k + H];
+        const double keep = up ? v[k + H] : v[k];
+        v[k] = keep + __shfl_xor_sync(0xffffffffu, send, H);
     }
-    if (lane < kAcc) smem[warp * kAcc + lane] = v[0];
+}
+
+// cluster-wide sums of the kAcc build sums v and of one more value `last`, in one exchange.  Inside a warp the 28 sums are folded
+// with a halving butterfly: at distance h every lane keeps one half of its slots and ships the other half to its partner, so
+// 16+8+4+2+1 = 31 exchanges replace 28 x 5 and lane L ends up with the warp total of slot L.  `last` is folded with shfl_down into
+// lane 0, the order the trial chi2 of the rho test is summed in (the build's chi2, slot 27, has its own order: both are kept, each
+// feeds its own LM decision).  The warp totals are added in warp order, the CTA totals go through ClusterXchg: out[0..kAcc].
+__device__ __forceinline__ void cluster_reduce(ClusterXchg& xc, double* v /* 32 slots, 28..31 zero */, double last, double* smem /* warps*kXchg */,
+                                               double* out /* kXchg, shared */) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    butterfly_step<16>(v, lane); butterfly_step<8>(v, lane); butterfly_step<4>(v, lane); butterfly_step<2>(v, lane); butterfly_step<1>(v, lane);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) last += __shfl_down_sync(0xffffffffu, last, o);
+    if (lane < kAcc) smem[warp * kXchg + lane] = v[0];
+    if (lane == 0) smem[warp * kXchg + kAcc] = last;
     __syncthreads();
     double s = 0;
-    if (threadIdx.x < kAcc) {
+    if (threadIdx.x < kXchg) {
         double t[kPoseWarps];
 #pragma unroll
-        for (int w = 0; w < kPoseWarps; ++w) t[w] = smem[w * kAcc + threadIdx.x];
+        for (int w = 0; w < kPoseWarps; ++w) t[w] = smem[w * kXchg + threadIdx.x];
 #pragma unroll
         for (int st = 1; st < kPoseWarps; st <<= 1)
 #pragma unroll
             for (int w = 0; w + st < kPoseWarps; w += 2 * st) t[w] += t[w + st];
         s = t[0];
     }
-    xc.sum(s, kAcc, out);
+    xc.sum(s, kXchg, out);
 }
 
 // structural zeros shared by the mono and the stereo Jacobian (d(u)/d(ty) = d(v)/d(tx) = d(ur)/d(ty) = 0)
@@ -328,15 +340,10 @@ __device__ constexpr bool kJnz[3][6] = {{true, true, true, true, false, true}, {
 __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads) pose_optimize_kernel(PoseProblemDev p, double* __restrict__ work, uint8_t* __restrict__ level,
                                                             uint8_t* __restrict__ outlier, float* __restrict__ pose_out,
                                                             int* __restrict__ n_inliers, ChainPrepDev next) {
-    // camera-frame point and 1/z of every edge at the LAST evaluated trial.  When that trial was accepted (s_cache_ok) the
-    // estimate the next system is built at IS that trial: the build reads pc, 1/z (here) and the errors (work[]) instead of
-    // redoing the SE3 action and the reciprocal - the head of its FP64 dependency chain.
-    __shared__ double s_pc[4][kCacheEdges];
-    __shared__ double red[kPoseWarps * kAcc];
-    __shared__ double acc[kAcc];
+    __shared__ double red[kPoseWarps * kXchg];
+    __shared__ double acc[kXchg];         // the cluster totals of the last exchange: the system the next solves start from + one value
     __shared__ __align__(16) double xchg_buf[2][kPoseCtas][32];      // partial sums of the CTAs (written remotely by st.async)
     __shared__ __align__(8) unsigned long long xchg_mbar[2];
-    __shared__ double s_tot[2];
     __shared__ float s_posef[7];
     pdl_trigger();                        // the next kernel of the chain may be scheduled (it waits for this grid's completion itself)
     cg::cluster_group cluster = cg::this_cluster();
@@ -347,7 +354,7 @@ __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads
     pdl_wait();                           // everything above is on-chip set-up and overlaps the tail of the previous kernel; global memory from here on
     __shared__ Se3d s_est, s_init, s_cand[kMaxTrials];
     __shared__ double s_cinv[kMaxTrials], s_lambda, s_ni, s_current, s_ini;
-    __shared__ int s_cache_ok, s_nbad_lm, s_ok, s_cok[kMaxTrials], s_continue;
+    __shared__ int s_build, s_nbad_lm, s_ok, s_cok[kMaxTrials], s_continue;
     const int tid = threadIdx.x, n = p.n_dev ? *p.n_dev : p.n;
     const int gtid = (int)rank * kPoseThreads + tid;
 #ifdef POSE_TIMING
@@ -416,94 +423,80 @@ __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads
         E.e[2] = E.st ? (double)ob[2] - (u - bf * iz) : 0.0;
     };
 
-    // evaluates errors of the active edges at pose T, stores them, returns this thread's partial robust chi2
-    auto eval_errors = [&](const Se3d& T, double& chi_part) {
-        chi_part = 0;
-        for (int k = gtid, lc = tid; k < n; k += kPoseStride, lc += kPoseThreads) {
-            Edge E;
-            load_edge(T, k, E);
-            if (!E.active) continue;
-            if (lc < kCacheEdges) { s_pc[0][lc] = E.pc[0]; s_pc[1][lc] = E.pc[1]; s_pc[2][lc] = E.pc[2]; s_pc[3][lc] = E.invz; }
-            work[3 * (size_t)k] = E.e[0]; work[3 * (size_t)k + 1] = E.e[1]; work[3 * (size_t)k + 2] = E.e[2];
-            double chi = E.e[0] * (E.info * E.e[0]) + E.e[1] * (E.info * E.e[1]) + E.e[2] * (E.info * E.e[2]);
-            if (robust) { double r0, r1; huber(chi, E.st ? ds : dm, E.st ? dsqr_s : dsqr_m, r0, r1); chi = r0; }
-            chi_part += chi;
+    // computeActiveErrors + activeRobustChi2 + buildSystem for one active edge at the pose its camera-frame point and errors E were
+    // computed at: adds its robust chi2 to v[27], rho' J^T Omega J to v[0..20] (upper triangle) and -rho' J^T Omega e to v[21..26]
+    auto accumulate = [&](const Edge& E, bool rob, double (&v)[32]) {
+        const bool st = E.st;
+        const double info = E.info, x = E.pc[0], y = E.pc[1], invz = E.invz, invz_2 = invz * invz;
+        const double e[3] = {E.e[0], E.e[1], E.e[2]};
+        double J[3][6];
+        // rows 0/1 are the same expressions for both edge types (mono: -projectJac * [-(p)x | I], expanded);
+        // the third row of a mono edge is zero, so its terms add exact zeros to the sums
+        J[0][0] = x * y * invz_2 * fx;       J[0][1] = -(1 + (x * x * invz_2)) * fx; J[0][2] = y * invz * fx;
+        J[0][3] = -invz * fx;                J[0][4] = 0;                           J[0][5] = x * invz_2 * fx;
+        J[1][0] = (1 + y * y * invz_2) * fy; J[1][1] = -x * y * invz_2 * fy;        J[1][2] = -x * invz * fy;
+        J[1][3] = 0;                         J[1][4] = -invz * fy;                  J[1][5] = y * invz_2 * fy;
+        const double sbf = st ? bf : 0.0;
+        J[2][0] = st ? J[0][0] - sbf * y * invz_2 : 0.0; J[2][1] = st ? J[0][1] + sbf * x * invz_2 : 0.0;
+        J[2][2] = st ? J[0][2] : 0.0;                    J[2][3] = st ? J[0][3] : 0.0;
+        J[2][4] = 0;                                     J[2][5] = st ? J[0][5] - sbf * invz_2 : 0.0;
+        double chi = 0;
+#pragma unroll
+        for (int r = 0; r < 3; ++r) chi += e[r] * (info * e[r]);
+        double w = 1.0, r0 = chi;
+        if (rob) huber(chi, st ? ds : dm, st ? dsqr_s : dsqr_m, r0, w);
+        v[27] += r0;
+        const double wi = w * info;
+        double WJ[3][6], we[3];
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+            we[r] = wi * e[r];
+#pragma unroll
+            for (int c = 0; c < 6; ++c) WJ[r][c] = kJnz[r][c] ? wi * J[r][c] : 0.0;
+        }
+#pragma unroll
+        for (int i = 0; i < 6; ++i) {
+            double sb = 0;
+#pragma unroll
+            for (int r = 0; r < 3; ++r) if (kJnz[r][i]) sb += J[r][i] * we[r];
+            v[21 + i] -= sb;
+#pragma unroll
+            for (int j = i; j < 6; ++j) {
+                double h = 0;
+#pragma unroll
+                for (int r = 0; r < 3; ++r) if (kJnz[r][i] && kJnz[r][j]) h += J[r][i] * WJ[r][j];
+                v[i * 6 - (i * (i - 1)) / 2 + (j - i)] += h;
+            }
         }
     };
 
     for (int it = 0; it < 4; ++it) {
-        if (tid == 0) { s_est = s_init; s_ok = 1; s_cache_ok = 0; }
+        // round 0 starts with a build pass at the initial pose; every later round's iteration-0 system was built by the previous
+        // round's classification pass
+        if (tid == 0) { s_est = s_init; s_ok = 1; s_build = it == 0; }
         __syncthreads();
         for (int iter = 0; iter < 10; ++iter) {
             if (!s_ok) break;
-            // ---- computeActiveErrors + activeRobustChi2 + buildSystem at the current estimate ----
-            double v[32];
+            // ---- a build pass of its own only where no pass before built this system: round 0's first one, and after an iteration
+            // that ended on a rejected trial without ending the round (rho > 0 with a non-finite chi2, or a NaN rho) ----
+            if (s_build) {
+                double v[32];
 #pragma unroll
-            for (int k = 0; k < 32; ++k) v[k] = 0;
-            TM_START();
-            {
+                for (int k = 0; k < 32; ++k) v[k] = 0;
+                TM_START();
                 const Se3d T = s_est;
-                for (int k = gtid, lc = tid; k < n; k += kPoseStride, lc += kPoseThreads) {
+                for (int k = gtid; k < n; k += kPoseStride) {
                     Edge E;
-                    if (s_cache_ok && lc < kCacheEdges) {
-                        E.st = p.stereo[k] != 0; E.info = (double)p.inv_sigma2[k]; E.active = level[k] == 0;
-                        E.pc[0] = s_pc[0][lc]; E.pc[1] = s_pc[1][lc]; E.pc[2] = s_pc[2][lc]; E.invz = s_pc[3][lc];
-                        E.e[0] = work[3 * (size_t)k]; E.e[1] = work[3 * (size_t)k + 1]; E.e[2] = work[3 * (size_t)k + 2];
-                    } else {
-                        load_edge(T, k, E);
-                    }
-                    if (!E.active) continue;
-                    const bool st = E.st;
-                    const double info = E.info, x = E.pc[0], y = E.pc[1], invz = E.invz, invz_2 = invz * invz;
-                    const double e[3] = {E.e[0], E.e[1], E.e[2]};
-                    double J[3][6];
-                    // rows 0/1 are the same expressions for both edge types (mono: -projectJac * [-(p)x | I], expanded);
-                    // the third row of a mono edge is zero, so its terms add exact zeros to the sums
-                    J[0][0] = x * y * invz_2 * fx;       J[0][1] = -(1 + (x * x * invz_2)) * fx; J[0][2] = y * invz * fx;
-                    J[0][3] = -invz * fx;                J[0][4] = 0;                           J[0][5] = x * invz_2 * fx;
-                    J[1][0] = (1 + y * y * invz_2) * fy; J[1][1] = -x * y * invz_2 * fy;        J[1][2] = -x * invz * fy;
-                    J[1][3] = 0;                         J[1][4] = -invz * fy;                  J[1][5] = y * invz_2 * fy;
-                    const double sbf = st ? bf : 0.0;
-                    J[2][0] = st ? J[0][0] - sbf * y * invz_2 : 0.0; J[2][1] = st ? J[0][1] + sbf * x * invz_2 : 0.0;
-                    J[2][2] = st ? J[0][2] : 0.0;                    J[2][3] = st ? J[0][3] : 0.0;
-                    J[2][4] = 0;                                     J[2][5] = st ? J[0][5] - sbf * invz_2 : 0.0;
-                    work[3 * (size_t)k] = e[0]; work[3 * (size_t)k + 1] = e[1]; work[3 * (size_t)k + 2] = e[2];
-                    double chi = 0;
-#pragma unroll
-                    for (int r = 0; r < 3; ++r) chi += e[r] * (info * e[r]);
-                    double w = 1.0, r0 = chi;
-                    if (robust) huber(chi, st ? ds : dm, st ? dsqr_s : dsqr_m, r0, w);
-                    v[27] += r0;
-                    const double wi = w * info;
-                    double WJ[3][6], we[3];
-#pragma unroll
-                    for (int r = 0; r < 3; ++r) {
-                        we[r] = wi * e[r];
-#pragma unroll
-                        for (int c = 0; c < 6; ++c) WJ[r][c] = kJnz[r][c] ? wi * J[r][c] : 0.0;
-                    }
-#pragma unroll
-                    for (int i = 0; i < 6; ++i) {
-                        double sb = 0;
-#pragma unroll
-                        for (int r = 0; r < 3; ++r) if (kJnz[r][i]) sb += J[r][i] * we[r];
-                        v[21 + i] -= sb;
-#pragma unroll
-                        for (int j = i; j < 6; ++j) {
-                            double h = 0;
-#pragma unroll
-                            for (int r = 0; r < 3; ++r) if (kJnz[r][i] && kJnz[r][j]) h += J[r][i] * WJ[r][j];
-                            v[i * 6 - (i * (i - 1)) / 2 + (j - i)] += h;
-                        }
-                    }
+                    load_edge(T, k, E);
+                    if (E.active) accumulate(E, robust, v);
                 }
-            }
-            TM_ADD(0);
-            cluster_reduce(xc, v, red, acc);
-            TM_ADD(1);
+                TM_ADD(0);
+                cluster_reduce(xc, v, 0.0, red, acc);
+                TM_ADD(1);
 #ifdef POSE_TIMING
-            tc[0]++;
+                tc[0]++;
 #endif
+            }
             // ---- LM trials.  A rejected trial only changes lambda (x nu, nu doubling), never H, b or the estimate, so the damped solves of all (<= 10) possible trials of this iteration
             // are independent: lane 0 of warp w solves trial w while the other warps would idle anyway, and a retry then
             // costs one error evaluation instead of a serial solve + exp. ----
@@ -549,57 +542,59 @@ __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads
             __syncthreads();
             TM_ADD(2);
             for (int trial = 0;; ++trial) {
+                // ---- one pass evaluates the trial (errors -> work[] for the classification, robust chi2 for the rho test) and builds
+                // the system at the trial's pose: if the trial is accepted, that pose is the next iteration's estimate and its
+                // solves start from this exchange; if it is rejected, the system is dropped ----
                 TM_START();
-                double part;
-                eval_errors(s_cand[trial], part);
-                TM_ADD(3);
+                double v[32];
+#pragma unroll
+                for (int k = 0; k < 32; ++k) v[k] = 0;
+                double part = 0;
                 {
-                    const int lane = tid & 31, warp = tid >> 5;
-                    double x = part;
-#pragma unroll
-                    for (int o = 16; o > 0; o >>= 1) x += __shfl_down_sync(0xffffffffu, x, o);
-                    if (lane == 0) red[warp] = x;
-                    __syncthreads();
-                    double s = 0.0;
-                    if (warp == 0) {           // the few warp totals: a pairwise tree read by broadcast, not five more shuffle steps
-                        double t[kPoseWarps];
-#pragma unroll
-                        for (int w = 0; w < kPoseWarps; ++w) t[w] = red[w];
-#pragma unroll
-                        for (int st = 1; st < kPoseWarps; st <<= 1)
-#pragma unroll
-                            for (int w = 0; w + st < kPoseWarps; w += 2 * st) t[w] += t[w + st];
-                        s = t[0];
+                    const Se3d T = s_cand[trial];
+                    for (int k = gtid; k < n; k += kPoseStride) {
+                        Edge E;
+                        load_edge(T, k, E);
+                        if (!E.active) continue;
+                        work[3 * (size_t)k] = E.e[0]; work[3 * (size_t)k + 1] = E.e[1]; work[3 * (size_t)k + 2] = E.e[2];
+                        double chi = E.e[0] * (E.info * E.e[0]) + E.e[1] * (E.info * E.e[1]) + E.e[2] * (E.info * E.e[2]);
+                        if (robust) { double r0, r1; huber(chi, E.st ? ds : dm, E.st ? dsqr_s : dsqr_m, r0, r1); chi = r0; }
+                        part += chi;
+                        accumulate(E, robust, v);
                     }
-                    xc.sum(s, 1, s_tot);
-                    if (tid == 0) {            // every CTA takes the decision from the same partials: identical everywhere
-                        double temp = s_tot[0];
-                        if (!s_cok[trial]) temp = DBL_MAX;
-                        const double rho = (s_current - temp) * s_cinv[trial];
-                        if (rho > 0 && isfinite(temp)) {
-                            const double r21 = 2 * rho - 1;
-                            double alpha = 1. - r21 * r21 * r21;
-                            alpha = fmin(alpha, 2. / 3.);
-                            const double sf = fmax(1. / 3., alpha);
-                            s_lambda *= sf; s_ni = 2; s_current = temp; s_est = s_cand[trial]; s_cache_ok = 1;
-                        } else {
-                            s_lambda *= s_ni; s_ni *= 2; s_cache_ok = 0;       // the estimate is restored = left untouched
-                        }
-                        const int qmax = trial + 1;
-                        const int cont = (rho < 0 && qmax < kMaxTrials) ? 1 : 0;
-                        s_continue = cont;
-                        if (!cont) {                              // end of this LM iteration: g2o's stop tests
-                            int ok = 1;
-                            if (qmax == kMaxTrials || rho == 0) ok = 0;
-                            else {
-                                if ((s_ini - s_current) * 1e3 < s_ini) s_nbad_lm += 1; else s_nbad_lm = 0;
-                                if (s_nbad_lm >= 3) ok = 0;
-                            }
-                            s_ok = ok;
-                        }
-                    }
-                    __syncthreads();
                 }
+                TM_ADD(3);
+                cluster_reduce(xc, v, part, red, acc);
+                if (tid == 0) {            // every CTA takes the decision from the same partials: identical everywhere
+                    double temp = acc[kAcc];
+                    if (!s_cok[trial]) temp = DBL_MAX;
+                    const double rho = (s_current - temp) * s_cinv[trial];
+                    if (rho > 0 && isfinite(temp)) {
+                        const double r21 = 2 * rho - 1;
+                        double alpha = 1. - r21 * r21 * r21;
+                        alpha = fmin(alpha, 2. / 3.);
+                        const double sf = fmax(1. / 3., alpha);
+                        s_lambda *= sf; s_ni = 2; s_current = temp; s_est = s_cand[trial]; s_build = 0;
+#ifdef POSE_TIMING
+                        tc[2]++;
+#endif
+                    } else {
+                        s_lambda *= s_ni; s_ni *= 2; s_build = 1;       // the estimate is restored = left untouched
+                    }
+                    const int qmax = trial + 1;
+                    const int cont = (rho < 0 && qmax < kMaxTrials) ? 1 : 0;
+                    s_continue = cont;
+                    if (!cont) {                              // end of this LM iteration: g2o's stop tests
+                        int ok = 1;
+                        if (qmax == kMaxTrials || rho == 0) ok = 0;
+                        else {
+                            if ((s_ini - s_current) * 1e3 < s_ini) s_nbad_lm += 1; else s_nbad_lm = 0;
+                            if (s_nbad_lm >= 3) ok = 0;
+                        }
+                        s_ok = ok;
+                    }
+                }
+                __syncthreads();
                 TM_ADD(4);
 #ifdef POSE_TIMING
                 tc[1]++;
@@ -607,9 +602,14 @@ __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads
                 if (!s_continue) break;
             }
         }
-        // ---- classification (src/Optimizer.cc:1014-1100) ----
+        // ---- classification (src/Optimizer.cc:1014-1100).  Its pass also builds the next round's iteration-0 system at the initial
+        // pose, with the levels just decided and that round's robust flag, and its exchange carries the outlier count ----
         {
             const Se3d T = s_est;
+            const bool build_next = it < 3 && n >= 10, robust_next = it < 2;
+            double v[32];
+#pragma unroll
+            for (int k = 0; k < 32; ++k) v[k] = 0;
             int bad = 0;
             for (int k = gtid; k < n; k += kPoseStride) {
                 const bool st = p.stereo[k] != 0;
@@ -627,17 +627,17 @@ __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads
                 if (st) chi += e2 * (info * e2);
                 const float chi2 = (float)chi;
                 if (chi2 > (st ? 7.815f : 5.991f)) { outlier[k] = 1; level[k] = 1; ++bad; }
-                else { outlier[k] = 0; level[k] = 0; }
+                else {
+                    outlier[k] = 0; level[k] = 0;
+                    if (build_next) {
+                        Edge E;
+                        load_edge(s_init, k, E);
+                        accumulate(E, robust_next, v);
+                    }
+                }
             }
-            __syncthreads();
-            // cluster sum of `bad`
-            __shared__ int s_bad;
-            if (tid == 0) s_bad = 0;
-            __syncthreads();
-            if (bad) atomicAdd(&s_bad, bad);
-            __syncthreads();
-            xc.sum((double)s_bad, 1, s_tot + 1);
-            n_bad = (int)s_tot[1];
+            cluster_reduce(xc, v, (double)bad, red, acc);
+            n_bad = (int)acc[kAcc];
         }
         if (it == 2) robust = false;
         if (n < 10) break;
@@ -651,7 +651,7 @@ __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads
         s_posef[4] = (float)T.tx; s_posef[5] = (float)T.ty; s_posef[6] = (float)T.tz;
         if (rank == 0) *n_inliers = n - n_bad;
 #ifdef POSE_TIMING
-        if (rank == 0) printf("pose n=%d total=%lld build=%lld(%d) breduce=%lld solve=%lld eval=%lld(%d) evalred=%lld solve6=%lld\n", n, clock64() - t0_, tm[0], tc[0], tm[1], tm[2], tm[3], tc[1], tm[4], tm[5]);
+        if (rank == 0) printf("pose n=%d total=%lld build=%lld(%d) breduce=%lld solve=%lld eval=%lld(%d, %d accepted) evalred=%lld solve6=%lld\n", n, clock64() - t0_, tm[0], tc[0], tm[1], tm[2], tm[3], tc[1], tc[2], tm[4], tm[5]);
 #endif
     }
     prepare_next();
