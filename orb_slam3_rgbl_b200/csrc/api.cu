@@ -1257,7 +1257,7 @@ static int check_sequence_io(Ctx* c, const rgbl_chain_params* chain, const rgbl_
     if (!chain || !io || !io->poses || !io->n_matches || !io->n_inliers) { c->err = "null argument"; return RGBL_E_INVALID; }
     const int T = io->frames_per_batch, nb = io->n_batches;
     if (T < 1 || T > c->cfg.max_batch || nb < 1) { c->err = "bad batch geometry"; return RGBL_E_INVALID; }
-    if (c->chain_pending) { c->err = "a tracking chain is in flight (rgbl_resident_track_end not called)"; return RGBL_E_INVALID; }
+    if (const int rc = require_idle(c)) return rc;
     if (io->gray) {
         int rc = check_batch_args(c, T, io->width, io->height, io->stride); if (rc) return rc;
     } else if (io->n_slots < 1 || io->n_slots > Ctx::kMaxStageSlots) { c->err = "resident mode needs 1..8 staged slots"; return RGBL_E_INVALID; }
@@ -1491,8 +1491,7 @@ int rgbl_set_stereo_rectification(rgbl_ctx* ctx, const float* m1l, const float* 
 // System::TrackStereo).  Every check runs before anything is changed, so a refused setting leaves the previous one in place.
 int rgbl_set_input_resize(rgbl_ctx* ctx, int src_width, int src_height) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    if (!c) return RGBL_E_INVALID;
-    if (c->chain_pending) { c->err = "a tracking chain is in flight (rgbl_resident_track_end not called)"; return RGBL_E_INVALID; }
+    if (const int rc = require_idle(c)) return rc;
     if (src_width < 0 || src_height < 0 || (src_width == 0) != (src_height == 0)) {
         c->err = "the input size is (0, 0) (no resize) or two positive sizes"; return RGBL_E_INVALID;
     }
@@ -1541,7 +1540,7 @@ int rgbl_set_camera_distortion(rgbl_ctx* ctx, float fx, float fy, float cx, floa
     bool finite = std::isfinite(fx) && std::isfinite(fy) && std::isfinite(cx) && std::isfinite(cy);
     for (int i = 0; i < n_dist; ++i) finite = finite && std::isfinite(dist[i]);
     if (!finite || !(fx > 0.f) || !(fy > 0.f)) { c->err = "the camera needs finite values and fx, fy > 0"; return RGBL_E_INVALID; }
-    if (c->chain_pending) { c->err = "a tracking chain is in flight (rgbl_resident_track_end not called)"; return RGBL_E_INVALID; }
+    if (const int rc = require_idle(c)) return rc;
     const UndistortDev m = make_undistort_dev(fx, fy, cx, cy, dist, n_dist);
     float b[4];
     image_bounds(m, dist[0], c->cfg.width, c->cfg.height, b);      // once per setting, with the kernel's arithmetic

@@ -488,8 +488,7 @@ extern "C" int rgbl_local_bundle_adjustment(rgbl_ctx* ctx, int n_poses, const fl
                                             const float* inv_sigma2, float fx, float fy, float cx, float cy, float bf, int iterations,
                                             float* poses_out, float* points_out, uint8_t* edge_erase, int* iterations_run) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
-    if (!c) return RGBL_E_INVALID;
-    if (c->chain_pending) { c->err = "a tracking chain is in flight (rgbl_resident_track_end not called)"; return RGBL_E_INVALID; }
+    if (const int rc = require_idle(c)) return rc;
     if (n_poses < 0 || n_points < 0 || n_edges < 0 || iterations < 0 || (n_poses && (!poses || !pose_fixed || !poses_out)) || (n_points && (!points || !points_out)) ||
         (n_edges && (!e_point || !e_pose || !obs || !stereo || !inv_sigma2 || !edge_erase))) { c->err = "bad local BA arguments"; return RGBL_E_INVALID; }
     for (int k = 0; k < n_edges; ++k)

@@ -94,8 +94,7 @@ int rgbl_compute_bow(rgbl_ctx* ctx, const rgbl_vocabulary* voc, int n, const uin
                      double* bow_value, int* n_words, int32_t* fv_node, int32_t* fv_start, int32_t* fv_feature, int* n_fv_nodes) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     const Vocab* v = reinterpret_cast<const Vocab*>(voc);
-    if (!c) return RGBL_E_INVALID;
-    if (c->chain_pending) { c->err = "a tracking chain is in flight (rgbl_resident_track_end not called)"; return RGBL_E_INVALID; }
+    if (const int rc = require_idle(c)) return rc;
     if (!v || n < 0 || (n > 0 && !desc) || !n_words || !n_fv_nodes || !fv_start || (n > 0 && (!bow_word || !bow_value || !fv_node || !fv_feature))) {
         c->err = "bad ComputeBoW arguments"; return RGBL_E_INVALID;
     }
@@ -113,8 +112,7 @@ int rgbl_resident_compute_bow(rgbl_ctx* ctx, const rgbl_vocabulary* voc, int fra
                               int* n_words, int32_t* fv_node, int32_t* fv_start, int32_t* fv_feature, int* n_fv_nodes) {
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     const Vocab* v = reinterpret_cast<const Vocab*>(voc);
-    if (!c) return RGBL_E_INVALID;
-    if (c->chain_pending) { c->err = "a tracking chain is in flight (rgbl_resident_track_end not called)"; return RGBL_E_INVALID; }
+    if (const int rc = require_idle(c)) return rc;
     if (!v || !n_words || !n_fv_nodes || !fv_start || !bow_word || !bow_value || !fv_node || !fv_feature) { c->err = "bad ComputeBoW arguments"; return RGBL_E_INVALID; }
     if (frame < 0 || frame >= c->last_frames) { c->err = "frame slot out of range"; return RGBL_E_INVALID; }
     if (v->device != c->cfg.device) { c->err = "vocabulary lives on another device"; return RGBL_E_INVALID; }

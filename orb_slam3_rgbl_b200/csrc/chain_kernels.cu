@@ -41,7 +41,7 @@ __device__ __forceinline__ int lb_exclusive_base(const Lookback& lb, int count, 
         for (int j = tid; j < b; j += 32) {
             int v = lb_load(lb.slots + j), spins = 0;
             while (v == 0 && ++spins < kSpinLimit) v = lb_load(lb.slots + j);
-            if (v == 0) { atomicExch(lb.fail, 9); v = 1; }
+            if (v == 0) { atomicExch(lb.fail, kTlmWaitFailed); v = 1; }
             sum += v - 1;
         }
 #pragma unroll

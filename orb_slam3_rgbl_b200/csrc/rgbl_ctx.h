@@ -1,7 +1,10 @@
-// Context of librgbl_b200.so: memory plan, streams, profiling state (shared by api.cu and api_track.cu).
+// Context of librgbl_b200.so: memory plan, streams, profiling state (shared by api.cu, api_track.cu, api_bow.cu, api_ba.cu and
+// api_mapping.cu).
 #ifndef RGBL_CTX_H
 #define RGBL_CTX_H
 
+#include <algorithm>
+#include <cstddef>
 #include <string>
 #include <vector>
 
@@ -21,6 +24,43 @@ constexpr int kMatchListCap = 512;    // admissible candidates kept per map poin
 // right image of a pair: rectified, or raw when the context rectifies them)
 enum class InputKind { rgbl, rgbd, stereo };
 
+// Words of TrackBufs::scalars (device, 16 ints) the tracking entry points use: the frame size FrameDev::n points at, a search's match
+// count and resolution rounds (adjacent: read back as one pair), PoseOptimization's inlier count.
+constexpr int kDevFrameN = 0, kDevMatches = 1, kDevRounds = 2, kDevPoseInliers = 8;
+// Words of Ctx::h_scalars (pinned, 16 ints).  Every call that uses them is synchronous, so each owns its words for its own duration only:
+//   api_track.cu   the words named here; kHostFusePose: ints 4..13 as ten floats (pose, camera centre) of rgbl_fuse_search
+//   api_bow.cu     [0..2] ComputeBoW's counts, [8] a frame's keypoint count;   api_mapping.cu   [0] a match count
+//   api_ba.cu      all 16 as eight doubles (a trial's scalars), [12] the solver's status
+constexpr int kHostFrameN = 0, kHostMatches = 4, kHostRounds = 5, kHostFusePose = 4, kHostPoseInliers = 8;
+static_assert(kDevRounds == kDevMatches + 1 && kHostRounds == kHostMatches + 1, "a search's match count and rounds are read back as one pair");
+
+// State that persists between the chains of one sequence (device, TrackBufs::carry), next to the carried frame's arrays: its keypoint
+// count and pose, the local map ring's frame counter, the pose of the frame before it.  The chain hands member addresses to its kernels.
+struct ChainCarry { int n_sel; float pose[7]; int ring_count; float prev_pose[7]; };
+static_assert(sizeof(ChainCarry) == 16 * 4 && offsetof(ChainCarry, pose) == 4 && offsetof(ChainCarry, ring_count) == 32 &&
+              offsetof(ChainCarry, prev_pose) == 36, "ChainCarry is 16 packed 32-bit words");
+
+// Counters of one chain over nF frames: TrackBufs::ch_counts on the device, a slot of Ctx::h_chain_i on the host (one copy brings all of
+// them back).  Four blocks of nF ints, then the tail: edges of the first and the second PoseOptimization, the forward / backward flags of the
+// last-frame search, the overflow word (matcher list overflow, or kTlmWaitFailed), the local search's query count.
+struct ChainCounts { int *n_matches, *n_inliers, *n_local_matches, *n_inliers_first, *n_edges, *n_edges2, *flags, *overflow, *n_queries; };
+constexpr size_t chain_count_ints(size_t nF) { return 4 * nF + 8; }
+inline ChainCounts chain_counts(int* base, size_t nF) {
+    int* tail = base + 4 * nF;
+    return {base, base + nF, base + 2 * nF, base + 3 * nF, tail, tail + 1, tail + 2, tail + 4, tail + 5};
+}
+// Poses of one chain in a slot of Ctx::h_chain_f: the pose given for frame 0 (read by a chain that starts a sequence), then the nF results
+constexpr size_t chain_pose_floats(size_t nF) { return 7 + nF * 7; }
+
+// Launch parameters of a chain: with the context's buffers and its settings fixed at rgbl_create, everything the enqueue of the chain
+// reads (api_track.cu: enqueue_chain takes this struct and nothing else of the call).
+struct ChainPlan { int nF, cap, mono, cont, K, prev_valid; float th, th_local, nn_local, fx, fy, cx, cy, bf, bounds[4]; };
+// capacity of the query arrays of the chain's local search: the queries are compacted, at most every point of the local map ring
+inline int local_query_cap(const ChainPlan& p) { return std::max(p.K * p.cap, 1); }
+// Key of a slot's CUDA graph: the plan, and Ctx::scratch_generation for the buffer addresses.  Compared with memcmp: value-initialise it.
+struct ChainGraphKey { ChainPlan plan; unsigned long long generation; };
+static_assert(sizeof(ChainPlan) % sizeof(unsigned long long) == 0, "no padding in ChainGraphKey");
+
 // Lazily grown device scratch of the tracking entry points (api_track.cu).
 struct TrackBufs {
     DeviceArray<rgbl_keypoint> keys; DeviceArray<float> uright; DeviceArray<uint8_t> desc, state;
@@ -38,7 +78,7 @@ struct TrackBufs {
     DeviceArray<int> s_nsel, b_cell_start, b_csr_idx, b_kp_cell;
     // state that persists between the chains of one sequence: the carried last frame and the local map ring (chain_kernels.cu)
     DeviceArray<rgbl_keypoint> c_kps; DeviceArray<uint8_t> c_desc; DeviceArray<float> c_depth;
-    DeviceArray<uint32_t> c_misc;                        // n_sel | pose[7] | ring frame counter
+    DeviceArray<ChainCarry> carry;                       // one element
     DeviceArray<uint8_t> r_valid, r_desc, lq_u8, lq_desc; DeviceArray<float> r_xw, r_normal, r_min, r_max, lq_f; DeviceArray<int> lq_i, match_local;
     DeviceArray<int> lookback;                           // slot arrays of the multi-CTA compactions (chain_kernels.cu), kept zero between launches
     // ComputeBoW
@@ -179,11 +219,10 @@ struct Ctx {
     bool chain_timing_on = false, chain_graphs_on = true;   // RGBL_CHAIN_TIMING / RGBL_CHAIN_GRAPH, read at rgbl_create
     bool chain_pdl_on = true;                               // RGBL_CHAIN_PDL=0: ordinary launches between the chain's kernels
     Event chain_tev[8];
-    PinnedArray<float> h_chain_f;  // per slot: pose0 (7) | poses (cap * 7)
-    PinnedArray<int> h_chain_i;    // per slot: n_matches | n_inliers | n_local_matches | n_inliers_first | n_edges x2, flags[2], overflow, n_queries
+    PinnedArray<float> h_chain_f;  // per slot: chain_pose_floats(h_chain_cap)
+    PinnedArray<int> h_chain_i;    // per slot: chain_count_ints(h_chain_cap), laid out by chain_counts(slot's base, the chain's frames)
     size_t h_chain_cap = 0;      // frames per slot
     // the chain of a slot as an instantiated CUDA graph (re-captured when any launch parameter or scratch pointer changes)
-    struct ChainGraphKey { int nF, cap, mono, cont, K, prev_valid; float th, th_local, nn_local, fx, fy, cx, cy, bf, bounds[4]; unsigned long long generation; };
     GraphExec chain_exec[2];
     ChainGraphKey chain_key[2] = {};
     bool chain_timing_recorded = false;      // RGBL_CHAIN_TIMING development aid: chain_tev hold the timings of a chain
@@ -236,6 +275,53 @@ struct ArenaCarve {
         }                                                                                          \
     } while (0)
 
+
+// Entry guard of every call that must not run beside a tracking chain: the context exists and no chain is in flight.  (Only
+// rgbl_resident_track_begin* / _end*, which queue and collect the chains, run with one pending.)
+inline int require_idle(Ctx* c) {
+    if (!c) return RGBL_E_INVALID;
+    if (c->chain_pending) { c->err = "a tracking chain is in flight (rgbl_resident_track_end not called)"; return RGBL_E_INVALID; }
+    return RGBL_OK;
+}
+
+// frames per half of the per-slot buffers: the context's full batch (frame construction refuses larger ones), so that the halves never
+// move while a chain is in flight
+inline size_t slot_frames(const Ctx* c) { return (size_t)std::max(c->last_frames, c->cfg.max_batch); }
+
+// A slot's half of the per-slot buffers: the snapshot of the batch's frame outputs, the per-frame grids, the pinned result staging.
+struct ChainSlot {
+    rgbl_keypoint* s_kps; uint8_t* s_desc; float* s_depth; float* s_uright; int* s_nsel;
+    int* b_cell_start; int* b_csr_idx; int* b_kp_cell;
+    float* h_f; int* h_i;
+};
+inline ChainSlot chain_slot(Ctx* c, int slot) {
+    TrackBufs& t = c->trk;
+    const size_t nF = slot_frames(c), tot = nF * c->cap_kp, cs = nF * (kGridCols * kGridRows + 1);
+    return {t.s_kps + slot * tot, t.s_desc + slot * tot * 32, t.s_depth + slot * tot, t.s_uright + slot * tot, t.s_nsel + slot * nF,
+            t.b_cell_start + slot * cs, t.b_csr_idx + slot * tot, t.b_kp_cell + slot * tot,
+            c->h_chain_f + slot * chain_pose_floats(c->h_chain_cap), c->h_chain_i + slot * chain_count_ints(c->h_chain_cap)};
+}
+
+// The query arrays of the chain's local search: planes of n_lq elements in lq_u8 (2), lq_f (8: five scalars, then xyz) and lq_i (2)
+constexpr int kLqU8Planes = 2, kLqFPlanes = 8, kLqIPlanes = 2;
+inline LocalQueriesDev local_queries(TrackBufs& t, int n_lq, int* n) {
+    const size_t s = (size_t)n_lq;
+    LocalQueriesDev lq{};
+    lq.cap = n_lq; lq.n = n; lq.in_view = t.lq_u8; lq.obs_pos = t.lq_u8 + s;
+    lq.proj_x = t.lq_f; lq.proj_y = t.lq_f + s; lq.proj_xr = t.lq_f + 2 * s; lq.depth = t.lq_f + 3 * s; lq.view_cos = t.lq_f + 4 * s; lq.xw = t.lq_f + 5 * s;
+    lq.level = t.lq_i; lq.src = t.lq_i + s; lq.desc = t.lq_desc;
+    return lq;
+}
+
+// n elements between host and device memory on the context's main stream; n == 0 issues nothing (the pointers may then be null).  The
+// element size comes from the host pointer's type; the device side (a DeviceArray or a pointer into one) converts to it.
+template <class T> struct SameAs { using type = T; };
+template <class T> inline cudaError_t h2d(Ctx* c, typename SameAs<T>::type* dst, const T* src, size_t n) {
+    return n ? cudaMemcpyAsync(dst, src, n * sizeof(T), cudaMemcpyHostToDevice, c->st) : cudaSuccess;
+}
+template <class T> inline cudaError_t d2h(Ctx* c, T* dst, const typename SameAs<T>::type* src, size_t n) {
+    return n ? cudaMemcpyAsync(dst, src, n * sizeof(T), cudaMemcpyDeviceToHost, c->st) : cudaSuccess;
+}
 
 // profiling helpers (api.cu)
 void stage_begin(Ctx* c, int stage, cudaStream_t st);

@@ -199,7 +199,8 @@ struct ChainTlmTail {
     int n_last_cap; const uint8_t* last_valid; const int* last_octave; const uint8_t* last_desc; const float* last_pose;
 };
 // tlm_prepare compacts over several CTAs in one launch; `lookback` = tlm_lookback_ints() ZERO-INITIALISED ints (the kernel leaves them zero),
-// `fail` = a device flag set to 9 if a CTA ever waited in vain
+// `fail` = a device flag set to kTlmWaitFailed if a CTA ever waited in vain
+constexpr int kTlmWaitFailed = 9;
 int tlm_lookback_ints();
 
 // stereo_kernels.cu --------------------------------------------------------------------------------
