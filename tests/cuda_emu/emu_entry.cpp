@@ -1,14 +1,14 @@
 // TEST INFRASTRUCTURE: C entry points that run the library's kernels (device code paths) on the CUDA-on-CPU shim.
 // The marshalling mirrors the host-twin hooks of the product library; the difference is that these go through the real
 // launchers (launch_fast_strips, launch_describe_staged, launch_quadtree) and therefore through the kernels' device branches.
-#include "cuda_runtime.h"
+// A unit of the emulated library (tests/cuda_emu/build.py); tests/test_cuda_emu.py calls it.
+#include <cstring>
+#include <string>
+#include <vector>
 
-#include "orb_kernels.emu.cpp"
-#include "fast_strip_kernels.emu.cpp"
-#include "describe_warp_kernels.emu.cpp"
-#include "quadtree_kernels.emu.cpp"
-#include "depth_kernels.emu.cpp"
-#include "depth_dilate_v2.emu.cpp"
+#include "rgbl_device.cuh"
+#include "rgbl_internal.h"
+#include "rgbl_kernels.h"
 
 using namespace rgbl;
 

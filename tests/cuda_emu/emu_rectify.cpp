@@ -1,8 +1,8 @@
 // TEST INFRASTRUCTURE: the stereo rectification kernels (map conversion, batched remap) on the CUDA-on-CPU shim, through the library's
-// real launchers (tests/test_cuda_emu_rectify.py builds this file against stereo_kernels.cu).
-#include "cuda_runtime.h"
-
-#include "stereo_kernels.emu.cpp"
+// real launchers.  A unit of the emulated library (tests/cuda_emu/build.py); tests/test_cuda_emu_rectify.py calls it.
+#include "rgbl_device.cuh"
+#include "rgbl_internal.h"
+#include "rgbl_kernels.h"
 
 using namespace rgbl;
 

@@ -1,12 +1,11 @@
 // TEST INFRASTRUCTURE: the input-resize kernels (the 8-bit plane resize of orb_kernels.cu, both its staged-tile and its gather form, and the
-// 16-bit depth resize of depth_kernels.cu) on the CUDA-on-CPU shim, through the library's real launchers (tests/test_cuda_emu_resize.py
-// builds this file against the two kernel files and host_tables.cpp).
-#include "cuda_runtime.h"
-
+// 16-bit depth resize of depth_kernels.cu) on the CUDA-on-CPU shim, through the library's real launchers.  A unit of the emulated library
+// (tests/cuda_emu/build.py); tests/test_cuda_emu_resize.py calls it.
 #include <vector>
 
-#include "orb_kernels.emu.cpp"
-#include "depth_kernels.emu.cpp"
+#include "rgbl_device.cuh"
+#include "rgbl_internal.h"
+#include "rgbl_kernels.h"
 
 using namespace rgbl;
 

@@ -1,9 +1,12 @@
 // TEST INFRASTRUCTURE: the RGB-D device code paths (16-bit depth PNG reconstruction, uint16 depth gather) on the CUDA-on-CPU shim,
-// through the library's real launchers (tests/test_cuda_emu_rgbd.py builds this file against png_kernels.cu and depth_kernels.cu).
-#include "cuda_runtime.h"
+// through the library's real launchers.  A unit of the emulated library (tests/cuda_emu/build.py); tests/test_cuda_emu_rgbd.py calls it.
+#include <cstring>
+#include <string>
+#include <vector>
 
-#include "png_kernels.emu.cpp"
-#include "depth_kernels.emu.cpp"
+#include "rgbl_device.cuh"
+#include "rgbl_internal.h"
+#include "rgbl_kernels.h"
 
 using namespace rgbl;
 

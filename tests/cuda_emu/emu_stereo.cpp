@@ -1,10 +1,10 @@
-// TEST INFRASTRUCTURE: the batched Frame::ComputeStereoMatches kernels on the CUDA-on-CPU shim, through the library's real launcher
-// (tests/test_cuda_emu_stereo.py builds this file against stereo_kernels.cu).
+// TEST INFRASTRUCTURE: the batched Frame::ComputeStereoMatches kernels on the CUDA-on-CPU shim, through the library's real launcher.
+// A unit of the emulated library (tests/cuda_emu/build.py); tests/test_cuda_emu_stereo.py calls it.
 #include <vector>
 
-#include "cuda_runtime.h"
-
-#include "stereo_kernels.emu.cpp"
+#include "rgbl_device.cuh"
+#include "rgbl_internal.h"
+#include "rgbl_kernels.h"
 
 using namespace rgbl;
 

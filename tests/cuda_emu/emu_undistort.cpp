@@ -1,8 +1,9 @@
 // TEST INFRASTRUCTURE: Frame::UndistortKeyPoints / ComputeImageBounds of a distorted camera on the CUDA-on-CPU shim, through the
-// library's real launcher and host helpers (tests/test_cuda_emu_undistort.py builds this file against depth_kernels.cu).
-#include "cuda_runtime.h"
-
-#include "depth_kernels.emu.cpp"
+// library's real launcher and host helpers.  A unit of the emulated library (tests/cuda_emu/build.py); tests/test_cuda_emu_undistort.py
+// calls it.
+#include "rgbl_device.cuh"
+#include "rgbl_internal.h"
+#include "rgbl_kernels.h"
 
 using namespace rgbl;
 

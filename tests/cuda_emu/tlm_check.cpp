@@ -1,7 +1,9 @@
 // TEST INFRASTRUCTURE: runs the multi-CTA TrackLocalMap glue kernel of chain_kernels.cu (tlm_prepare: ordered compaction by "publish and look
 // back") on the CUDA-on-CPU shim and compares them with a serial restatement that walks the same arrays in index order.
-// Built and run by tests/test_cuda_emu.py::test_tlm_kernels_device_path.  Exit code 0 = identical.
+// A unit of the emulated library (tests/cuda_emu/build.py); tests/test_cuda_emu.py::test_tlm_kernels_device_path calls it.
+#include <cmath>
 #include <cstdio>
+#include <cstring>
 #include <random>
 #include <vector>
 
@@ -13,8 +15,9 @@ using namespace rgbl;
 static int fails = 0;
 #define CHECK(c, ...) do { if (!(c)) { if (fails < 20) { std::printf("FAIL %s:%d: ", __FILE__, __LINE__); std::printf(__VA_ARGS__); std::printf("\n"); } ++fails; } } while (0)
 
-int main(int argc, char** argv) {
-    const unsigned seed = argc > 1 ? (unsigned)std::atoi(argv[1]) : 1u;
+// one random frame, pose and ring from `seed`; returns the number of mismatches (0 = identical)
+extern "C" int emu_tlm_check(unsigned seed) {
+    fails = 0;
     std::mt19937 rng(seed);
     std::uniform_real_distribution<float> U(0.f, 1.f);
     const int K = 3, cap = 700 + (int)(seed % 5) * 97;        // not a multiple of the CTA size
@@ -94,6 +97,6 @@ int main(int argc, char** argv) {
         for (int i = 0; i < cap; ++i) { CHECK(state[i] == st_ref[i], "state[%d]", i); CHECK(match_last[i] == ml[i], "match_last[%d]", i); }
     }
     std::printf("tlm_prepare: %d queries of %d ring points, %d mismatches\n", nq, n_ring, fails);
-
-    return fails ? 1 : 0;
+    std::fflush(stdout);
+    return fails;
 }

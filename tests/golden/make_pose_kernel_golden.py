@@ -10,11 +10,10 @@ ROOT = Path(__file__).resolve().parents[2]
 sys.path.insert(0, str(ROOT)); sys.path.insert(0, str(ROOT / "tests"))
 import test_cuda_emu_pose_bitwise as TB  # noqa: E402
 
-mod = TB._build_module()
 libs, out = {}, {}
 for shape, name in TB.CHECKED:
     if shape not in libs:
-        libs[shape] = TB.emulated(mod, shape)
+        libs[shape] = TB.emulated(shape)
     for key, a in zip(("n_inliers", "pose", "outlier"), TB.outputs(libs[shape], TB.CASES[name])):
         out[f"{shape}/{name}/{key}"] = a
 for e in libs.values():

@@ -3,12 +3,13 @@
 rgbl_create and of the lazily allocating entry points fail in turn, and expects RGBL_E_CUDA, then a retry on the same context with
 a fresh context's outputs.  LeakSanitizer reports anything left allocated at exit.  PoseOptimization and the tracking chain are not
 emulated: their streams, events, pinned staging and graphs are covered by the GPU suite only."""
-import importlib.util
 import os
 import subprocess
 from pathlib import Path
 
 import pytest
+
+from cuda_emu import build
 
 HERE = Path(__file__).resolve().parent
 ROOT = HERE.parent
@@ -27,9 +28,7 @@ def test_ctx_lifetime_under_address_sanitizer(tmp_path):
     if "LeakSanitizer: detected memory leaks" not in probe.stderr:
         pytest.skip("LeakSanitizer cannot run here: a program that leaks on purpose is not reported (" + probe.stderr.strip()[-200:] + ")")
 
-    spec = importlib.util.spec_from_file_location("cuda_emu_build", HERE / "cuda_emu" / "build.py")
-    mod = importlib.util.module_from_spec(spec); spec.loader.exec_module(mod)
-    lib = mod.build_full(force=True, sanitize="address", out_dir=tmp_path / "asan")
+    lib = build.build_full(sanitize="address")
     driver = tmp_path / "lifetime_driver"
     subprocess.run(["gcc", "-std=c99", "-O1", "-g", "-fsanitize=address", f"-I{ROOT / 'include'}", str(HERE / "cuda_emu" / "lifetime_driver.c"),
                     f"-L{lib.parent}", "-lrgbl_b200_emu", f"-Wl,-rpath,{lib.parent}", "-lz", "-lm", "-o", str(driver)], check=True)

@@ -3,28 +3,24 @@
 The host twins (tests/test_host_abi.py) check the algorithms; this checks the device-only glue around them: shuffle scans,
 shared-memory atomics, warp reductions, dynamic shared-memory carving and the launch geometry."""
 import ctypes as C
-import importlib.util
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import oracle
+from cuda_emu import build
 from orb_slam3_rgbl_b200 import _lib as L
 from orb_slam3_rgbl_b200 import synthetic as S
-
-HERE = Path(__file__).resolve().parent
 
 
 @pytest.fixture(scope="module")
 def emu():
-    spec = importlib.util.spec_from_file_location("cuda_emu_build", HERE / "cuda_emu" / "build.py")
-    mod = importlib.util.module_from_spec(spec); spec.loader.exec_module(mod)
-    lib = C.CDLL(str(mod.build()))
+    lib = C.CDLL(str(build.build_full()))
     vp, i = C.c_void_p, C.c_int
     lib.emu_fast_strips.argtypes = [vp, i, i, i, vp, i, i, i, vp, i]
     lib.emu_describe_staged.argtypes = [vp, vp, vp, i, i, i, i, vp, vp, vp]
     lib.emu_quadtree.argtypes = [vp, i, i, i, i, vp, i]
+    lib.emu_tlm_check.argtypes = [C.c_uint]
     return lib
 
 
@@ -131,12 +127,8 @@ def test_whole_extraction_pipeline_device_path(emu):
 
 
 @pytest.mark.parametrize("seed", [1, 2, 3])
-def test_tlm_kernels_device_path(seed):
+def test_tlm_kernels_device_path(emu, seed):
     """The multi-CTA TrackLocalMap glue kernels (chain_kernels.cu: ordered compaction by 'publish and look back', the in-kernel grid
-    barrier before the ring hand-over, self-cleaning slot arrays) against a serial restatement (tests/cuda_emu/tlm_check.cpp)."""
-    import subprocess
-    spec = importlib.util.spec_from_file_location("cuda_emu_build", HERE / "cuda_emu" / "build.py")
-    mod = importlib.util.module_from_spec(spec); spec.loader.exec_module(mod)
-    exe = mod.build_tlm_check()
-    r = subprocess.run([str(exe), str(seed)], capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-2000:]
+    barrier before the ring hand-over, self-cleaning slot arrays) against a serial restatement (tests/cuda_emu/tlm_check.cpp, which
+    prints the first mismatches)."""
+    assert emu.emu_tlm_check(seed) == 0

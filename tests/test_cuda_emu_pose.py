@@ -3,23 +3,15 @@ over the CUDA-on-CPU shim (tests/cuda_emu): all CTAs of the cluster run at once,
 mbarrier exchange.  A subset of the edge cases of pose_cases.py against oracle.pose_optimize_trace, at the shipped cluster shape
 (16 CTAs x 64 threads) and at 8 x 128, with the bars of pose_cases.compare; every call is repeated and must give identical outputs."""
 import ctypes as C
-import importlib.util
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import pose_cases as PC
+from cuda_emu import build
 from orb_slam3_rgbl_b200 import _lib as L
 
-HERE = Path(__file__).resolve().parent
 SHAPES = {"16x64": [], "8x128": ["-DPOSE_CTAS=8", "-DPOSE_THREADS=128"]}
-
-
-def _build_module():
-    spec = importlib.util.spec_from_file_location("cuda_emu_build", HERE / "cuda_emu" / "build.py")
-    mod = importlib.util.module_from_spec(spec); spec.loader.exec_module(mod)
-    return mod
 
 
 class EmuPose:
@@ -51,9 +43,7 @@ class EmuPose:
 
 @pytest.fixture(scope="module", params=list(SHAPES))
 def emu(request):
-    mod = _build_module()
-    out = mod.BUILD / ("pose_" + request.param) if request.param != "16x64" else None
-    e = EmuPose(mod.build_full(defines=SHAPES[request.param], out_dir=out))
+    e = EmuPose(build.build_full(defines=SHAPES[request.param]))
     yield e
     e.close()
 

@@ -14,7 +14,8 @@ import numpy as np
 import pytest
 
 import pose_cases as PC
-from test_cuda_emu_pose import SHAPES, EmuPose, _build_module
+from cuda_emu import build
+from test_cuda_emu_pose import SHAPES, EmuPose
 
 GOLD = Path(__file__).resolve().parent / "golden" / "pose_kernel_base.npz"
 CASES = {c["name"]: c for c in PC.all_cases()}
@@ -28,17 +29,17 @@ def outputs(e, c):
     return np.array([ni], np.int32), pose, out
 
 
-def emulated(mod, shape):
-    return EmuPose(mod.build_full(defines=SHAPES[shape], out_dir=mod.BUILD / ("pose_" + shape) if shape != "16x64" else None))
+def emulated(shape):
+    return EmuPose(build.build_full(defines=SHAPES[shape]))
 
 
 @pytest.fixture(scope="module")
 def emu():
-    mod, libs = _build_module(), {}
+    libs = {}
 
     def get(shape):
         if shape not in libs:
-            libs[shape] = emulated(mod, shape)
+            libs[shape] = emulated(shape)
         return libs[shape]
     yield get
     for e in libs.values():

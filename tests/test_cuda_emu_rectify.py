@@ -3,34 +3,18 @@ remap of both cameras' frames) on the CUDA-on-CPU shim (tests/cuda_emu), bit for
 to cv2 in tests/test_oracle_rectify.py): both cameras and several frames per camera in one launch, maps past every edge, wholly outside
 the image, exact 1/64 ties and saturating values, an odd width (a partial last group of 4 pixels) and the last row and column."""
 import ctypes as C
-import importlib.util
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
+from cuda_emu import build
 from oracle import _p
 from oracle import rectify as RC
-
-HERE = Path(__file__).resolve().parent
 
 
 @pytest.fixture(scope="module")
 def emu():
-    spec = importlib.util.spec_from_file_location("cuda_emu_build", HERE / "cuda_emu" / "build.py")
-    mod = importlib.util.module_from_spec(spec); spec.loader.exec_module(mod)
-    d = mod.BUILD / "rectify"
-    d.mkdir(parents=True, exist_ok=True)
-    for f in mod.CSRC.iterdir():
-        if f.suffix in (".h", ".cuh", ".inc"):
-            (d / f.name).write_text(mod._transform(f.read_text()))
-    (d / "stereo_kernels.emu.cpp").write_text(mod._transform((mod.CSRC / "stereo_kernels.cu").read_text()))
-    lib = d / "libcuda_emu_rectify.so"
-    subprocess.run(["g++", "-std=c++20", "-O1", "-g", "-pthread", "-fPIC", "-shared", "-ffp-contract=off", "-Wno-unknown-pragmas", "-Wno-attributes",
-                    f"-I{HERE / 'cuda_emu'}", f"-I{d}", "-o", str(lib), str(HERE / "cuda_emu" / "emu_rectify.cpp"),
-                    str(HERE / "cuda_emu" / "emu_runtime.cpp")], check=True)
-    L_ = C.CDLL(str(lib))
+    L_ = C.CDLL(str(build.build_full()))
     L_.emu_rectify_maps.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
     L_.emu_rectify.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int]
     return L_

@@ -3,36 +3,18 @@ reading separate source planes, staged-tile form up to a ratio of about 1.35, ga
 several planes per launch.  Whole output planes must equal cv2.resize(INTER_LINEAR) - or, without cv2, the oracle pinned to it in
 tests/test_oracle_resize.py - bit for bit, and nothing outside the destination images may be written."""
 import ctypes as C
-import importlib.util
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import resize_oracle as RO
+from cuda_emu import build
 from oracle import _p
-
-HERE = Path(__file__).resolve().parent
 
 
 @pytest.fixture(scope="module")
 def emu():
-    spec = importlib.util.spec_from_file_location("cuda_emu_build", HERE / "cuda_emu" / "build.py")
-    mod = importlib.util.module_from_spec(spec); spec.loader.exec_module(mod)
-    d = mod.BUILD / "resize"
-    d.mkdir(parents=True, exist_ok=True)
-    for f in mod.CSRC.iterdir():
-        if f.suffix in (".h", ".cuh", ".inc"):
-            (d / f.name).write_text(mod._transform(f.read_text()))
-    for f in ("orb_kernels.cu", "depth_kernels.cu"):
-        (d / (f[:-3] + ".emu.cpp")).write_text(mod._transform((mod.CSRC / f).read_text()))
-    (d / "host_tables.cpp").write_text(mod._transform((mod.CSRC / "host_tables.cpp").read_text()))
-    lib = d / "libcuda_emu_resize.so"
-    subprocess.run(["g++", "-std=c++20", "-O1", "-g", "-pthread", "-fPIC", "-shared", "-ffp-contract=off", "-Wno-unknown-pragmas", "-Wno-attributes",
-                    f"-I{HERE / 'cuda_emu'}", f"-I{d}", "-include", str(HERE / "cuda_emu" / "cuda_runtime.h"), "-o", str(lib),
-                    str(HERE / "cuda_emu" / "emu_resize.cpp"), str(d / "host_tables.cpp"), str(HERE / "cuda_emu" / "emu_runtime.cpp")], check=True)
-    L_ = C.CDLL(str(lib))
+    L_ = C.CDLL(str(build.build_full()))
     L_.emu_resize_planes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
     L_.emu_resize_depth16.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]
     return L_

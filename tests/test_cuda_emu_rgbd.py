@@ -1,37 +1,20 @@
 """The RGB-D device code paths on the CUDA-on-CPU shim (tests/cuda_emu): the 16-bit depth PNG reconstruction (png_unfilter_gray_kernel's
 depth output stage, an image taller than one 512-row band) and the uint16 depth gather (depth_gather_kernel<uint16_t>), against the oracle."""
 import ctypes as C
-import importlib.util
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import oracle
+from cuda_emu import build
 from oracle import rgbd as R
 from orb_slam3_rgbl_b200 import _lib as L
 from orb_slam3_rgbl_b200 import synthetic as S
 
-HERE = Path(__file__).resolve().parent
-
 
 @pytest.fixture(scope="module")
 def emu():
-    spec = importlib.util.spec_from_file_location("cuda_emu_build", HERE / "cuda_emu" / "build.py")
-    mod = importlib.util.module_from_spec(spec); spec.loader.exec_module(mod)
-    d = mod.BUILD / "rgbd"
-    d.mkdir(parents=True, exist_ok=True)
-    for f in mod.CSRC.iterdir():
-        if f.suffix in (".h", ".cuh", ".inc"):
-            (d / f.name).write_text(mod._transform(f.read_text()))
-    for f in ("png_kernels.cu", "depth_kernels.cu"):
-        (d / (f[:-3] + ".emu.cpp")).write_text(mod._transform((mod.CSRC / f).read_text()))
-    lib = d / "libcuda_emu_rgbd.so"
-    subprocess.run(["g++", "-std=c++20", "-O1", "-g", "-pthread", "-fPIC", "-shared", "-ffp-contract=off", "-Wno-unknown-pragmas", "-Wno-attributes",
-                    f"-I{HERE / 'cuda_emu'}", f"-I{d}", "-o", str(lib), str(HERE / "cuda_emu" / "emu_rgbd.cpp"),
-                    str(HERE / "cuda_emu" / "emu_runtime.cpp"), "-lz"], check=True)
-    L_ = C.CDLL(str(lib))
+    L_ = C.CDLL(str(build.build_full()))
     L_.emu_png_depth16.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_void_p]
     L_.emu_gather_u16.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
     return L_

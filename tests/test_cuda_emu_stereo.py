@@ -1,37 +1,22 @@
 """The batched Frame::ComputeStereoMatches kernels (stereo_kernels.cu: row index count / scan / fill, match, median rejection) on the
 CUDA-on-CPU shim (tests/cuda_emu), several pairs in one launch, against the oracle's restatement of the reference (stereo_oracle.cpp)."""
 import ctypes as C
-import importlib.util
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import oracle
+from cuda_emu import build
 from oracle import _p
 from orb_slam3_rgbl_b200 import _lib as L
 from orb_slam3_rgbl_b200 import synthetic as S
 
-HERE = Path(__file__).resolve().parent
 W, H = 320, 160
 
 
 @pytest.fixture(scope="module")
 def emu():
-    spec = importlib.util.spec_from_file_location("cuda_emu_build", HERE / "cuda_emu" / "build.py")
-    mod = importlib.util.module_from_spec(spec); spec.loader.exec_module(mod)
-    d = mod.BUILD / "stereo"
-    d.mkdir(parents=True, exist_ok=True)
-    for f in mod.CSRC.iterdir():
-        if f.suffix in (".h", ".cuh", ".inc"):
-            (d / f.name).write_text(mod._transform(f.read_text()))
-    (d / "stereo_kernels.emu.cpp").write_text(mod._transform((mod.CSRC / "stereo_kernels.cu").read_text()))
-    lib = d / "libcuda_emu_stereo.so"
-    subprocess.run(["g++", "-std=c++20", "-O1", "-g", "-pthread", "-fPIC", "-shared", "-ffp-contract=off", "-Wno-unknown-pragmas", "-Wno-attributes",
-                    f"-I{HERE / 'cuda_emu'}", f"-I{d}", "-o", str(lib), str(HERE / "cuda_emu" / "emu_stereo.cpp"),
-                    str(HERE / "cuda_emu" / "emu_runtime.cpp")], check=True)
-    L_ = C.CDLL(str(lib))
+    L_ = C.CDLL(str(build.build_full()))
     L_.emu_stereo_idx_cap.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_int]
     L_.emu_stereo_matches.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

@@ -1,37 +1,22 @@
 """Frame::UndistortKeyPoints / ComputeImageBounds of a distorted camera on the CUDA-on-CPU shim (tests/cuda_emu): undistort_keypoints_kernel
 through its launcher and the host bounds helper of rgbl_set_camera_distortion, bit for bit against the oracle, with 4 and 5 coefficients."""
 import ctypes as C
-import importlib.util
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
+from cuda_emu import build
 from oracle import undistort as U
 from orb_slam3_rgbl_b200 import _lib as L
 from orb_slam3_rgbl_b200 import synthetic as S
 
-HERE = Path(__file__).resolve().parent
 CAM = (S.TUM1_FX, S.TUM1_FY, S.TUM1_CX, S.TUM1_CY)
 DISTS = {"tum1": S.TUM1_DIST, "tum1_4": S.TUM1_DIST[:4], "barrel": np.array([-0.31, 0.11, 0.0012, -0.0021, -0.02], np.float32)}
 
 
 @pytest.fixture(scope="module")
 def emu():
-    spec = importlib.util.spec_from_file_location("cuda_emu_build", HERE / "cuda_emu" / "build.py")
-    mod = importlib.util.module_from_spec(spec); spec.loader.exec_module(mod)
-    d = mod.BUILD / "undistort"
-    d.mkdir(parents=True, exist_ok=True)
-    for f in mod.CSRC.iterdir():
-        if f.suffix in (".h", ".cuh", ".inc"):
-            (d / f.name).write_text(mod._transform(f.read_text()))
-    (d / "depth_kernels.emu.cpp").write_text(mod._transform((mod.CSRC / "depth_kernels.cu").read_text()))
-    lib = d / "libcuda_emu_undistort.so"
-    subprocess.run(["g++", "-std=c++20", "-O1", "-g", "-pthread", "-fPIC", "-shared", "-ffp-contract=off", "-Wno-unknown-pragmas", "-Wno-attributes",
-                    f"-I{HERE / 'cuda_emu'}", f"-I{d}", "-o", str(lib), str(HERE / "cuda_emu" / "emu_undistort.cpp"),
-                    str(HERE / "cuda_emu" / "emu_runtime.cpp")], check=True)
-    L_ = C.CDLL(str(lib))
+    L_ = C.CDLL(str(build.build_full()))
     f, i, vp = C.c_float, C.c_int, C.c_void_p
     L_.emu_undistort_keypoints.argtypes = [f, f, f, f, vp, i, vp, vp, i, i, vp]
     L_.emu_image_bounds.argtypes = [f, f, f, f, vp, i, i, i, vp]

@@ -4,17 +4,15 @@
 batch of the case's kind is uploaded, processed and downloaded, and must equal a fresh context's outputs bit for bit.  Every runner
 case is refused before its tracking chain starts."""
 import ctypes as C
-import importlib.util
-from pathlib import Path
 
 import numpy as np
 import pytest
 
+from cuda_emu import build
 from orb_slam3_rgbl_b200 import _lib as L
 from orb_slam3_rgbl_b200 import frontend as F
 from orb_slam3_rgbl_b200 import synthetic as S
 
-HERE = Path(__file__).resolve().parent
 W, H, B, NPTS = 160, 120, 4, 400      # context size, max_batch, max_points
 N = 2                                 # frames (RGB-L, RGB-D) or pairs (stereo) of a valid batch
 INV, CAP, EMPTY, UNSUP = L.RGBL_E_INVALID, L.RGBL_E_CAPACITY, L.RGBL_E_EMPTY, L.RGBL_E_UNSUPPORTED
@@ -24,9 +22,7 @@ FX, FY, CX, CY = 100.0, 100.0, 80.0, 60.0
 
 @pytest.fixture(scope="module")
 def lib():
-    spec = importlib.util.spec_from_file_location("cuda_emu_build", HERE / "cuda_emu" / "build.py")
-    mod = importlib.util.module_from_spec(spec); spec.loader.exec_module(mod)
-    so = C.CDLL(str(mod.build_full()))
+    so = C.CDLL(str(build.build_full()))
     for name, (res, args) in L.SYMBOLS.items():
         fn = getattr(so, name)
         fn.restype, fn.argtypes = res, args

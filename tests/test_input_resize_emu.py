@@ -4,19 +4,17 @@ rectification) built from input-size images equal, bit for bit, the frames of a 
 inputs; every status rule of the setting and of the entry points it changes; after each refused call the context still builds the frames
 of a fresh context with the same setting, and clearing the setting gives back the frames of a context that never had it."""
 import ctypes as C
-import importlib.util
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import resize_oracle as RO
+from cuda_emu import build
 from oracle import rectify as RC
 from orb_slam3_rgbl_b200 import _lib as L
 from orb_slam3_rgbl_b200 import frontend as F
 from orb_slam3_rgbl_b200 import synthetic as S
 
-HERE = Path(__file__).resolve().parent
 W, H, B, NPTS = 160, 120, 4, 400      # context size (Settings::newImSize), max_batch, max_points
 SW, SH = 320, 240                     # input size, integer factors (RGB-D and stereo)
 TW, TH = 200, 150                     # input size, factor 1.25 (stereo only; the staged-tile kernel form)
@@ -28,9 +26,7 @@ FX, FY, CX, CY = 100.0, 100.0, 80.0, 60.0
 
 @pytest.fixture(scope="module")
 def lib():
-    spec = importlib.util.spec_from_file_location("cuda_emu_build", HERE / "cuda_emu" / "build.py")
-    mod = importlib.util.module_from_spec(spec); spec.loader.exec_module(mod)
-    so = C.CDLL(str(mod.build_full()))
+    so = C.CDLL(str(build.build_full()))
     for name, (res, args) in L.SYMBOLS.items():
         fn = getattr(so, name)
         fn.restype, fn.argtypes = res, args

@@ -2,12 +2,13 @@
 (tests/cuda_emu/rectify_lifetime_driver.c), both with AddressSanitizer.  Each lazy allocation of the rectification (the fixed-point maps,
 their float staging, the raw planes) fails once: the call returns RGBL_E_CUDA, the retry gives a
 fresh context's outputs, and LeakSanitizer finds nothing left allocated."""
-import importlib.util
 import os
 import subprocess
 from pathlib import Path
 
 import pytest
+
+from cuda_emu import build
 
 HERE = Path(__file__).resolve().parent
 ROOT = HERE.parent
@@ -24,9 +25,7 @@ def test_rectification_allocations_under_address_sanitizer(tmp_path):
     subprocess.run(["gcc", "-fsanitize=address", "-o", str(tmp_path / "leak"), str(leak)], check=True)
     if "LeakSanitizer: detected memory leaks" not in _run([str(tmp_path / "leak")]).stderr:
         pytest.skip("LeakSanitizer cannot run here: a program that leaks on purpose is not reported")
-    spec = importlib.util.spec_from_file_location("cuda_emu_build", HERE / "cuda_emu" / "build.py")
-    mod = importlib.util.module_from_spec(spec); spec.loader.exec_module(mod)
-    lib = mod.build_full(force=True, sanitize="address", out_dir=tmp_path / "asan")
+    lib = build.build_full(sanitize="address")
     driver = tmp_path / "rectify_lifetime_driver"
     subprocess.run(["gcc", "-std=c99", "-O1", "-g", "-fsanitize=address", f"-I{ROOT / 'include'}", str(HERE / "cuda_emu" / "rectify_lifetime_driver.c"),
                     f"-L{lib.parent}", "-lrgbl_b200_emu", f"-Wl,-rpath,{lib.parent}", "-lz", "-lm", "-o", str(driver)], check=True)

@@ -1,16 +1,13 @@
 """rgbl_frame_rgbl_batch (extraction + LiDAR depth of a 2-frame batch) through the real C ABI of the EMULATED library
-(tests/cuda_emu, `build.py full`), compared bit for bit with the oracle, without a GPU:
+(tests/cuda_emu/build.py), compared bit for bit with the oracle, without a GPU:
     python tests/tools/emu_abi_variants.py
 """
 import sys, os
 ROOT = __import__('pathlib').Path(__file__).resolve().parent.parent.parent
 sys.path.insert(0, str(ROOT)); sys.path.insert(0, str(ROOT / 'tests'))
-from pathlib import Path
 from orb_slam3_rgbl_b200 import _lib
-import importlib.util
-spec = importlib.util.spec_from_file_location('cuda_emu_build', ROOT / 'tests' / 'cuda_emu' / 'build.py')
-mod = importlib.util.module_from_spec(spec); spec.loader.exec_module(mod)
-_lib.LIB_PATH = mod.build_full()
+from cuda_emu import build
+_lib.LIB_PATH = build.build_full()
 import numpy as np, oracle
 from orb_slam3_rgbl_b200 import frontend as F, synthetic as S
 W,H=420,260

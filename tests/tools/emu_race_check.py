@@ -1,13 +1,15 @@
 """Race check of the emulated kernels (tests/cuda_emu) under ThreadSanitizer: every conflicting pair of accesses that is not
 separated by a barrier / warp rendezvous is reported, whatever the timing.  Usage:
     bash tests/tools/emu_race_check.sh
-(builds tests/cuda_emu/build/libcuda_emu_tsan.so and runs this file under LD_PRELOAD=libtsan for: the extraction pipeline and the
+(builds the emulated library with -fsanitize=thread and runs this file under LD_PRELOAD=libtsan for: the extraction pipeline and the
 dilation kernel)."""
 import ctypes as C, os, sys, numpy as np
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
+ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
 import oracle
+from cuda_emu import build
 from orb_slam3_rgbl_b200 import _lib as L, synthetic as S
-lib=C.CDLL(os.path.join(os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))), 'tests/cuda_emu/build/libcuda_emu_tsan.so'))
+lib=C.CDLL(str(build.build_full(sanitize='thread')))
 which=sys.argv[1]
 if which=='extract':
     w,h=200,160; img=S.make_image(81,w,h); prm=L.OrbParams(200,1.2,3,12,7)
