@@ -615,6 +615,54 @@ def local_bundle_adjustment(poses, pose_fixed, points, e_point, e_pose, obs, ste
     return po, pt, er, it, chi.value
 
 
+class BATraceC(C.Structure):
+    """BATrace (oracle/ba_oracle.cpp)."""
+    _fields_ = [("cap_trials", C.c_int), ("cap_iters", C.c_int),
+                ("trial_lambda", C.c_void_p), ("trial_rho", C.c_void_p), ("trial_accepted", C.c_void_p), ("trial_ok", C.c_void_p),
+                ("iter_qmax", C.c_void_p), ("iter_bad", C.c_void_p), ("iter_margin", C.c_void_p), ("edge_margin", C.c_void_p),
+                ("n_trials", C.c_int), ("n_iters", C.c_int), ("max_reject_run", C.c_int),
+                ("term_qmax", C.c_int), ("term_nbad", C.c_int), ("term_rho0", C.c_int),
+                ("solver_failures", C.c_int), ("ended_on_rejected_trial", C.c_int),
+                ("min_rho_margin", C.c_double), ("min_stop_margin", C.c_double), ("min_huber_margin", C.c_double),
+                ("min_flag_margin", C.c_double), ("min_margin", C.c_double)]
+
+
+def local_bundle_adjustment_trace(poses, pose_fixed, points, e_point, e_pose, obs, stereo, inv_sigma2, fx, fy, cx, cy, bf, iterations=10):
+    """local_bundle_adjustment with the same outputs plus a dict of what the call did.  Per LM trial: trial_lambda, trial_rho,
+    trial_accepted, trial_ok (the factorisation succeeded).  Per iteration: iter_qmax (trials run), iter_bad (the
+    (ini - current) * 1e3 < ini decision; False when the iteration ended the run before that test) and iter_margin (its relative
+    margin).  Totals: max_reject_run (most consecutive rejected trials in one iteration), term_qmax / term_nbad / term_rho0 (how the
+    run ended; none set = the iteration limit), solver_failures, ended_on_rejected_trial (the erase flags then use the errors of a
+    state that was not kept).  Margins (relative distance of a decision from its threshold, inf when none was taken):
+    min_rho_margin (the smaller of |rho| and the relative chi2 change of the trial), min_stop_margin, min_huber_margin, min_flag_margin (chi2 against 5.991 / 7.815 and depth against 0, per edge in
+    edge_margin) and min_margin, the smallest of them.
+    -> (poses[n,7], points[m,3], erase[n_edges], iterations, chi2, trace)"""
+    L = lib()
+    _late(L)
+    if L.orc_local_bundle_adjustment_trace.argtypes is None:
+        L.orc_local_bundle_adjustment_trace.argtypes = L.orc_local_bundle_adjustment.argtypes + [C.POINTER(BATraceC)]
+        L.orc_local_bundle_adjustment_trace.restype = C.c_int
+    poses = np.ascontiguousarray(poses, np.float32).reshape(-1, 7); pose_fixed = np.ascontiguousarray(pose_fixed, np.uint8)
+    points = np.ascontiguousarray(points, np.float32).reshape(-1, 3)
+    e_point = np.ascontiguousarray(e_point, np.int32); e_pose = np.ascontiguousarray(e_pose, np.int32)
+    obs = np.ascontiguousarray(obs, np.float32).reshape(-1, 3); stereo = np.ascontiguousarray(stereo, np.uint8)
+    inv_sigma2 = np.ascontiguousarray(inv_sigma2, np.float32)
+    po = np.empty_like(poses); pt = np.empty_like(points); er = np.zeros(len(e_point), np.uint8); chi = C.c_double(0)
+    ct, ci = 10 * iterations + 1, iterations + 1
+    arr = dict(trial_lambda=np.zeros(ct), trial_rho=np.zeros(ct), trial_accepted=np.zeros(ct, np.uint8), trial_ok=np.zeros(ct, np.uint8),
+               iter_qmax=np.zeros(ci, np.int32), iter_bad=np.zeros(ci, np.uint8), iter_margin=np.full(ci, np.inf),
+               edge_margin=np.full(max(len(e_point), 1), np.inf))
+    tr = BATraceC(ct, ci, *[a.ctypes.data for a in arr.values()])
+    it = L.orc_local_bundle_adjustment_trace(len(poses), _p(poses), _p(pose_fixed), len(points), _p(points), len(e_point), _p(e_point), _p(e_pose),
+                                             _p(obs), _p(stereo), _p(inv_sigma2), fx, fy, cx, cy, bf, iterations, _p(po), _p(pt), _p(er),
+                                             C.byref(chi), C.byref(tr))
+    trace = {name: getattr(tr, name) for name, t in BATraceC._fields_ if t is not C.c_void_p and not name.startswith("cap_")}
+    for name, a in arr.items():
+        n = len(e_point) if name == "edge_margin" else (tr.n_trials if name.startswith("trial_") else tr.n_iters)
+        trace[name] = a[:n].astype(bool) if a.dtype == np.uint8 else a[:n]
+    return po, pt, er, it, chi.value, trace
+
+
 def distinctive_descriptors(obs_start, desc):
     _late(lib())
     obs_start = np.ascontiguousarray(obs_start, np.int32); desc = np.ascontiguousarray(desc, np.uint8).reshape(-1, 32)

@@ -26,6 +26,28 @@ struct Cam { float fx, fy, cx, cy, bf; };
 
 struct BAEdge { int point, pose; double obs[3]; double info; bool stereo; double err[3]; };
 
+// What one call did (orc_local_bundle_adjustment_trace): every LM trial and iteration, how the run ended, and how close each discrete
+// decision came to going the other way.  Margins are relative: for the accept / reject test the smaller of |rho| (already a ratio) and
+// |chi2 - trial chi2| / chi2 (near convergence rho is a ratio of two rounding-sized numbers and says nothing about its own sign),
+// |(ini - cur) * 1e3 - ini| / |ini| for the stop test, |e2 - delta^2| / delta^2 for the Huber switch, and per edge of the erase test
+// min(|chi2 - threshold| / threshold, |z| / |p_camera|).  Decisions that do not depend on rounding (a failed solve, a non-finite
+// value, 0 against 0) are not counted.  The per-trial / per-iteration / per-edge arrays belong to the caller (capacities cap_*).
+struct BATrace {
+    int cap_trials, cap_iters;
+    double* trial_lambda; double* trial_rho; uint8_t* trial_accepted; uint8_t* trial_ok;
+    int* iter_qmax; uint8_t* iter_bad; double* iter_margin;     // per iteration: trials run; of those that reached the stop test, its decision and margin
+    double* edge_margin;                                        // n_edges: margin of each edge's erase test
+    int n_trials, n_iters;
+    int max_reject_run;                                         // most consecutive rejected trials in one iteration
+    int term_qmax, term_nbad, term_rho0;                        // how the run ended (none set: the iteration limit)
+    int solver_failures, ended_on_rejected_trial;
+    double min_rho_margin, min_stop_margin, min_huber_margin, min_flag_margin, min_margin;
+};
+
+inline void margin(double& m, double dist, double scale) {
+    if (std::isfinite(dist) && std::isfinite(scale) && scale != 0) m = std::min(m, std::fabs(dist) / std::fabs(scale));
+}
+
 struct BA {
     Cam cam;
     std::vector<SE3> poses; std::vector<uint8_t> fixed; std::vector<int> pose_slot;     // slot in the reduced system or -1
@@ -38,6 +60,7 @@ struct BA {
     std::vector<double> Hpl;           // per edge 18 (6 x 3), valid when the pose is not fixed
     std::vector<double> x;             // solution: poses then points
     double lambda = 0, ni = 2; int n_bad = 0;
+    BATrace* tr = nullptr;
     const double delta_mono = (double)(float)std::sqrt(5.991), delta_stereo = (double)(float)std::sqrt(7.815);
 
     void edge_error(BAEdge& e) const {
@@ -65,6 +88,7 @@ struct BA {
             double rho[2];
             const double d = e.stereo ? delta_stereo : delta_mono;
             huber(chi2(e), d, (float)(d * d), rho);
+            if (tr) margin(tr->min_huber_margin, chi2(e) - (double)(float)(d * d), (double)(float)(d * d));
             s += rho[0];
         }
         return s;
@@ -246,7 +270,7 @@ struct BA {
             for (int l = 0; l < np; ++l) for (int j = 0; j < 3; ++j) mx = std::max(std::fabs(Hll[9 * (size_t)l + 4 * j]), mx);
             lambda = 1e-5 * mx; ni = 2; n_bad = 0;
         }
-        double rho = 0; int qmax = 0;
+        double rho = 0; int qmax = 0, reject_run = 0;
         do {
             const std::vector<SE3> backup_poses = poses; const std::vector<double> backup_pts = pts;      // push()
             const bool ok2 = solve(lambda);
@@ -260,6 +284,22 @@ struct BA {
             for (int j = 0; j < 3 * np; ++j) scale += x[n + j] * (lambda * x[n + j] + bl[j]);
             scale += 1e-3;
             rho /= scale;
+            if (tr) {
+                const bool accepted = rho > 0 && std::isfinite(temp);
+                if (tr->n_trials < tr->cap_trials) {
+                    tr->trial_lambda[tr->n_trials] = lambda; tr->trial_rho[tr->n_trials] = rho;
+                    tr->trial_accepted[tr->n_trials] = accepted; tr->trial_ok[tr->n_trials] = ok2;
+                }
+                ++tr->n_trials;
+                if (!ok2) ++tr->solver_failures;
+                if (ok2 && !(current == 0 && temp == 0) && std::isfinite(rho)) {
+                    tr->min_rho_margin = std::min(tr->min_rho_margin, std::fabs(rho));
+                    margin(tr->min_rho_margin, current - temp, std::max(current, temp));
+                }
+                tr->ended_on_rejected_trial = !accepted;
+                reject_run = accepted ? 0 : reject_run + 1;
+                tr->max_reject_run = std::max(tr->max_reject_run, reject_run);
+            }
             if (rho > 0 && std::isfinite(temp)) {
                 double alpha = 1. - std::pow(2 * rho - 1, 3);
                 alpha = std::min(alpha, 2. / 3.);
@@ -269,6 +309,18 @@ struct BA {
             }
             ++qmax;
         } while (rho < 0 && qmax < 10);
+        if (tr) {
+            const int i = tr->n_iters++;
+            const bool stop = qmax == 10 || rho == 0;
+            if (qmax == 10) tr->term_qmax = 1; else if (rho == 0) tr->term_rho0 = 1;
+            if (i < tr->cap_iters) {
+                tr->iter_qmax[i] = qmax; tr->iter_bad[i] = !stop && (ini - current) * 1e3 < ini;
+                tr->iter_margin[i] = std::numeric_limits<double>::infinity();
+                if (!stop && ini != 0) margin(tr->iter_margin[i], (ini - current) * 1e3 - ini, ini);
+            }
+            if (!stop && ini != 0) margin(tr->min_stop_margin, (ini - current) * 1e3 - ini, ini);
+            if (!stop && (ini - current) * 1e3 < ini && n_bad + 1 >= 3) tr->term_nbad = 1;
+        }
         if (qmax == 10 || rho == 0) return 1;
         if ((ini - current) * 1e3 < ini) ++n_bad; else n_bad = 0;
         if (n_bad >= 3) return 1;
@@ -276,19 +328,16 @@ struct BA {
     }
 };
 
-}  // namespace
-
-extern "C" {
-
 // poses: n_poses x 7 floats (qx qy qz qw tx ty tz, Tcw); pose_fixed[n_poses]; points: n_points x 3 floats;
 // edges: e_point, e_pose, obs (n_edges x 3 floats: u, v, ur), stereo flags, inv_sigma2.  Outputs: optimised poses / points (float,
 // fixed poses unchanged) and per edge the reference's erase test (chi2 > 5.991 / 7.815 with the errors of the LAST evaluated
 // trial, or non-positive depth at the final estimates).  Returns the number of LM iterations run.
-int orc_local_bundle_adjustment(int n_poses, const float* poses, const uint8_t* pose_fixed, int n_points, const float* points, int n_edges,
-                                const int32_t* e_point, const int32_t* e_pose, const float* obs, const uint8_t* stereo,
-                                const float* inv_sigma2, float fx, float fy, float cx, float cy, float bf, int iterations,
-                                float* poses_out, float* points_out, uint8_t* edge_erase, double* final_chi2) {
+int local_bundle_adjustment(int n_poses, const float* poses, const uint8_t* pose_fixed, int n_points, const float* points, int n_edges,
+                            const int32_t* e_point, const int32_t* e_pose, const float* obs, const uint8_t* stereo,
+                            const float* inv_sigma2, float fx, float fy, float cx, float cy, float bf, int iterations,
+                            float* poses_out, float* points_out, uint8_t* edge_erase, double* final_chi2, BATrace* tr) {
     BA ba;
+    ba.tr = tr;
     ba.cam = Cam{fx, fy, cx, cy, bf};
     ba.poses.resize(n_poses); ba.fixed.assign(pose_fixed, pose_fixed + n_poses); ba.pose_slot.resize(n_poses);
     for (int p = 0; p < n_poses; ++p) {
@@ -321,9 +370,42 @@ int orc_local_bundle_adjustment(int n_poses, const float* poses, const uint8_t* 
         double p[3];
         se3_map(ba.poses[e.pose], &ba.pts[3 * (size_t)e.point], p);
         edge_erase[k] = (ba.chi2(e) > (e.stereo ? 7.815 : 5.991) || !(p[2] > 0.0)) ? 1 : 0;
+        if (tr) {
+            double m = std::numeric_limits<double>::infinity();
+            margin(m, ba.chi2(e) - (e.stereo ? 7.815 : 5.991), e.stereo ? 7.815 : 5.991);
+            margin(m, p[2], std::sqrt(p[0] * p[0] + p[1] * p[1] + p[2] * p[2]));
+            tr->edge_margin[k] = m;
+            tr->min_flag_margin = std::min(tr->min_flag_margin, m);
+        }
     }
+    if (tr) tr->min_margin = std::min(std::min(tr->min_rho_margin, tr->min_stop_margin), std::min(tr->min_huber_margin, tr->min_flag_margin));
+    ba.tr = nullptr;
     if (final_chi2) { *final_chi2 = ba.active_robust_chi2(); }
     return it;
+}
+
+}  // namespace
+
+extern "C" {
+
+int orc_local_bundle_adjustment(int n_poses, const float* poses, const uint8_t* pose_fixed, int n_points, const float* points, int n_edges,
+                                const int32_t* e_point, const int32_t* e_pose, const float* obs, const uint8_t* stereo,
+                                const float* inv_sigma2, float fx, float fy, float cx, float cy, float bf, int iterations,
+                                float* poses_out, float* points_out, uint8_t* edge_erase, double* final_chi2) {
+    return local_bundle_adjustment(n_poses, poses, pose_fixed, n_points, points, n_edges, e_point, e_pose, obs, stereo, inv_sigma2, fx, fy, cx, cy, bf, iterations,
+                                   poses_out, points_out, edge_erase, final_chi2, nullptr);
+}
+
+// orc_local_bundle_adjustment with the same arithmetic and outputs, plus what the call did (BATrace above); the caller sets the
+// capacities and array pointers of *tr
+int orc_local_bundle_adjustment_trace(int n_poses, const float* poses, const uint8_t* pose_fixed, int n_points, const float* points, int n_edges,
+                                      const int32_t* e_point, const int32_t* e_pose, const float* obs, const uint8_t* stereo,
+                                      const float* inv_sigma2, float fx, float fy, float cx, float cy, float bf, int iterations,
+                                      float* poses_out, float* points_out, uint8_t* edge_erase, double* final_chi2, BATrace* tr) {
+    tr->n_trials = tr->n_iters = tr->max_reject_run = tr->term_qmax = tr->term_nbad = tr->term_rho0 = tr->solver_failures = tr->ended_on_rejected_trial = 0;
+    tr->min_rho_margin = tr->min_stop_margin = tr->min_huber_margin = tr->min_flag_margin = tr->min_margin = std::numeric_limits<double>::infinity();
+    return local_bundle_adjustment(n_poses, poses, pose_fixed, n_points, points, n_edges, e_point, e_pose, obs, stereo, inv_sigma2, fx, fy, cx, cy, bf, iterations,
+                                   poses_out, points_out, edge_erase, final_chi2, tr);
 }
 
 }  // extern "C"

@@ -376,13 +376,19 @@ __global__ void __launch_bounds__(1024) ba_cholesky_kernel(int n, int use_smem, 
     if (use_smem) for (int i = tid; i < n; i += nt) x[i] = y[i];
 }
 
-// landmark increments, trial points, gain denominator terms of the landmarks
+// landmark increments, trial points, gain denominator terms of the landmarks.  After a failed factorisation (status[0] != 0) the whole
+// solution is zero: g2o's solve() (core/block_solver.hpp:354-486) returns when the reduced system cannot be solved, before the landmark
+// back substitution.  The trial points are then the current ones, so the errors the rejected trial leaves behind (the erase test reads
+// them) are those of the estimate, and no increment is formed from a D^-1 that need not be finite
 __global__ void __launch_bounds__(128) ba_point_update_kernel(BaDev g, const double* __restrict__ blk, const double* __restrict__ Hll, const double* __restrict__ bl,
-                                                              double lam, const double* __restrict__ xp, const double* __restrict__ pts,
-                                                              double* __restrict__ pts_try, double* __restrict__ partial) {
+                                                              double lam, const double* __restrict__ xp, const int* __restrict__ status,
+                                                              const double* __restrict__ pts, double* __restrict__ pts_try, double* __restrict__ partial) {
     const int l = blockIdx.x * 128 + threadIdx.x;
     double sc = 0;
-    if (l < g.n_points) {
+    if (l < g.n_points && status[0] != 0) {
+#pragma unroll
+        for (int i = 0; i < 3; ++i) pts_try[3 * (size_t)l + i] = pts[3 * (size_t)l + i];
+    } else if (l < g.n_points) {
         double D[9];
         dinv3(Hll + 6 * (size_t)l, lam, D);
         double c[3] = {bl[3 * (size_t)l], bl[3 * (size_t)l + 1], bl[3 * (size_t)l + 2]};
@@ -543,6 +549,7 @@ extern "C" int rgbl_local_bundle_adjustment(rgbl_ctx* ctx, int n_poses, const fl
     CU(up(d_psstart, ps_start.data(), (size_t)(n_opt + 1) * 4)); CU(up(d_psedges, ps_edges.data(), ps_edges.size() * 4));
     CU(up(d_poses_f, poses, (size_t)n_poses * 28)); CU(up(d_pts_f, points, (size_t)n_points * 12));
     CU(cudaMemsetAsync(d_status, 0, 16, st));
+    CU(cudaMemsetAsync(d_err, 0, (size_t)3 * n_edges * sizeof(double), st));      // iterations = 0: the erase test sees zero errors, only depth can flag
     BaDev g{n_poses, n_opt, n_points, n_edges, fx, fy, cx, cy, bf, d_epoint, d_epose, d_obs, d_stereo, d_info, d_slot, d_ptstart, d_ptedges, d_psstart, d_psedges};
     const int init_n = std::max(n_poses, 3 * n_points);
     ba_init_state_kernel<<<(init_n + 255) / 256, 256, 0, st>>>(n_poses, d_poses_f, d_pose[0], 3 * n_points, d_pts_f, d_pts[0]);
@@ -584,7 +591,7 @@ extern "C" int rgbl_local_bundle_adjustment(rgbl_ctx* ctx, int n_poses, const fl
                 ba_cholesky_kernel<<<1, chol_threads, chol_smem, st>>>(n, chol_in_smem, d_S, d_bp, d_coef, d_xp, d_status);
                 launches += 3;
             }
-            ba_point_update_kernel<<<pb, 128, 0, st>>>(g, d_blk, d_Hll, d_bl, lambda, d_xp, d_pts[cur], d_pts[nxt], d_part);
+            ba_point_update_kernel<<<pb, 128, 0, st>>>(g, d_blk, d_Hll, d_bl, lambda, d_xp, d_status, d_pts[cur], d_pts[nxt], d_part);
             ba_final_sum_kernel<<<1, 256, 0, st>>>(d_part, pb, d_scal + 2);
             ba_pose_update_kernel<<<qb, 128, 0, st>>>(g, lambda, d_xp, d_bp, d_pose[cur], d_pose[nxt], d_part + n_part);
             ba_final_sum_kernel<<<1, 256, 0, st>>>(d_part + n_part, qb, d_scal + 3);

@@ -36,8 +36,7 @@ def test_partial_iterations_and_empty_graph(ctx):
         rpo, rpt, rer, rit, _ = oracle.local_bundle_adjustment(*D.args(p), iterations=k)
         gpo, gpt, ger, git = F.local_bundle_adjustment(ctx, *D.args(p), iterations=k)
         assert git == rit and np.abs(gpo - rpo).max() < 1e-4 and np.abs(gpt - rpt).max() < 1e-3
-        if k:
-            assert np.array_equal(ger, rer)
+        assert np.array_equal(ger, rer)
     none = (p["poses"], p["pose_fixed"], p["points"], np.zeros(0, np.int32), np.zeros(0, np.int32), np.zeros((0, 3), np.float32),
             np.zeros(0, np.uint8), np.zeros(0, np.float32), *p["cam"])
     gpo, gpt, ger, git = F.local_bundle_adjustment(ctx, *none)
