@@ -443,8 +443,9 @@ int rgbl_track_sequence_stereo(rgbl_ctx* ctx, float mb, float mbf, const rgbl_ch
  * partial set of NULLs, map_stride < width or a value that is not finite is RGBL_E_INVALID and the previous setting stays.
  * While rectification is on, the stereo entry points take the RAW images at the context's size (Settings without resize): uploads and
  * PNG decodes keep them in raw planes, staged slots hold them as they always do, and rgbl_resident_process_stereo / the stereo runner
- * remap both images of every pair into level 0 before the extraction, billed to the `pyramid` profiling stage.  PNG streams must then
- * be 8-bit gray (colour: RGBL_E_UNSUPPORTED, since the reference remaps before its conversion to gray).  The camera model
+ * remap both images of every pair into level 0 before the extraction, billed to the `pyramid` profiling stage.  On a gray context PNG
+ * streams must then be 8-bit gray (colour: RGBL_E_UNSUPPORTED, since the reference remaps before its conversion to gray); a colour context
+ * (rgbl_set_input_channels) accepts colour streams and converts them after the remap.  The camera model
  * (rgbl_set_camera_distortion) keeps describing the rectified images, so it stays k1 = 0; mb / mbf and the chain's camera are the
  * rectified ones (Settings: P1's intrinsics, bf = b * P1(0,0)).  Setting or clearing the maps discards a pending stereo upload (the process
  * call then reports "nothing uploaded"); staged slots stay valid.                                                                       */
@@ -463,7 +464,8 @@ int rgbl_set_stereo_rectification(rgbl_ctx* ctx, const float* m1l, const float* 
  *     context-size depth plane of the gather (on the aux stream, billed to `depth_gather`).  Both are bit-exact with OpenCV;
  *   - RGB-D needs integer factors (src_width % width == 0 and src_height % height == 0; else RGBL_E_UNSUPPORTED), the case OpenCV's
  *     16-bit linear resize is restated for; stereo and 8-bit images take any downscale;
- *   - image PNG streams must be 8-bit gray (colour: RGBL_E_UNSUPPORTED: the reference resizes before its conversion to gray);
+ *   - on a gray context image PNG streams must be 8-bit gray (colour: RGBL_E_UNSUPPORTED: the reference resizes before its conversion to
+ *     gray); a colour context (rgbl_set_input_channels) accepts colour streams and converts them after the resize;
  *   - a staged slot holds input-size planes and records the input size: a runner given a slot staged at another size returns
  *     RGBL_E_INVALID;
  *   - every RGB-L entry point (uploads, _kitti, _kitti_png, stage, process, rgbl_track_sequence, rgbl_frame_rgbl_batch) returns
@@ -472,6 +474,22 @@ int rgbl_set_stereo_rectification(rgbl_ctx* ctx, const float* m1l, const float* 
  *     coordinates index the input-size images (Settings builds them for newImSize);
  *   - rgbl_decode_png_gray / rgbl_decode_png_depth16, rgbl_orb_extract* and the depth-from-map / point-cloud calls keep the context's size. */
 int rgbl_set_input_resize(rgbl_ctx* ctx, int src_width, int src_height);
+/* Colour camera input on the device: the cvtColor of Tracking::GrabImageRGBL, GrabImageRGBD and GrabImageStereo (src/Tracking.cc:1518 ff.,
+ * 1567-1580).  channels 3 or 4: the image arguments of the camera-input entry points are interleaved 8-bit images of `channels` bytes per
+ * pixel in the cv::Mat's memory order, `stride` in bytes (>= width * channels).  Those entry points keep their signatures: the RGB-L, RGB-D
+ * and stereo uploads, the three rgbl_resident_stage* calls and the host mode of rgbl_track_sequence / _rgbd / _stereo.  camera_rgb =
+ * Camera.RGB (mbRGB): 1 -> COLOR_RGB2GRAY / RGBA2GRAY (channel 0 weighted as red), 0 -> COLOR_BGR2GRAY / BGRA2GRAY (channel 0 weighted as
+ * blue); alpha is ignored.  The conversion is bit-exact with OpenCV and runs where level 0 is written (billed to the `pyramid` stage): alone,
+ * or after the input resize (rgbl_set_input_resize) or the stereo remap (rgbl_set_stereo_rectification) in the same kernel, which then
+ * interpolate each colour channel first, as the reference does.  channels 1 (the default): 8-bit gray images.
+ * channels not 1 / 3 / 4, camera_rgb not 0 / 1 or a chain in flight is RGBL_E_INVALID, and a refused call leaves the previous setting in
+ * place.  Setting or clearing the value discards a pending upload of any kind.  A staged slot records the channel count it was staged with:
+ * a runner given a slot staged with another count returns RGBL_E_INVALID.
+ * PNG uploads keep their per-call camera_rgb and decode what the stream holds; with a raw stage (the resize, the rectification) a colour
+ * context accepts colour streams, whose reconstructed pixels are converted to gray after the interpolation.
+ * Unaffected (8-bit gray, CV_8UC1, as ORBextractor::operator() asserts): rgbl_orb_extract*, rgbl_frame_rgbl_batch, rgbl_decode_png_gray and
+ * the depth calls.                                                                                                                       */
+int rgbl_set_input_channels(rgbl_ctx* ctx, int channels /* 1 (default), 3 or 4 */, int camera_rgb /* Camera.RGB: 0 or 1 */);
 
 /* ---- Camera model of Frame::UndistortKeyPoints / ComputeImageBounds (src/Frame.cc:837-899) for every later batched frame construction
  * (rgbl_frame_rgbl_batch, rgbl_resident_process, rgbl_resident_process_rgbd, both sequence runners) and tracking chain of this context:

@@ -185,10 +185,10 @@ void prof_collect(Ctx* c) {
 // Stage 2 (host):   quad-tree per (frame, level) on worker threads -> SelKp lists.
 // Stage 3 (device): describe.  Results stay in d_kps / d_desc (copied out by the callers).
 
-// The image planes of a batch: plane f at base + f * stride + off, rows pitch bytes apart, w x h pixels.  raw: the planes are the source of
-// the kernel that writes level 0 (the remap of stereo pairs with rectification on, or the input resize), not level 0.
+// The image planes of a batch: plane f at base + f * stride + off, rows pitch bytes apart, w x h pixels of ch bytes.  raw: the planes are the
+// source of the kernel that writes level 0 (the remap of stereo pairs with rectification on, the input resize, the gray conversion), not level 0.
 struct Planes {
-    uint8_t* base; size_t stride, off; int pitch; bool raw; int w, h;
+    uint8_t* base; size_t stride, off; int pitch; bool raw; int w, h; int ch = 1;
     uint8_t* at(int f) const { return base + (size_t)f * stride + off; }
 };
 
@@ -199,7 +199,7 @@ static Planes level0_planes(const Ctx* c) {
 // H2D of n host images into planes [first, first + n) of dst, on stream st
 static int upload_planes(Ctx* c, const Planes& dst, int first, int n, const uint8_t* const* img, int stride, cudaStream_t st) {
     for (int f = 0; f < n; ++f)
-        CU(cudaMemcpy2DAsync(dst.at(first + f), dst.pitch, img[f], stride, dst.w, dst.h, cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpy2DAsync(dst.at(first + f), dst.pitch, img[f], stride, (size_t)dst.w * dst.ch, dst.h, cudaMemcpyHostToDevice, st));
     return RGBL_OK;
 }
 
@@ -690,10 +690,11 @@ int rgbl_depth_from_map(rgbl_ctx* ctx, const float* depth_map, int width, int he
     return RGBL_OK;
 }
 
-// input_size: the images are camera input (the input size, rgbl_set_input_resize), else they have the context's size
-static int check_batch_args(Ctx* c, int n_frames, int width, int height, int stride, bool input_size = true) {
+// input_size: the images are camera input (the input size, rgbl_set_input_resize), else they have the context's size; ch: their bytes per pixel
+static int check_batch_args(Ctx* c, int n_frames, int width, int height, int stride, bool input_size = true, int ch = 1) {
     if (width <= 0 || height <= 0) { c->err = "empty image"; return RGBL_E_EMPTY; }
     const bool rs = input_size && c->resize;
+    if (ch > 1 && stride < width * ch) { c->err = "stride < width * channels (rgbl_set_input_channels)"; return RGBL_E_INVALID; }
     if (width != (rs ? c->in_w : c->cfg.width) || height != (rs ? c->in_h : c->cfg.height) || stride < width) {
         c->err = rs ? "image size does not match the input size (rgbl_set_input_resize)" : "image size does not match the context"; return RGBL_E_INVALID;
     }
@@ -719,13 +720,14 @@ static void set_resident(Ctx* c, InputKind kind, int n, int max_pts) {
 // one batch of host inputs of one kind: n frames (RGB-L, RGB-D) or n pairs (stereo, the right images in `right`).  RGB-L clouds:
 // layout 0 planar 4 x N rows (x, y, z, 1) as LoadPointcloudBinaryMat builds them; layout 1 the raw KITTI .bin records (x, y, z,
 // reflectance) x N, de-interleaved on the device (the 4th row becomes 1, Examples/RGB-L/rgbl_kitti.cc:168-177).  gray == nullptr: the
-// images are already on the device (PNG decode).
+// images are already on the device (PNG decode).  ch: bytes per pixel of the images (camera(): the context's colour input setting).
 struct HostInputs {
     InputKind kind;
     int n;
     const uint8_t* const* gray; const uint8_t* const* right; int stride;
     const float* const* pts; const int* n_pts; int layout;
     const uint16_t* const* depth; int depth_stride;
+    int ch = 1;
 
     static HostInputs rgbl(int n, const uint8_t* const* gray, int stride, const float* const* pts, const int* n_pts, int layout = 0) {
         return {InputKind::rgbl, n, gray, nullptr, stride, pts, n_pts, layout, nullptr, 0};
@@ -736,6 +738,8 @@ struct HostInputs {
     static HostInputs stereo(int n, const uint8_t* const* left, const uint8_t* const* right, int stride) {
         return {InputKind::stereo, n, left, right, stride, nullptr, nullptr, 0, nullptr, 0};
     }
+    // the images are camera input, of the context's channel count (rgbl_set_input_channels)
+    HostInputs camera(const Ctx* c) const { HostInputs r = *this; r.ch = c->in_ch; return r; }
     // batch b of consecutive batches of n
     HostInputs batch(int b) const {
         const size_t o = (size_t)b * n;
@@ -814,38 +818,54 @@ static int png_status(Ctx* c, cudaStream_t st) {
     return RGBL_OK;
 }
 
-// one raw image plane: level 0's layout at the input size (in_w x in_h, row pitch in_pitch) without the frame slot around it
+// the row pitch of an input-size image of ch bytes per pixel (64-byte rows); in_pitch = input_pitch(c, in_ch)
+static int input_pitch(const Ctx* c, int ch) { return (c->in_w * ch + 63) & ~63; }
+// one image plane of a stage slot: an input-size image of the context's channel count, without the frame slot around it
 static size_t raw_plane_bytes(const Ctx* c) { return (size_t)c->in_pitch * c->in_h; }
 
-// Where the image planes of the batch being loaded go: into stage slot `slot` if given, else level 0 of the frame slots.  With
-// rectification on (stereo pairs) or the input resize on (RGB-D frames, stereo pairs), process_stereo / process_rgbd write level 0 from
-// raw planes and nothing else writes it: the raw planes (raw_src) are the planes of the slot `staged` that already holds them (base ==
-// nullptr: nothing to copy), or else d_raw_img.
-static int image_planes(Ctx* c, InputKind kind, Ctx::StageSlot* slot, const Ctx::StageSlot* staged, Planes* p) {
-    const bool raw = (kind == InputKind::stereo && c->rectify) || (kind != InputKind::rgbl && c->resize);
-    if (slot) { *p = {slot->img, raw_plane_bytes(c), 0, c->in_pitch, raw, c->in_w, c->in_h}; return RGBL_OK; }
-    if (!raw) { *p = level0_planes(c); return RGBL_OK; }
-    if (staged) { c->raw_src = staged->img; *p = {nullptr, 0, 0, 0, true, 0, 0}; return RGBL_OK; }
-    if (!ensure(c->d_raw_img, c->cfg.max_batch * raw_plane_bytes(c))) { c->err = "device allocation failed (raw image planes)"; return RGBL_E_CUDA; }
-    c->raw_src = c->d_raw_img;
-    *p = {c->d_raw_img, raw_plane_bytes(c), 0, c->in_pitch, true, c->in_w, c->in_h};
+// the input of `kind` goes through a kernel that reads the whole image before level 0 is written: System::TrackStereo's remap (stereo
+// pairs, rectification on) or TrackRGBD's / TrackStereo's resize (input resize on)
+static bool raw_stage(const Ctx* c, InputKind kind) { return (kind == InputKind::stereo && c->rectify) || (kind != InputKind::rgbl && c->resize); }
+
+// Where the image planes (ch bytes per pixel) of the batch being loaded go: into stage slot `slot` if given, else level 0 of the frame slots.
+// With a raw stage (raw_stage) or colour images, process_* write level 0 from raw planes and nothing else writes it: the raw planes
+// (raw_src) are the planes of the slot `staged` that already holds them (base == nullptr: nothing to copy), or else d_raw_img.  Records
+// what the raw planes hold (raw_ch, raw_w0 = the context's weight, raw_pitch).
+static int image_planes(Ctx* c, InputKind kind, int ch, Ctx::StageSlot* slot, const Ctx::StageSlot* staged, Planes* p) {
+    const bool raw = ch > 1 || raw_stage(c, kind);
+    if (slot) { *p = {slot->img, raw_plane_bytes(c), 0, c->in_pitch, raw, c->in_w, c->in_h, ch}; return RGBL_OK; }
+    if (!raw) { *p = level0_planes(c); c->raw_ch = 0; return RGBL_OK; }
+    const int pitch = staged ? c->in_pitch : input_pitch(c, ch);
+    if (staged) *p = {nullptr, 0, 0, 0, true, 0, 0};
+    else if (!ensure(c->d_raw_img, (size_t)c->cfg.max_batch * pitch * c->in_h)) { c->err = "device allocation failed (raw image planes)"; return RGBL_E_CUDA; }
+    else *p = {c->d_raw_img, (size_t)pitch * c->in_h, 0, pitch, true, c->in_w, c->in_h, ch};
+    c->raw_src = staged ? staged->img.get() : c->d_raw_img.get();
+    c->raw_ch = ch; c->raw_w0 = c->in_w0; c->raw_pitch = pitch;
     return RGBL_OK;
 }
 
-// n PNG streams into the image planes of the batch being loaded (image_planes); raw planes take 8-bit gray streams only, since the
-// reference remaps or resizes the image imread returned and converts it to gray afterwards, which differs for colour images
+// n PNG streams into the image planes of the batch being loaded (image_planes).  Without a raw stage the unfilter kernel converts to gray
+// and writes level 0.  With one, the reference remaps or resizes the image imread returned and converts it to gray afterwards, which differs
+// for colour images: the raw planes then take the reconstructed pixels as they are, colour streams on a colour context only (a gray
+// context refuses them).  The file's samples are in R, G, B order, imread's in B, G, R: channel 0 gets the red weight when camera_rgb is 0.
 static int decode_png_gray(Ctx* c, InputKind kind, int n_frames, const uint8_t* const* png, const size_t* png_bytes, int camera_rgb, cudaStream_t st) {
-    Planes p;
-    int rc = image_planes(c, kind, nullptr, nullptr, &p); if (rc) return rc;
-    const char* gray_only = !p.raw ? nullptr
-                          : kind == InputKind::stereo && c->rectify ? "rectified stereo takes 8-bit gray PNGs only (the reference remaps colour images before their conversion to gray)"
-                                                                    : "with the input resize on, image PNGs must be 8-bit gray (the reference resizes colour images before their conversion to gray)";
-    const int ch = inflate_png_batch(c, n_frames, png, png_bytes, p.w, p.h, false, st, gray_only);
+    const bool raw = raw_stage(c, kind);
+    const char* gray_only = !raw || c->in_ch > 1 ? nullptr
+                          : kind == InputKind::stereo && c->rectify ? "rectified stereo takes 8-bit gray PNGs only on a gray context (the reference remaps colour images before their conversion to gray; rgbl_set_input_channels)"
+                                                                    : "with the input resize on, image PNGs must be 8-bit gray on a gray context (the reference resizes colour images before their conversion to gray; rgbl_set_input_channels)";
+    const int ch = inflate_png_batch(c, n_frames, png, png_bytes, raw ? c->in_w : c->cfg.width, raw ? c->in_h : c->cfg.height, false, st, gray_only);
     if (ch < 0) return ch;
-    LevelGeom g = c->levels[0];
-    g.off = p.off; g.pitch = p.pitch;
-    launch_png_unfilter_gray(st, c->d_png_raw, c->png_raw_stride, p.w, p.h, ch, p.raw ? 0 : camera_rgb, p.base, p.stride, g,
-                             c->d_png_band, c->d_png_status, n_frames);
+    Planes p;
+    int rc = image_planes(c, kind, raw ? ch : 1, nullptr, nullptr, &p); if (rc) return rc;
+    if (p.ch > 1) {
+        launch_png_unfilter_pixels(st, c->d_png_raw, c->png_raw_stride, p.w, p.h, ch, p.base, p.stride, p.pitch, c->d_png_band, c->d_png_status, n_frames);
+        c->raw_w0 = camera_rgb ? 3735 : 9798;
+    } else {
+        LevelGeom g = c->levels[0];
+        g.off = p.off; g.pitch = p.pitch;
+        launch_png_unfilter_gray(st, c->d_png_raw, c->png_raw_stride, p.w, p.h, ch, p.raw ? 0 : camera_rgb, p.base, p.stride, g,
+                                 c->d_png_band, c->d_png_status, n_frames);
+    }
     return png_status(c, st);
 }
 
@@ -911,7 +931,7 @@ static int copy_inputs(Ctx* c, const HostInputs& in, int max_pts, Ctx::StageSlot
     }
     if (!in.gray) return RGBL_OK;          // level 0 was written by a PNG decode
     Planes p;
-    int rc = image_planes(c, in.kind, slot, nullptr, &p); if (rc) return rc;
+    int rc = image_planes(c, in.kind, in.ch, slot, nullptr, &p); if (rc) return rc;
     rc = upload_planes(c, p, 0, in.n, in.gray, in.stride, c->st); if (rc) return rc;
     return in.right ? upload_planes(c, p, in.n, in.n, in.right, in.stride, c->st) : RGBL_OK;
 }
@@ -941,30 +961,57 @@ static int stage_inputs(Ctx* c, int slot, const HostInputs& in) {
     rc = copy_inputs(c, in, max_pts, &sl); if (rc) return rc;
     CU(cudaStreamSynchronize(c->st));
     CU(cudaStreamSynchronize(c->st_aux));
-    sl.n_frames = in.n; sl.max_pts = max_pts; sl.kind = in.kind; sl.in_w = c->in_w; sl.in_h = c->in_h;
+    sl.n_frames = in.n; sl.max_pts = max_pts; sl.kind = in.kind; sl.in_w = c->in_w; sl.in_h = c->in_h; sl.ch = in.ch;
     return RGBL_OK;
 }
 
-// Everything of Frame::Frame (RGB-L) after the inputs are in HBM: depth maps (aux stream) || extraction, then gather.
+// The level0 step of run_extract for the n images of the uploaded batch (stereo: n / 2 pairs, left then right), on the main stream: the raw
+// planes remapped (System::TrackStereo's cv::remap, stereo pairs with rectification on), else resized (TrackRGBD's / TrackStereo's
+// cv::resize, input resize on), else converted to gray (Tracking::GrabImage*'s cvtColor of colour input) into level 0 of frame slots
+// [0, n); colour planes are converted to gray after the remap or the resize, in the same kernel.  *step = nullptr when the upload wrote
+// level 0 itself.  With the rectification and the resize both on, the remap alone reads the input-size planes: the maps have the
+// context's size and their coordinates index the input-size images (Settings builds them with initUndistortRectifyMap(..., newImSize_, ...)).
+static int level0_step(Ctx* c, InputKind kind, int n, std::function<int()>* step) {
+    const bool remap = kind == InputKind::stereo && c->rectify, resize = raw_stage(c, kind) && !remap;
+    *step = nullptr;
+    if (!remap && !resize && !c->raw_ch) return RGBL_OK;
+    if (!c->raw_src || !c->raw_ch) { c->err = remap ? "no raw stereo planes to rectify" : "no input-size planes to resize"; return RGBL_E_INVALID; }
+    *step = [c, n, remap, resize]() {
+        const size_t stride = (size_t)c->raw_pitch * c->in_h;
+        LevelGeom src{};
+        src.w = c->in_w; src.h = c->in_h; src.pitch = c->raw_pitch;
+        if (remap) {
+            const LevelGeom& l0 = c->levels[0];
+            RectifyDev r{};
+            r.xy = c->d_rect_xy; r.a = c->d_rect_a; r.map_pitch = c->rect_pitch;
+            r.W = c->cfg.width; r.H = c->cfg.height; r.src_W = c->in_w; r.src_H = c->in_h;
+            r.src = c->raw_src; r.src_stride = stride; r.src_pitch = c->raw_pitch; r.ch = c->raw_ch; r.w0 = c->raw_w0;
+            r.dst = c->d_pyr; r.dst_stride = c->frame_bytes; r.dst_off = l0.off; r.dst_pitch = l0.pitch;
+            launch_rectify(c->st, r, n / 2);
+        } else if (resize) {
+            launch_resize_planes(c->st, c->raw_src, stride, src, c->d_pyr, c->frame_bytes, c->levels[0], c->d_resize_coefs,
+                                 c->d_resize_coefs + c->cfg.width, n, c->raw_ch, c->raw_w0);
+        } else {
+            launch_gray_planes(c->st, c->raw_src, stride, src, c->d_pyr, c->frame_bytes, c->levels[0], c->raw_ch, c->raw_w0, n);
+        }
+        return 1;
+    };
+    return RGBL_OK;
+}
+
+// Everything of Frame::Frame (RGB-L) after the inputs are in HBM: (colour input: the gray conversion into level 0), depth maps (aux
+// stream) || extraction, then gather.
 static int process_rgbl(Ctx* c, int n_frames, int max_pts, const float P[12], const rgbl_depth_params* prm) {
     DepthDev dd;
     int rc = setup_depth(c, P, prm, dd); if (rc) return rc;
+    std::function<int()> level0;
+    rc = level0_step(c, InputKind::rgbl, n_frames, &level0); if (rc) return rc;
     // depth maps run on the aux stream behind the blur, overlapping the host quad-tree; describe waits for both
-    int max_n = run_extract(c, n_frames, [&]() { run_depth_maps(c, dd, n_frames, max_pts, nullptr, c->st_aux); });
+    int max_n = run_extract(c, n_frames, [&]() { run_depth_maps(c, dd, n_frames, max_pts, nullptr, c->st_aux); }, level0);
     if (max_n < 0) return max_n;
     run_depth_keypoints(c, dd, c->d_kps, c->d_kps, c->d_n_sel, max_n, n_frames, c->st, true);
     CU(cudaGetLastError());
     return max_n;
-}
-
-// System::TrackStereo's / TrackRGBD's cv::resize(im, im, newImSize) of the n raw planes (raw_src, in_w x in_h) into level 0 of frame slots
-// [0, n), on the main stream (a level0 step of run_extract) -> its launch count
-static int resize_images(Ctx* c, int n) {
-    LevelGeom src{};
-    src.w = c->in_w; src.h = c->in_h; src.pitch = c->in_pitch;
-    launch_resize_planes(c->st, c->raw_src, raw_plane_bytes(c), src, c->d_pyr, c->frame_bytes, c->levels[0], c->d_resize_coefs,
-                         c->d_resize_coefs + c->cfg.width, n);
-    return 1;
 }
 
 // Everything of the RGB-D Frame constructor (src/Frame.cc:200-237) after the inputs are in HBM: extraction, UndistortKeyPoints (context's
@@ -975,9 +1022,9 @@ static int resize_images(Ctx* c, int n) {
 static int process_rgbd(Ctx* c, int n_frames, float depth_scale, float bf) {
     std::function<int()> level0;
     std::function<void()> depth_resize;
+    int rc = level0_step(c, InputKind::rgbd, n_frames, &level0); if (rc) return rc;
     if (c->resize) {
-        if (!c->raw_src || !c->depth_src) { c->err = "no input-size planes to resize"; return RGBL_E_INVALID; }
-        level0 = [&]() { return resize_images(c, n_frames); };
+        if (!c->depth_src) { c->err = "no input-size planes to resize"; return RGBL_E_INVALID; }
         depth_resize = [&]() {
             if (c->prof_on) cudaEventRecord(c->ev_rsd_b, c->st_aux);
             launch_resize_depth16(c->st_aux, c->depth_src, depth16_in_frame_elems(c), c->depth16_raw_pitch, c->resize_kx, c->resize_ky, c->d_depth16,
@@ -1010,28 +1057,14 @@ static int check_rgbd_params(Ctx* c, float depth_scale, float bf) {
 // so an overflow in a right frame, which changes the left frame's depths, fails the chain's _end2 like a left-frame overflow.
 // With rectification on, the raw planes of the pairs (raw_src) are first remapped into level 0 of the slots, in one launch billed to the
 // pyramid stage: System::TrackStereo's cv::remap of both images (src/System.cc:251 ff.).  Else, with the input resize on, they are resized
-// into level 0 in the same way (TrackStereo's cv::resize, the branch after the rectification's).  With both on, the remap alone reads the
-// input-size planes: the maps have the context's size and their coordinates index the input-size images (Settings builds them with
-// initUndistortRectifyMap(..., newImSize_, ...)).
+// into level 0 in the same way (TrackStereo's cv::resize, the branch after the rectification's); colour pairs are converted to gray
+// after either, or alone (level0_step).
 static int process_stereo(Ctx* c, int n_pairs, float mb, float mbf) {
     std::function<int()> level0;
-    if (c->rectify || c->resize) {
-        if (!c->raw_src) { c->err = c->rectify ? "no raw stereo planes to rectify" : "no input-size planes to resize"; return RGBL_E_INVALID; }
-        if (!c->rectify) level0 = [&]() { return resize_images(c, 2 * n_pairs); };
-        else level0 = [&]() {
-            const LevelGeom& l0 = c->levels[0];
-            RectifyDev r{};
-            r.xy = c->d_rect_xy; r.a = c->d_rect_a; r.map_pitch = c->rect_pitch;
-            r.W = c->cfg.width; r.H = c->cfg.height; r.src_W = c->in_w; r.src_H = c->in_h;
-            r.src = c->raw_src; r.src_stride = raw_plane_bytes(c); r.src_pitch = c->in_pitch;
-            r.dst = c->d_pyr; r.dst_stride = c->frame_bytes; r.dst_off = l0.off; r.dst_pitch = l0.pitch;
-            launch_rectify(c->st, r, n_pairs);
-            return 1;
-        };
-    }
+    int rc = level0_step(c, InputKind::stereo, 2 * n_pairs, &level0); if (rc) return rc;
     const int max_n = run_extract(c, 2 * n_pairs, nullptr, level0);
     if (max_n < 0) return max_n;
-    int rc = stereo_matches(c, 0, n_pairs, n_pairs, mb, mbf); if (rc) return rc;
+    rc = stereo_matches(c, 0, n_pairs, n_pairs, mb, mbf); if (rc) return rc;
     c->last_frames = n_pairs;
     return max_n;
 }
@@ -1123,9 +1156,9 @@ int rgbl_resident_upload(rgbl_ctx* ctx, int n_frames, const uint8_t* const* gray
     if (!c) return RGBL_E_INVALID;
     if (!gray || !pts4xn || !n_pts) { c->err = "null argument"; return RGBL_E_INVALID; }
     int rc = check_rgbl_input(c); if (rc) return rc;
-    rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
+    rc = check_batch_args(c, n_frames, width, height, stride, true, c->in_ch); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
-    return upload_inputs_sync(c, HostInputs::rgbl(n_frames, gray, stride, pts4xn, n_pts));
+    return upload_inputs_sync(c, HostInputs::rgbl(n_frames, gray, stride, pts4xn, n_pts).camera(c));
 }
 
 int rgbl_resident_upload_kitti(rgbl_ctx* ctx, int n_frames, const uint8_t* const* gray, int width, int height, int stride,
@@ -1134,9 +1167,9 @@ int rgbl_resident_upload_kitti(rgbl_ctx* ctx, int n_frames, const uint8_t* const
     if (!c) return RGBL_E_INVALID;
     if (!gray || !xyzr || !n_pts) { c->err = "null argument"; return RGBL_E_INVALID; }
     int rc = check_rgbl_input(c); if (rc) return rc;
-    rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
+    rc = check_batch_args(c, n_frames, width, height, stride, true, c->in_ch); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
-    return upload_inputs_sync(c, HostInputs::rgbl(n_frames, gray, stride, xyzr, n_pts, 1));
+    return upload_inputs_sync(c, HostInputs::rgbl(n_frames, gray, stride, xyzr, n_pts, 1).camera(c));
 }
 
 int rgbl_resident_upload_kitti_png(rgbl_ctx* ctx, int n_frames, const uint8_t* const* png, const size_t* png_bytes, int camera_rgb,
@@ -1193,9 +1226,9 @@ int rgbl_resident_stage(rgbl_ctx* ctx, int slot, int n_frames, const uint8_t* co
     if (slot < 0 || slot >= Ctx::kMaxStageSlots) { c->err = "stage slot out of range"; return RGBL_E_INVALID; }
     if (!c->d_pts) { c->err = "context was created with max_points == 0"; return RGBL_E_INVALID; }
     int rc = check_rgbl_input(c); if (rc) return rc;
-    rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
+    rc = check_batch_args(c, n_frames, width, height, stride, true, c->in_ch); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
-    return stage_inputs(c, slot, HostInputs::rgbl(n_frames, gray, stride, pts4xn, n_pts));
+    return stage_inputs(c, slot, HostInputs::rgbl(n_frames, gray, stride, pts4xn, n_pts).camera(c));
 }
 
 int rgbl_resident_stage_rgbd(rgbl_ctx* ctx, int slot, int n_frames, const uint8_t* const* gray, int width, int height, int stride,
@@ -1205,10 +1238,10 @@ int rgbl_resident_stage_rgbd(rgbl_ctx* ctx, int slot, int n_frames, const uint8_
     if (!gray || !depth) { c->err = "null argument"; return RGBL_E_INVALID; }
     if (slot < 0 || slot >= Ctx::kMaxStageSlots) { c->err = "stage slot out of range"; return RGBL_E_INVALID; }
     int rc = check_rgbd_input(c); if (rc) return rc;
-    rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
+    rc = check_batch_args(c, n_frames, width, height, stride, true, c->in_ch); if (rc) return rc;
     if (depth_stride < width) { c->err = "depth_stride < width"; return RGBL_E_INVALID; }
     CU(cudaSetDevice(c->cfg.device));
-    return stage_inputs(c, slot, HostInputs::rgbd(n_frames, gray, stride, depth, depth_stride));
+    return stage_inputs(c, slot, HostInputs::rgbd(n_frames, gray, stride, depth, depth_stride).camera(c));
 }
 
 int rgbl_resident_stage_stereo(rgbl_ctx* ctx, int slot, int n_pairs, const uint8_t* const* left, const uint8_t* const* right, int width, int height,
@@ -1217,10 +1250,10 @@ int rgbl_resident_stage_stereo(rgbl_ctx* ctx, int slot, int n_pairs, const uint8
     if (!c) return RGBL_E_INVALID;
     if (!left || !right) { c->err = "null argument"; return RGBL_E_INVALID; }
     if (slot < 0 || slot >= Ctx::kMaxStageSlots) { c->err = "stage slot out of range"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_pairs, width, height, stride); if (rc) return rc;
+    int rc = check_batch_args(c, n_pairs, width, height, stride, true, c->in_ch); if (rc) return rc;
     rc = check_stereo(c, n_pairs); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
-    return stage_inputs(c, slot, HostInputs::stereo(n_pairs, left, right, stride));
+    return stage_inputs(c, slot, HostInputs::stereo(n_pairs, left, right, stride).camera(c));
 }
 
 // staged slot -> the context's working input buffers (device-to-device, ~76 MB per 32 KITTI frames: tens of microseconds); the slot must hold
@@ -1234,8 +1267,9 @@ static int restage(Ctx* c, int slot, InputKind kind) {
         return RGBL_E_INVALID;
     }
     if (sl.in_w != c->in_w || sl.in_h != c->in_h) { c->err = "stage slot was staged at another input size (rgbl_set_input_resize)"; return RGBL_E_INVALID; }
+    if (sl.ch != c->in_ch) { c->err = "stage slot was staged with another channel count (rgbl_set_input_channels)"; return RGBL_E_INVALID; }
     Planes dst;
-    int rc = image_planes(c, kind, nullptr, &sl, &dst); if (rc) return rc;
+    int rc = image_planes(c, kind, sl.ch, nullptr, &sl, &dst); if (rc) return rc;
     const size_t img_bytes = raw_plane_bytes(c);
     const int n_img = kind == InputKind::stereo ? 2 * sl.n_frames : sl.n_frames;
     if (dst.base)
@@ -1259,7 +1293,7 @@ static int check_sequence_io(Ctx* c, const rgbl_chain_params* chain, const rgbl_
     if (T < 1 || T > c->cfg.max_batch || nb < 1) { c->err = "bad batch geometry"; return RGBL_E_INVALID; }
     if (const int rc = require_idle(c)) return rc;
     if (io->gray) {
-        int rc = check_batch_args(c, T, io->width, io->height, io->stride); if (rc) return rc;
+        int rc = check_batch_args(c, T, io->width, io->height, io->stride, true, c->in_ch); if (rc) return rc;
     } else if (io->n_slots < 1 || io->n_slots > Ctx::kMaxStageSlots) { c->err = "resident mode needs 1..8 staged slots"; return RGBL_E_INVALID; }
     if (io->kps && (!io->desc || !io->depth || !io->uright || !io->n_kp || io->cap != c->cap_kp)) {
         c->err = "frame outputs need kps, desc, depth, uright, n_kp and cap == rgbl_keypoint_capacity()"; return RGBL_E_INVALID;
@@ -1326,7 +1360,7 @@ int rgbl_track_sequence(rgbl_ctx* ctx, const float P[12], const rgbl_depth_param
     if (io->gray && (!io->pts4xn || !io->n_pts)) { c->err = "null argument"; return RGBL_E_INVALID; }
     CU(cudaSetDevice(c->cfg.device));
     const int T = io->frames_per_batch;
-    const auto load = batch_loader(c, io, HostInputs::rgbl(T, io->gray, io->stride, io->pts4xn, io->n_pts));
+    const auto load = batch_loader(c, io, HostInputs::rgbl(T, io->gray, io->stride, io->pts4xn, io->n_pts).camera(c));
     return run_sequence(c, chain, io, load, [&]() { return process_rgbl(c, T, c->resident_max_pts, P, prm); });
 }
 
@@ -1341,7 +1375,7 @@ int rgbl_track_sequence_rgbd(rgbl_ctx* ctx, float depth_scale, float bf, const r
     if (io->gray && (!depth || depth_stride < io->width)) { c->err = "host mode needs one depth image per frame and depth_stride >= width"; return RGBL_E_INVALID; }
     CU(cudaSetDevice(c->cfg.device));
     const int T = io->frames_per_batch;
-    const auto load = batch_loader(c, io, HostInputs::rgbd(T, io->gray, io->stride, depth, depth_stride));
+    const auto load = batch_loader(c, io, HostInputs::rgbd(T, io->gray, io->stride, depth, depth_stride).camera(c));
     return run_sequence(c, chain, io, load, [&]() { return process_rgbd(c, T, depth_scale, bf); });
 }
 
@@ -1355,7 +1389,7 @@ int rgbl_track_sequence_stereo(rgbl_ctx* ctx, float mb, float mbf, const rgbl_ch
     if (io->gray && !right) { c->err = "host mode needs one right image per frame"; return RGBL_E_INVALID; }
     CU(cudaSetDevice(c->cfg.device));
     const int T = io->frames_per_batch;
-    const auto load = batch_loader(c, io, HostInputs::stereo(T, io->gray, right, io->stride));
+    const auto load = batch_loader(c, io, HostInputs::stereo(T, io->gray, right, io->stride).camera(c));
     return run_sequence(c, chain, io, load, [&]() { return process_stereo(c, T, mb, mbf); });
 }
 
@@ -1366,9 +1400,9 @@ int rgbl_resident_upload_rgbd(rgbl_ctx* ctx, int n_frames, const uint8_t* const*
     if (!c) return RGBL_E_INVALID;
     if (!gray || !depth) { c->err = "null argument"; return RGBL_E_INVALID; }
     int rc = check_rgbd_input(c); if (rc) return rc;
-    rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
+    rc = check_batch_args(c, n_frames, width, height, stride, true, c->in_ch); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
-    return upload_inputs_sync(c, HostInputs::rgbd(n_frames, gray, stride, depth, depth_stride));
+    return upload_inputs_sync(c, HostInputs::rgbd(n_frames, gray, stride, depth, depth_stride).camera(c));
 }
 
 int rgbl_resident_upload_rgbd_png(rgbl_ctx* ctx, int n_frames, const uint8_t* const* png, const size_t* png_bytes, int camera_rgb,
@@ -1415,10 +1449,10 @@ int rgbl_resident_upload_stereo(rgbl_ctx* ctx, int n_pairs, const uint8_t* const
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
     if (!left || !right) { c->err = "null argument"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_pairs, width, height, stride); if (rc) return rc;
+    int rc = check_batch_args(c, n_pairs, width, height, stride, true, c->in_ch); if (rc) return rc;
     rc = check_stereo(c, n_pairs); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
-    return upload_inputs_sync(c, HostInputs::stereo(n_pairs, left, right, stride));
+    return upload_inputs_sync(c, HostInputs::stereo(n_pairs, left, right, stride).camera(c));
 }
 
 int rgbl_resident_upload_stereo_png(rgbl_ctx* ctx, int n_pairs, const uint8_t* const* left_png, const size_t* left_bytes, const uint8_t* const* right_png,
@@ -1514,10 +1548,25 @@ int rgbl_set_input_resize(rgbl_ctx* ctx, int src_width, int src_height) {
     }
     c->resize = on;
     c->in_w = on ? src_width : W; c->in_h = on ? src_height : H;
-    c->in_pitch = (c->in_w + 63) & ~63;
+    c->in_pitch = input_pitch(c, c->in_ch);
     c->resize_kx = c->in_w % W == 0 ? c->in_w / W : 0;
     c->resize_ky = c->in_h % H == 0 ? c->in_h / H : 0;
     c->depth16_raw_pitch = ((size_t)c->in_w * sizeof(uint16_t) + 63) / 64 * 32;
+    c->resident_frames = 0;                   // the uploaded batch was loaded for the other setting
+    return RGBL_OK;
+}
+
+// Tracking::GrabImageRGBL / GrabImageRGBD / GrabImageStereo's cvtColor of 3- and 4-channel camera images (src/Tracking.cc:1518 ff., 1567-1580).
+// Every check runs before anything is changed, so a refused setting leaves the previous one in place.
+int rgbl_set_input_channels(rgbl_ctx* ctx, int channels, int camera_rgb) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (const int rc = require_idle(c)) return rc;
+    if ((channels != 1 && channels != 3 && channels != 4) || (camera_rgb != 0 && camera_rgb != 1)) {
+        c->err = "channels must be 1, 3 or 4 and camera_rgb 0 or 1"; return RGBL_E_INVALID;
+    }
+    c->in_ch = channels;
+    c->in_w0 = camera_rgb ? 9798 : 3735;      // mbRGB: COLOR_RGB2GRAY weights channel 0 as red, COLOR_BGR2GRAY as blue
+    c->in_pitch = input_pitch(c, channels);
     c->resident_frames = 0;                   // the uploaded batch was loaded for the other setting
     return RGBL_OK;
 }

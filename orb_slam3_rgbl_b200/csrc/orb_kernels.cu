@@ -18,21 +18,43 @@ namespace rgbl {
 // the number of load instructions, not by HBM.)
 // Both kernels read plane z at src_base + z * src_stride + src.off and write plane z at dst_base + z * dst_stride + dst.off: the pyramid
 // passes its frame slots twice (level l-1 -> level l), the input resize the source-size raw planes and level 0 (launch_resize_planes).
-constexpr int kRzTW = 128, kRzTH = 16, kRzSrcRows = 24, kRzSrcVec = 12;     // staged source: 24 rows x 192 bytes max
+// CH > 1: the source planes are interleaved colour images of CH bytes per pixel (src.pitch in bytes); every channel is resized exactly as a
+// gray plane is (cv::resize of an 8UC3 / 8UC4 image equals the per-channel 8UC1 resize), and the 3 rounded channel values are converted to
+// gray (gray_of, channel 0 weighted w0) - System::TrackRGBD's / TrackStereo's resize of the colour image, then GrabImage*'s cvtColor, without
+// the resized colour image ever being written.  The staged tile holds CH times the bytes, so its ratio limit is the gray one.
+constexpr int kRzTW = 128, kRzTH = 16, kRzSrcRows = 24, kRzSrcVec = 12;     // staged source: 24 rows x 192 bytes (x CH) max
+
+// one output pixel from the source rows r0 / r1: left / right source pixel at byte offsets s0 / s1 (x CH), weights c0 / c1 (x), b0 / b1 (y)
+template <int CH>
+__device__ __forceinline__ uint32_t resize_px(const uint8_t* r0, const uint8_t* r1, int s0, int s1, int c0, int c1, int b0, int b1, uint32_t w0) {
+    constexpr int NC = CH == 1 ? 1 : 3;          // alpha is not read
+    uint32_t v[NC];
+#pragma unroll
+    for (int k = 0; k < NC; ++k) {
+        const int h0 = (int)r0[s0 + k] * c0 + (int)r0[s1 + k] * c1;
+        const int h1 = (int)r1[s0 + k] * c0 + (int)r1[s1 + k] * c1;
+        v[k] = (uint32_t)((((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2) & 0xffu;
+    }
+    if constexpr (CH == 1) return v[0];
+    else return gray_of(v[0], v[1], v[2], w0);
+}
+
+template <int CH>
 __global__ void __launch_bounds__(256) resize_level_kernel(const uint8_t* __restrict__ src_base, size_t src_stride, LevelGeom src,
                                                            uint8_t* __restrict__ dst_base, size_t dst_stride, LevelGeom dst,
                                                            const LinCoef* __restrict__ tabx,
-                                                           const LinCoef* __restrict__ taby) {
-    __shared__ uint4 tile[kRzSrcRows][kRzSrcVec];
+                                                           const LinCoef* __restrict__ taby, uint32_t w0) {
+    constexpr int kVec = kRzSrcVec * CH;
+    __shared__ uint4 tile[kRzSrcRows][kVec];
     const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
     const int x0 = blockIdx.x * kRzTW, y0 = blockIdx.y * kRzTH;
     const uint8_t* s = src_base + (size_t)blockIdx.z * src_stride + src.off;
     uint8_t* d = dst_base + (size_t)blockIdx.z * dst_stride + dst.off;
-    // source rectangle of this tile (tables are monotone)
+    // source rectangle of this tile (tables are monotone), in bytes
     const int xl = min(x0 + kRzTW - 1, dst.w - 1), yl = min(y0 + kRzTH - 1, dst.h - 1);
-    const int sx_lo = tabx[x0].s & ~15, sx_hi = min(tabx[xl].s + 1, src.w - 1);
+    const int sx_lo = (tabx[x0].s * CH) & ~15, sx_hi = min(tabx[xl].s + 1, src.w - 1) * CH + CH - 1;
     const int sy_lo = taby[y0].s, sy_hi = min(taby[yl].s + 1, src.h - 1);
-    const int n_vec = min(min((sx_hi - sx_lo) / 16 + 1, kRzSrcVec), (src.pitch - sx_lo) / 16);
+    const int n_vec = min(min((sx_hi - sx_lo) / 16 + 1, kVec), (src.pitch - sx_lo) / 16);
     const int n_rows = min(sy_hi - sy_lo + 1, kRzSrcRows);
     for (int i = tid; i < n_rows * n_vec; i += 256) {
         const int r = i / n_vec, v = i - r * n_vec;
@@ -42,12 +64,12 @@ __global__ void __launch_bounds__(256) resize_level_kernel(const uint8_t* __rest
     const int x4 = x0 + 4 * tx;
     if (x4 >= dst.w) return;
     const uint8_t* tb = reinterpret_cast<const uint8_t*>(&tile[0][0]);
-    constexpr int kTP = kRzSrcVec * 16;
+    constexpr int kTP = kVec * 16;
     int s0[4], s1[4], c0[4], c1[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
         const LinCoef cx = tabx[min(x4 + i, dst.w - 1)];
-        s0[i] = cx.s - sx_lo; s1[i] = min(cx.s + 1, src.w - 1) - sx_lo; c0[i] = cx.c0; c1[i] = cx.c1;
+        s0[i] = cx.s * CH - sx_lo; s1[i] = min(cx.s + 1, src.w - 1) * CH - sx_lo; c0[i] = cx.c0; c1[i] = cx.c1;
     }
 #pragma unroll
     for (int ry = 0; ry < 2; ++ry) {
@@ -56,27 +78,21 @@ __global__ void __launch_bounds__(256) resize_level_kernel(const uint8_t* __rest
         const LinCoef cy = taby[y];
         const uint8_t* r0 = tb + (cy.s - sy_lo) * kTP;
         const uint8_t* r1 = tb + (min(cy.s + 1, src.h - 1) - sy_lo) * kTP;
-        const int b0 = cy.c0, b1 = cy.c1;
         uint32_t out = 0;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            if (x4 + i < dst.w) {
-                const int h0 = (int)r0[s0[i]] * c0[i] + (int)r0[s1[i]] * c1[i];
-                const int h1 = (int)r1[s0[i]] * c0[i] + (int)r1[s1[i]] * c1[i];
-                const int v = (((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2;
-                out |= (uint32_t)(v & 0xff) << (8 * i);
-            }
-        }
+        for (int i = 0; i < 4; ++i)
+            if (x4 + i < dst.w) out |= resize_px<CH>(r0, r1, s0[i], s1[i], c0[i], c1[i], cy.c0, cy.c1, w0) << (8 * i);
         *reinterpret_cast<uint32_t*>(d + (size_t)y * dst.pitch + x4) = out;
     }
 }
 
 // Fallback for level ratios whose source rectangle does not fit the staged tile (scale factors above ~1.35): one thread
-// gathers the 16 source bytes of 4 adjacent outputs directly from global memory.
+// gathers the 16 source bytes (x CH) of 4 adjacent outputs directly from global memory.
+template <int CH>
 __global__ void __launch_bounds__(256) resize_level_gather_kernel(const uint8_t* __restrict__ src_base, size_t src_stride, LevelGeom src,
                                                                   uint8_t* __restrict__ dst_base, size_t dst_stride, LevelGeom dst,
                                                                   const LinCoef* __restrict__ tabx,
-                                                                  const LinCoef* __restrict__ taby) {
+                                                                  const LinCoef* __restrict__ taby, uint32_t w0) {
     const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
     const int y = blockIdx.y * blockDim.y + threadIdx.y;
     if (x4 >= dst.w || y >= dst.h) return;
@@ -85,21 +101,47 @@ __global__ void __launch_bounds__(256) resize_level_gather_kernel(const uint8_t*
     const LinCoef cy = taby[y];
     const uint8_t* r0 = s + (size_t)cy.s * src.pitch;
     const uint8_t* r1 = s + (size_t)min(cy.s + 1, src.h - 1) * src.pitch;
-    const int b0 = cy.c0, b1 = cy.c1;
     uint32_t out = 0;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
         const int x = x4 + i;
         if (x < dst.w) {
             const LinCoef cx = tabx[x];
-            const int s0 = cx.s, s1 = min(s0 + 1, src.w - 1);
-            const int h0 = (int)__ldg(r0 + s0) * cx.c0 + (int)__ldg(r0 + s1) * cx.c1;
-            const int h1 = (int)__ldg(r1 + s0) * cx.c0 + (int)__ldg(r1 + s1) * cx.c1;
-            const int v = (((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2;
-            out |= (uint32_t)(v & 0xff) << (8 * i);
+            out |= resize_px<CH>(r0, r1, cx.s * CH, min(cx.s + 1, src.w - 1) * CH, cx.c0, cx.c1, cy.c0, cy.c1, w0) << (8 * i);
         }
     }
     *reinterpret_cast<uint32_t*>(d + (size_t)y * dst.pitch + x4) = out;
+}
+
+// cvtColor of CH-channel planes into gray planes of the same size (the colour input without resize or remap): one thread per 4 pixels,
+// one 12- or 16-byte load (three 4-byte loads for CH = 3: a group starts 12-byte aligned) and one 32-bit store.  A row's last partial group
+// reads and writes single bytes, so neither the source row's end nor the destination row's padding is touched.
+template <int CH>
+__global__ void __launch_bounds__(256) gray_planes_kernel(const uint8_t* __restrict__ src_base, size_t src_stride, LevelGeom src,
+                                                          uint8_t* __restrict__ dst_base, size_t dst_stride, LevelGeom dst, uint32_t w0) {
+    const int x4 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
+    const int y = blockIdx.y * blockDim.y + threadIdx.y;
+    if (x4 >= dst.w || y >= dst.h) return;
+    const uint8_t* s = src_base + (size_t)blockIdx.z * src_stride + src.off + (size_t)y * src.pitch + (size_t)x4 * CH;
+    uint8_t* d = dst_base + (size_t)blockIdx.z * dst_stride + dst.off + (size_t)y * dst.pitch + x4;
+    const int n = min(4, dst.w - x4);
+    if (n == 4) {
+        uint32_t wd[CH];
+        if constexpr (CH == 4) {
+            const uint4 v = __ldg(reinterpret_cast<const uint4*>(s));
+            wd[0] = v.x; wd[1] = v.y; wd[2] = v.z; wd[3] = v.w;
+        } else {
+#pragma unroll
+            for (int k = 0; k < CH; ++k) wd[k] = __ldg(reinterpret_cast<const uint32_t*>(s) + k);
+        }
+        auto byte = [&](int i) { return (wd[i >> 2] >> (8 * (i & 3))) & 0xffu; };
+        uint32_t out = 0;
+#pragma unroll
+        for (int p = 0; p < 4; ++p) out |= gray_of(byte(p * CH), byte(p * CH + 1), byte(p * CH + 2), w0) << (8 * p);
+        *reinterpret_cast<uint32_t*>(d) = out;
+    } else {
+        for (int p = 0; p < n; ++p) d[p] = (uint8_t)gray_of(__ldg(s + p * CH), __ldg(s + p * CH + 1), __ldg(s + p * CH + 2), w0);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -269,17 +311,33 @@ __global__ void padded_level_kernel(const uint8_t* __restrict__ pyr, size_t fram
 // ------------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------------
-void launch_resize_planes(cudaStream_t st, const uint8_t* src_base, size_t src_stride, const LevelGeom& src, uint8_t* dst_base, size_t dst_stride,
-                          const LevelGeom& dst, const LinCoef* tabx, const LinCoef* taby, int n_planes) {
-    if (n_planes < 1) return;
+template <int CH>
+static void resize_planes(cudaStream_t st, const uint8_t* src_base, size_t src_stride, const LevelGeom& src, uint8_t* dst_base, size_t dst_stride,
+                          const LevelGeom& dst, const LinCoef* tabx, const LinCoef* taby, int n_planes, uint32_t w0) {
     const double rx = (double)src.w / dst.w, ry = (double)src.h / dst.h;
     if (rx * (kRzTW - 1) + 18.0 <= kRzSrcVec * 16 - 1 && ry * (kRzTH - 1) + 3.0 <= kRzSrcRows) {
         dim3 grd((dst.w + kRzTW - 1) / kRzTW, (dst.h + kRzTH - 1) / kRzTH, n_planes);
-        resize_level_kernel<<<grd, 256, 0, st>>>(src_base, src_stride, src, dst_base, dst_stride, dst, tabx, taby);
+        resize_level_kernel<CH><<<grd, 256, 0, st>>>(src_base, src_stride, src, dst_base, dst_stride, dst, tabx, taby, w0);
     } else {
         dim3 blk(32, 8), grd(((dst.w + 3) / 4 + 31) / 32, (dst.h + 7) / 8, n_planes);
-        resize_level_gather_kernel<<<grd, blk, 0, st>>>(src_base, src_stride, src, dst_base, dst_stride, dst, tabx, taby);
+        resize_level_gather_kernel<CH><<<grd, blk, 0, st>>>(src_base, src_stride, src, dst_base, dst_stride, dst, tabx, taby, w0);
     }
+}
+
+void launch_resize_planes(cudaStream_t st, const uint8_t* src_base, size_t src_stride, const LevelGeom& src, uint8_t* dst_base, size_t dst_stride,
+                          const LevelGeom& dst, const LinCoef* tabx, const LinCoef* taby, int n_planes, int ch, int w0) {
+    if (n_planes < 1) return;
+    if (ch == 3) resize_planes<3>(st, src_base, src_stride, src, dst_base, dst_stride, dst, tabx, taby, n_planes, (uint32_t)w0);
+    else if (ch == 4) resize_planes<4>(st, src_base, src_stride, src, dst_base, dst_stride, dst, tabx, taby, n_planes, (uint32_t)w0);
+    else resize_planes<1>(st, src_base, src_stride, src, dst_base, dst_stride, dst, tabx, taby, n_planes, 0u);
+}
+
+void launch_gray_planes(cudaStream_t st, const uint8_t* src_base, size_t src_stride, const LevelGeom& src, uint8_t* dst_base, size_t dst_stride,
+                        const LevelGeom& dst, int ch, int w0, int n_planes) {
+    if (n_planes < 1) return;
+    dim3 blk(32, 8), grd(((dst.w + 3) / 4 + 31) / 32, (dst.h + 7) / 8, n_planes);
+    if (ch == 3) gray_planes_kernel<3><<<grd, blk, 0, st>>>(src_base, src_stride, src, dst_base, dst_stride, dst, (uint32_t)w0);
+    else gray_planes_kernel<4><<<grd, blk, 0, st>>>(src_base, src_stride, src, dst_base, dst_stride, dst, (uint32_t)w0);
 }
 
 void launch_pyramid(cudaStream_t st, uint8_t* pyr, size_t frame_stride, const LevelGeom* h_levels, int n_levels,

@@ -4,7 +4,9 @@
 //          chunks inflated (zlib) straight into a pinned staging buffer - entropy decoding is a serial bit stream and stays on the host,
 //          one worker thread per frame;
 //   device (png_unfilter_gray_kernel): scanline reconstruction (None / Sub / Up / Average / Paeth, spec 9.2-9.4) + the gray conversion,
-//          written into level 0 of the frame's pyramid slot, so the decoded colour image never exists in memory.
+//          written into level 0 of the frame's pyramid slot, so the decoded colour image never exists in memory - except where the reference
+//          resizes or remaps the colour image before its conversion (a colour context with the input resize or the stereo rectification on):
+//          the kernel then stores the pixels' bytes in colour raw planes, and the resize / remap converts after interpolating.
 // A reconstructed sample depends on its left neighbour (same row) and on the row above, so the parallel order is a wavefront: one CTA per
 // frame, one thread per row of a band of up to 512 rows, thread r one pixel behind thread r-1; neighbours meet in a double-buffered
 // shared-memory exchange (one barrier per step), the row above a band comes from a global one-row buffer written by the band before.
@@ -28,8 +30,11 @@ namespace {
 
 constexpr int kPngRows = 512;
 
-// DEPTH16: CH = 2 bytes of one big-endian 16-bit sample -> uint16 at (pyr + frame * frame_stride + off0) with row pitch pitch0 bytes
-template <int CH, bool DEPTH16 = false>
+// What the kernel stores per reconstructed pixel: its gray value (kOutGray); one big-endian 16-bit sample as uint16 (kOutDepth16, CH = 2);
+// its CH bytes as they are (kOutPixels: the colour raw planes that the input resize or the remap converts to gray after interpolating).
+// Destination of frame f: pyr + f * frame_stride + off0, rows of pitch0 bytes.
+enum PngOut { kOutGray, kOutDepth16, kOutPixels };
+template <int CH, int OUT = kOutGray>
 __global__ void __launch_bounds__(kPngRows) png_unfilter_gray_kernel(const uint8_t* __restrict__ raw, size_t raw_stride, int w, int h, int camera_rgb,
                                                                      uint8_t* __restrict__ pyr, size_t frame_stride, int off0, int pitch0,
                                                                      uint32_t* __restrict__ band_rows, int* __restrict__ status) {
@@ -73,7 +78,11 @@ __global__ void __launch_bounds__(kPngRows) png_unfilter_gray_kernel(const uint8
                 a = px; c = b;
                 ex[s & 1][tid] = px;
                 if (tid == rows - 1 && y0 + kPngRows < h) brow[x] = px;             // the row above the next band
-                if constexpr (DEPTH16) {
+                if constexpr (OUT == kOutPixels) {
+                    uint8_t* o = dst + (size_t)y * pitch0 + (size_t)x * CH;
+#pragma unroll
+                    for (int k = 0; k < CH; ++k) o[k] = (uint8_t)(px >> (8 * k));
+                } else if constexpr (OUT == kOutDepth16) {
                     gacc |= (((px & 255u) << 8) | ((px >> 8) & 255u)) << (16 * (x & 1));
                     if ((x & 1) == 1 || x == w - 1) {                              // depth rows are 64-byte aligned and padded too
                         *reinterpret_cast<uint32_t*>(dst + (size_t)y * pitch0 + (size_t)(x & ~1) * 2) = gacc;
@@ -185,9 +194,15 @@ void launch_png_unfilter_gray(cudaStream_t st, const uint8_t* d_raw, size_t raw_
     else png_unfilter_gray_kernel<4><<<n_frames, kPngRows, 0, st>>>(d_raw, raw_stride, w, h, camera_rgb, pyr, frame_stride, l0.off, l0.pitch, band_rows, status);
 }
 
+void launch_png_unfilter_pixels(cudaStream_t st, const uint8_t* d_raw, size_t raw_stride, int w, int h, int channels, uint8_t* dst, size_t dst_stride,
+                                int pitch, uint32_t* band_rows, int* status, int n_frames) {
+    if (channels == 3) png_unfilter_gray_kernel<3, kOutPixels><<<n_frames, kPngRows, 0, st>>>(d_raw, raw_stride, w, h, 0, dst, dst_stride, 0, pitch, band_rows, status);
+    else png_unfilter_gray_kernel<4, kOutPixels><<<n_frames, kPngRows, 0, st>>>(d_raw, raw_stride, w, h, 0, dst, dst_stride, 0, pitch, band_rows, status);
+}
+
 void launch_png_unfilter_depth16(cudaStream_t st, const uint8_t* d_raw, size_t raw_stride, int w, int h, uint16_t* depth, size_t frame_elems,
                                  size_t pitch_elems, uint32_t* band_rows, int* status, int n_frames) {
-    png_unfilter_gray_kernel<2, true><<<n_frames, kPngRows, 0, st>>>(d_raw, raw_stride, w, h, 0, reinterpret_cast<uint8_t*>(depth), frame_elems * 2, 0,
+    png_unfilter_gray_kernel<2, kOutDepth16><<<n_frames, kPngRows, 0, st>>>(d_raw, raw_stride, w, h, 0, reinterpret_cast<uint8_t*>(depth), frame_elems * 2, 0,
                                                                       (int)(pitch_elems * 2), band_rows, status);
 }
 

@@ -145,13 +145,21 @@ struct Ctx {
     bool resize = false;
     int in_w = 0, in_h = 0, in_pitch = 0, resize_kx = 0, resize_ky = 0;
     DeviceArray<LinCoef> d_resize_coefs;
-    // Raw image planes: the images of the uploaded batch before the conditioning kernel (rectification or resize) writes level 0 of the frame
-    // slots.  d_raw_img: max_batch planes of in_pitch x in_h bytes, allocated by the first upload that needs them (and reallocated when the
-    // input size grows); host uploads and PNG decodes write there instead of level 0.  raw_src: the raw planes of the uploaded batch
-    // (d_raw_img, or a staged slot's planes).  d_depth16_raw / depth_src: the same for RGB-D depth images with the resize on (row pitch
-    // depth16_raw_pitch elements).  No chain graph references these buffers, so they need no scratch_generation bump.
+    // colour camera input (rgbl_set_input_channels): the camera-input entry points take images of in_ch bytes per pixel (1, or 3 / 4
+    // interleaved), whose channel 0 has the gray weight in_w0 (gray_of: 9798 with Camera.RGB = 1, else 3735).  in_pitch: the row pitch of
+    // an input-size image of in_ch bytes per pixel (64-byte rows).
+    int in_ch = 1, in_w0 = 3735;
+    // Raw image planes: the images of the uploaded batch before the conditioning kernel (rectification, resize or gray conversion) writes
+    // level 0 of the frame slots.  d_raw_img: max_batch planes of in_h rows, allocated by the first upload that needs them (and reallocated
+    // when a later one needs more); host uploads and PNG decodes write there instead of level 0.  raw_src: the raw planes of the uploaded
+    // batch (d_raw_img, or a staged slot's planes); raw_ch / raw_w0 / raw_pitch: what they hold (bytes per pixel, the gray weight of channel
+    // 0, row pitch; plane z at raw_src + z * raw_pitch * in_h), raw_ch = 0: the upload wrote level 0 itself.  A colour context can receive
+    // gray PNG streams, and a PNG file's samples are in R, G, B order, so these are recorded per upload.  d_depth16_raw / depth_src: the same
+    // for RGB-D depth images with the resize on (row pitch depth16_raw_pitch elements).  No chain graph references these buffers, so they
+    // need no scratch_generation bump.
     DeviceArray<uint8_t> d_raw_img;
     const uint8_t* raw_src = nullptr;
+    int raw_ch = 0, raw_w0 = 0, raw_pitch = 0;
     DeviceArray<uint16_t> d_depth16_raw;
     size_t depth16_raw_pitch = 0;
     const uint16_t* depth_src = nullptr;
@@ -231,10 +239,10 @@ struct Ctx {
     // rgbl_track_sequence_rgbd, rgbl_resident_stage_stereo / rgbl_track_sequence_stereo): level-0 planes + clouds (RGB-L), uint16 depth
     // planes (RGB-D) or the left then the right level-0 planes (stereo: n_frames pairs, 2 n_frames planes) of whole batches
     static constexpr int kMaxStageSlots = 8;
-    // (in_w x in_h: the input size the slot was staged at)
+    // (in_w x in_h, ch: the input size and channel count the slot was staged with)
     struct StageSlot {
         DeviceArray<uint8_t> img; DeviceArray<float> pts; DeviceArray<int> n_pts; DeviceArray<uint16_t> depth;
-        int n_frames = 0, max_pts = 0, in_w = 0, in_h = 0; InputKind kind = InputKind::rgbl;
+        int n_frames = 0, max_pts = 0, in_w = 0, in_h = 0, ch = 1; InputKind kind = InputKind::rgbl;
     };
     StageSlot stage[kMaxStageSlots];
 

@@ -37,6 +37,13 @@ namespace rgbl {
 #define RGBL_DDIV(a, b) ((double)(a) / (double)(b))
 #endif
 
+// cv::cvtColor({RGB,BGR,RGBA,BGRA}2GRAY) of one 8-bit pixel: cvtColor's 15-bit fixed point (9798 R, 19235 G, 3735 B, + 2^14, >> 15; the
+// same formula as png_unfilter_gray_kernel's).  w0 = the weight of channel 0 (9798 or 3735); channel 2 gets the other one, alpha none.
+constexpr int kGrayWeightRB = 9798 + 3735;
+RGBL_HD uint32_t gray_of(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t w0) {
+    return (c0 * w0 + c1 * 19235u + c2 * (kGrayWeightRB - w0) + (1u << 14)) >> 15;
+}
+
 // cv::undistortPoints(src, dst, K, D, noArray(), K) for one CV_32FC2 point, as Frame::UndistortKeyPoints and Frame::ComputeImageBounds
 // call it (src/Frame.cc:837-899): OpenCV's cvUndistortPointsInternal (calib3d/src/undistort.dispatch.cpp) in double precision with
 // its default criterion (MAX_ITER 5) and the operations in its order.  K = P and R = I, so the tilt matrix and R P are exact identities

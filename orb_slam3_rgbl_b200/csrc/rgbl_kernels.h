@@ -21,9 +21,14 @@ struct __align__(8) SelKp {
 void launch_pyramid(cudaStream_t st, uint8_t* pyr, size_t frame_stride, const LevelGeom* h_levels, int n_levels,
                     const LinCoef* d_coefs, int n_frames);
 // cv::resize(INTER_LINEAR) of n_planes 8-bit planes, src.w x src.h -> dst.w x dst.h with the tables tabx / taby (linear_coefs): plane z at
-// src_base + z * src_stride + src.off -> dst_base + z * dst_stride + dst.off; both rows 64-byte aligned (pitch % 64 == 0, 16-byte aligned bases)
+// src_base + z * src_stride + src.off -> dst_base + z * dst_stride + dst.off; both rows 64-byte aligned (pitch % 64 == 0, 16-byte aligned bases).
+// ch 3 / 4: the source planes are interleaved colour images (src.pitch in bytes), resized per channel and converted to gray (gray_of, channel 0
+// weighted w0, rgbl_device.cuh) into the 8-bit destination planes
 void launch_resize_planes(cudaStream_t st, const uint8_t* src_base, size_t src_stride, const LevelGeom& src, uint8_t* dst_base, size_t dst_stride,
-                          const LevelGeom& dst, const LinCoef* tabx, const LinCoef* taby, int n_planes);
+                          const LevelGeom& dst, const LinCoef* tabx, const LinCoef* taby, int n_planes, int ch = 1, int w0 = 0);
+// cvtColor to gray of n_planes interleaved colour planes of ch (3 / 4) bytes per pixel, dst.w x dst.h, laid out as for launch_resize_planes
+void launch_gray_planes(cudaStream_t st, const uint8_t* src_base, size_t src_stride, const LevelGeom& src, uint8_t* dst_base, size_t dst_stride,
+                        const LevelGeom& dst, int ch, int w0, int n_planes);
 // fast_strip_kernels.cu: per-cell FAST with the iniTh -> minTh fallback, one CTA per strip of cells (fast_strip.cuh); survivors in
 // each cell's slot array; returns -1 when the shared-memory request is refused
 int launch_fast_strips(cudaStream_t st, const uint8_t* pyr, size_t frame_stride, const LevelGeom* d_levels, const CellInfo* d_cells,
@@ -38,6 +43,10 @@ int png_inflate_batch(int n_frames, const uint8_t* const* png, const size_t* png
                       std::string& err, bool depth16 = false);
 void launch_png_unfilter_gray(cudaStream_t st, const uint8_t* d_raw, size_t raw_stride, int w, int h, int channels, int camera_rgb, uint8_t* pyr,
                               size_t frame_stride, const LevelGeom& l0, uint32_t* band_rows, int* status, int n_frames);
+// the same reconstruction of 3 / 4-channel streams with the pixels' bytes stored as they are (the file's R, G, B(, A) order) in colour planes:
+// frame f at dst + f * dst_stride, rows of `pitch` bytes (a multiple of 4)
+void launch_png_unfilter_pixels(cudaStream_t st, const uint8_t* d_raw, size_t raw_stride, int w, int h, int channels, uint8_t* dst, size_t dst_stride,
+                                int pitch, uint32_t* band_rows, int* status, int n_frames);
 // 16-bit depth PNG scanlines (ch = 2) -> uint16 depth planes (frame f at depth + f * frame_elems, row pitch pitch_elems, pitch a multiple of 32)
 void launch_png_unfilter_depth16(cudaStream_t st, const uint8_t* d_raw, size_t raw_stride, int w, int h, uint16_t* depth, size_t frame_elems,
                                  size_t pitch_elems, uint32_t* band_rows, int* status, int n_frames);
@@ -229,6 +238,7 @@ struct RectifyDev {
     int W, H;                                                        // output (and map) size: the context's
     int src_W, src_H;                                                // raw plane size: the input resize's source size (0, 0: W x H)
     const uint8_t* src; size_t src_stride; int src_pitch;            // raw plane of slot s at src + s * src_stride
+    int ch, w0;                                                      // ch 3 / 4: colour raw planes, remapped per channel, then gray_of(w0); else 8-bit
     uint8_t* dst; size_t dst_stride; int dst_off, dst_pitch;         // rectified plane of slot s at dst + s * dst_stride + dst_off (4-byte aligned rows)
 };
 // slots [0, n_pairs) through the left camera's map, [n_pairs, 2 n_pairs) through the right camera's, in one launch

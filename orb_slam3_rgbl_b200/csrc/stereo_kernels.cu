@@ -258,6 +258,10 @@ constexpr int kGroup = 4;                  // output pixels per thread: one 32-b
 
 // One thread per group of 4 output pixels of row blockIdx.y of camera blockIdx.z: the group's map entries are read once, then the
 // camera's n frames are remapped with them.  Taps outside the source get weight 0 and offset 0, so the frame loop has no branch.
+// CH > 1: colour raw planes of CH bytes per pixel; each channel is remapped as a gray plane is (cv::remap of an 8UC3 / 8UC4 image equals the
+// per-channel 8UC1 remap) and the 3 channel values are converted to gray (gray_of) - TrackStereo's remap of the colour image, then
+// GrabImageStereo's cvtColor.
+template <int CH>
 __global__ void __launch_bounds__(128) rectify_kernel(RectifyDev r, int n) {
     const int x0 = (blockIdx.x * blockDim.x + threadIdx.x) * kGroup, y = blockIdx.y, cam = blockIdx.z;
     if (x0 >= r.W) return;
@@ -275,7 +279,7 @@ __global__ void __launch_bounds__(128) rectify_kernel(RectifyDev r, int n) {
         for (int t = 0; t < 4; ++t) {
             const int tx = sx + (t & 1), ty = sy + (t >> 1);
             const bool in = tx >= 0 && tx < r.src_W && ty >= 0 && ty < r.src_H;
-            off[p][t] = in ? ty * r.src_pitch + tx : 0;
+            off[p][t] = in ? ty * r.src_pitch + tx * CH : 0;
             w[p][t] = in ? wt[t] : 0;
         }
     }
@@ -286,10 +290,17 @@ __global__ void __launch_bounds__(128) rectify_kernel(RectifyDev r, int n) {
         uint32_t packed = 0;
 #pragma unroll
         for (int p = 0; p < kGroup; ++p) {
-            int s = 1 << 14;
+            constexpr int NC = CH == 1 ? 1 : 3;          // alpha is not read
+            uint32_t v[NC];
 #pragma unroll
-            for (int t = 0; t < 4; ++t) s += (int)__ldg(src + off[p][t]) * w[p][t];
-            packed |= (uint32_t)min(s >> 15, 255) << (8 * p);
+            for (int k = 0; k < NC; ++k) {
+                int s = 1 << 14;
+#pragma unroll
+                for (int t = 0; t < 4; ++t) s += (int)__ldg(src + off[p][t] + k) * w[p][t];
+                v[k] = (uint32_t)min(s >> 15, 255);
+            }
+            if constexpr (CH == 1) packed |= v[0] << (8 * p);
+            else packed |= gray_of(v[0], v[1], v[2], (uint32_t)r.w0) << (8 * p);
         }
         uint8_t* dst = r.dst + (size_t)slot * r.dst_stride + r.dst_off + (size_t)y * r.dst_pitch + x0;
         if (n_out == kGroup) *reinterpret_cast<uint32_t*>(dst) = packed;
@@ -308,7 +319,10 @@ void launch_rectify(cudaStream_t st, const RectifyDev& r, int n_pairs) {
     RectifyDev k = r;
     if (!k.src_W) { k.src_W = k.W; k.src_H = k.H; }
     const int groups = (k.W + kGroup - 1) / kGroup;
-    rectify_kernel<<<dim3((groups + 127) / 128, k.H, 2), 128, 0, st>>>(k, n_pairs);
+    const dim3 grd((groups + 127) / 128, k.H, 2);
+    if (k.ch == 3) rectify_kernel<3><<<grd, 128, 0, st>>>(k, n_pairs);
+    else if (k.ch == 4) rectify_kernel<4><<<grd, 128, 0, st>>>(k, n_pairs);
+    else rectify_kernel<1><<<grd, 128, 0, st>>>(k, n_pairs);
 }
 
 }  // namespace rgbl

@@ -78,6 +78,12 @@ class Context:
         width x height is Camera.newWidth x Camera.newHeight.  (0, 0) or the context's size: off."""
         check(lib().rgbl_set_input_resize(self.handle, int(src_width), int(src_height)), self.handle)
 
+    def set_input_channels(self, channels: int = 1, camera_rgb: bool = True):
+        """Take colour camera images (rgbl_set_input_channels, the cvtColor of Tracking::GrabImageRGBL / GrabImageRGBD / GrabImageStereo):
+        the uploads, stage calls and runners then take H x W x channels uint8 images (3 or 4, the cv::Mat's channel order) and convert them
+        to gray on the device.  camera_rgb = Camera.RGB (True: channel 0 is red).  channels 1: gray images (the default)."""
+        check(lib().rgbl_set_input_channels(self.handle, int(channels), int(bool(camera_rgb))), self.handle)
+
     def set_host_quadtree(self, on: bool):
         check(lib().rgbl_set_host_quadtree(self.handle, int(on)), self.handle)
 
@@ -538,12 +544,18 @@ def make_chain_params(pose0, fx, fy, cx, cy, bf, th_last=15.0, mono=False, conti
     return p
 
 
+def _image_shape(img) -> tuple:
+    """(H, W, channels) of a gray (H x W) or colour (H x W x C) camera image"""
+    return (img.shape[0], img.shape[1], img.shape[2] if img.ndim == 3 else 1)
+
+
 class _FrameBatch:
     """The output buffers of one batch of frame constructions, and the calls that read the batch from the device: download,
     download_keys_un and the tracking chain.  The input kinds (RgblBatch, RgbdBatch, StereoBatch) add their inputs and upload calls."""
 
-    def __init__(self, ctx: Context, nF: int, W: int, H: int, pinned: bool):
-        self.ctx, self.nF, self.cap, self.W, self.H = ctx, nF, ctx.cap, W, H
+    def __init__(self, ctx: Context, nF: int, W: int, H: int, pinned: bool, channels: int = 1):
+        self.ctx, self.nF, self.cap, self.W, self.H, self.C = ctx, nF, ctx.cap, W, H, channels
+        self.stride = W * channels          # bytes per image row (colour images: rgbl_set_input_channels)
         self._alloc = alloc = _pinned_alloc if pinned else (lambda shape, dt: np.empty(shape, dt))
         self.kps = alloc((nF, self.cap), KP_DTYPE); self.desc = alloc((nF, self.cap, 32), np.uint8)
         self.depth = alloc((nF, self.cap), np.float32); self.uright = alloc((nF, self.cap), np.float32)
@@ -577,13 +589,14 @@ class _FrameBatch:
 
 
 class RgblBatch(_FrameBatch):
-    """Reusable (pinned if torch+CUDA are available) host buffers for rgbl_frame_rgbl_batch / the resident API."""
+    """Reusable (pinned if torch+CUDA are available) host buffers for rgbl_frame_rgbl_batch / the resident API.  Images: H x W gray, or
+    H x W x C colour for a context that takes colour input (Context.set_input_channels; the resident API only)."""
 
     def __init__(self, ctx: Context, images, clouds, P, depth_params: DepthParams, pinned=True):
-        H, W = images[0].shape
-        super().__init__(ctx, len(images), W, H, pinned)
+        H, W, Ch = _image_shape(images[0])
+        super().__init__(ctx, len(images), W, H, pinned, Ch)
         nF, alloc = self.nF, self._alloc
-        self.img = alloc((nF, H, W), np.uint8)
+        self.img = alloc((nF,) + images[0].shape, np.uint8)
         maxn = max(p.shape[1] for p in clouds)
         self.pts = alloc((nF, 4 * maxn), np.float32)
         self.npts = np.array([p.shape[1] for p in clouds], np.int32)
@@ -594,7 +607,7 @@ class RgblBatch(_FrameBatch):
         self.pa = (C.c_void_p * nF)(*[self.pts[f].ctypes.data for f in range(nF)])
         self.P = np.ascontiguousarray(P, np.float32).reshape(12)
         self.prm = depth_params
-        self.h2d_bytes = int(nF * W * H + 4 * 4 * int(self.npts.sum()))
+        self.h2d_bytes = int(nF * W * H * Ch + 4 * 4 * int(self.npts.sum()))
 
     def run_e2e(self):
         """One end-to-end call with host buffers: H2D inputs + all kernels + D2H results."""
@@ -609,7 +622,7 @@ class RgblBatch(_FrameBatch):
 
     def upload(self):
         c = self.ctx
-        check(lib().rgbl_resident_upload(c.handle, self.nF, self.ia, self.W, self.H, self.W, self.pa, ptr(self.npts)), c.handle)
+        check(lib().rgbl_resident_upload(c.handle, self.nF, self.ia, self.W, self.H, self.stride, self.pa, ptr(self.npts)), c.handle)
 
     def upload_kitti(self, xyzr_list):
         """Resident upload with raw KITTI .bin records (n x 4: x, y, z, reflectance) instead of the planar 4 x n clouds."""
@@ -617,7 +630,7 @@ class RgblBatch(_FrameBatch):
         raw = [np.ascontiguousarray(r, np.float32).reshape(-1, 4) for r in xyzr_list]
         npts = np.array([len(r) for r in raw], np.int32)
         arr = (C.c_void_p * self.nF)(*[r.ctypes.data for r in raw])
-        check(lib().rgbl_resident_upload_kitti(c.handle, self.nF, self.ia, self.W, self.H, self.W, arr, ptr(npts)), c.handle)
+        check(lib().rgbl_resident_upload_kitti(c.handle, self.nF, self.ia, self.W, self.H, self.stride, arr, ptr(npts)), c.handle)
 
     def upload_kitti_png(self, png_list, xyzr_list, camera_rgb=True):
         """Resident upload with the images as PNG FILE BYTES (cv::imread + cvtColor to gray on the way, rgbl_resident_upload_kitti_png)
@@ -667,7 +680,7 @@ class RgblBatch(_FrameBatch):
             assert 4 * n <= self.pts.shape[1]
             self.pts[f, :4 * n] = np.ascontiguousarray(clouds[f], np.float32).reshape(-1)
             self.npts[f] = n
-        self.h2d_bytes = int(self.nF * self.W * self.H + 4 * 4 * int(self.npts.sum()))
+        self.h2d_bytes = int(self.nF * self.W * self.H * self.C + 4 * 4 * int(self.npts.sum()))
 
 
 class RgbdBatch(_FrameBatch):
@@ -675,10 +688,10 @@ class RgbdBatch(_FrameBatch):
     constructor (src/Frame.cc:200-237) is upload + process_resident; download / track_begin2 / track_end2 as for RgblBatch."""
 
     def __init__(self, ctx: Context, images, depths, pinned=True):
-        H, W = images[0].shape
-        super().__init__(ctx, len(images), W, H, pinned)
+        H, W, Ch = _image_shape(images[0])
+        super().__init__(ctx, len(images), W, H, pinned, Ch)
         nF, alloc = self.nF, self._alloc
-        self.img = alloc((nF, H, W), np.uint8); self.dep = alloc((nF, H, W), np.uint16)
+        self.img = alloc((nF,) + images[0].shape, np.uint8); self.dep = alloc((nF, H, W), np.uint16)
         self.set_inputs(images, depths)
         self.ia = (C.c_void_p * nF)(*[self.img[f].ctypes.data for f in range(nF)])
         self.da = (C.c_void_p * nF)(*[self.dep[f].ctypes.data for f in range(nF)])
@@ -691,7 +704,7 @@ class RgbdBatch(_FrameBatch):
 
     def upload(self):
         c = self.ctx
-        check(lib().rgbl_resident_upload_rgbd(c.handle, self.nF, self.ia, self.W, self.H, self.W, self.da, self.W), c.handle)
+        check(lib().rgbl_resident_upload_rgbd(c.handle, self.nF, self.ia, self.W, self.H, self.stride, self.da, self.W), c.handle)
 
     def upload_png(self, png_list, depth_png_list, camera_rgb=True):
         """Resident upload of the files' bytes: image PNGs (imread + cvtColor to gray) and 16-bit depth PNGs (imread IMREAD_UNCHANGED)."""
@@ -715,10 +728,10 @@ class StereoBatch(_FrameBatch):
     download_keys_un / track_begin2 / track_end2 then see the left frames, as for RgblBatch."""
 
     def __init__(self, ctx: Context, lefts, rights, pinned=True):
-        H, W = lefts[0].shape
-        super().__init__(ctx, len(lefts), W, H, pinned)
+        H, W, Ch = _image_shape(lefts[0])
+        super().__init__(ctx, len(lefts), W, H, pinned, Ch)
         nF, alloc = self.nF, self._alloc
-        self.left = alloc((nF, H, W), np.uint8); self.right = alloc((nF, H, W), np.uint8)
+        self.left = alloc((nF,) + lefts[0].shape, np.uint8); self.right = alloc((nF,) + lefts[0].shape, np.uint8)
         self.set_inputs(lefts, rights)
         self.la = (C.c_void_p * nF)(*[self.left[f].ctypes.data for f in range(nF)])
         self.ra = (C.c_void_p * nF)(*[self.right[f].ctypes.data for f in range(nF)])
@@ -730,7 +743,7 @@ class StereoBatch(_FrameBatch):
 
     def upload(self):
         c = self.ctx
-        check(lib().rgbl_resident_upload_stereo(c.handle, self.nF, self.la, self.ra, self.W, self.H, self.W), c.handle)
+        check(lib().rgbl_resident_upload_stereo(c.handle, self.nF, self.la, self.ra, self.W, self.H, self.stride), c.handle)
 
     def upload_png(self, left_pngs, right_pngs, camera_rgb=True):
         """Resident upload of the files' bytes (KITTI image_0 / image_1 PNGs: imread + cvtColor to gray on the way)."""
@@ -757,37 +770,42 @@ class SequenceIO(C.Structure):
 
 class SequenceRunner:
     """rgbl_track_sequence: many consecutive batches of one RGB-L sequence per native call (the loop of Examples/RGB-L/rgbl_kitti.cc).
-    Holds M batches of T frames in pinned host buffers (and, after stage(), in device slots); batches are visited round-robin."""
+    Holds M batches of T frames in pinned host buffers (and, after stage(), in device slots); batches are visited round-robin.
+    channels 3 / 4: the images are H x W x channels colour images (Context.set_input_channels)."""
 
-    def __init__(self, ctx: Context, P, depth_params: DepthParams, T: int, W: int, H: int, max_points: int, n_host_batches: int, pinned=True):
-        self._init(ctx, T, W, H, n_host_batches, pinned, "rgbl", (4 * max_points,), np.float32)
+    def __init__(self, ctx: Context, P, depth_params: DepthParams, T: int, W: int, H: int, max_points: int, n_host_batches: int, pinned=True,
+                 channels: int = 1):
+        self._init(ctx, T, W, H, n_host_batches, pinned, "rgbl", (4 * max_points,), np.float32, channels)
         self.maxn, self.pts, self.npts = max_points, self.second, np.zeros((self.M, T), np.int32)
         self.P = np.ascontiguousarray(P, np.float32).reshape(12)
         self.prm = depth_params
 
     @classmethod
-    def rgbd(cls, ctx: Context, depth_scale: float, bf: float, T: int, W: int, H: int, n_host_batches: int, pinned=True) -> "SequenceRunner":
+    def rgbd(cls, ctx: Context, depth_scale: float, bf: float, T: int, W: int, H: int, n_host_batches: int, pinned=True,
+             channels: int = 1) -> "SequenceRunner":
         """RGB-D mode (rgbl_track_sequence_rgbd, the loop of Examples/RGB-D/rgbd_kitti.cc): batches of gray images + CV_16U depth images;
         set_batch(m, images, depths).  depth_scale = Tracking::mDepthMapFactor, bf = Camera.bf."""
         self = cls.__new__(cls)
-        self._init(ctx, T, W, H, n_host_batches, pinned, "rgbd", (H, W), np.uint16)
+        self._init(ctx, T, W, H, n_host_batches, pinned, "rgbd", (H, W), np.uint16, channels)
         self.dep, self.depth_scale, self.bf = self.second, float(depth_scale), float(bf)
         return self
 
     @classmethod
-    def stereo(cls, ctx: Context, mb: float, mbf: float, T: int, W: int, H: int, n_host_batches: int, pinned=True) -> "SequenceRunner":
+    def stereo(cls, ctx: Context, mb: float, mbf: float, T: int, W: int, H: int, n_host_batches: int, pinned=True,
+               channels: int = 1) -> "SequenceRunner":
         """Stereo mode (rgbl_track_sequence_stereo, the loop of Examples/Stereo/stereo_kitti.cc): batches of T rectified pairs, extracted as
         batches of 2T frames (ctx.max_batch >= 2T); set_batch(m, lefts, rights).  mb = mbf / fx, mbf = Camera.bf."""
         self = cls.__new__(cls)
-        self._init(ctx, T, W, H, n_host_batches, pinned, "stereo", (H, W), np.uint8)
+        self._init(ctx, T, W, H, n_host_batches, pinned, "stereo", (H, W) + ((channels,) if channels > 1 else ()), np.uint8, channels)
         self.right, self.mb, self.mbf = self.second, float(mb), float(mbf)
         return self
 
-    def _init(self, ctx, T, W, H, n_host_batches, pinned, kind, second_shape, second_dtype):
+    def _init(self, ctx, T, W, H, n_host_batches, pinned, kind, second_shape, second_dtype, channels):
         """The images of M batches and, per frame, the kind's second input (`second`): a flat cloud, a depth image or a right image."""
         self.ctx, self.T, self.W, self.H, self.M, self.maxn, self.kind = ctx, T, W, H, n_host_batches, 0, kind
+        self.C, self.stride = channels, W * channels
         self._alloc = _pinned_alloc if pinned else (lambda shape, dt: np.empty(shape, dt))
-        self.img = self._alloc((self.M, T, H, W), np.uint8)
+        self.img = self._alloc((self.M, T, H, W) + ((channels,) if channels > 1 else ()), np.uint8)
         self.second = self._alloc((self.M, T) + second_shape, second_dtype)
         self._out = None
 
@@ -808,14 +826,14 @@ class SequenceRunner:
 
     def stage(self, slot: int, m: int):
         """Upload host batch m into device slot `slot` (rgbl_resident_stage / _stage_rgbd / _stage_stereo)."""
-        h, T, W, H = self.ctx.handle, self.T, self.W, self.H
+        h, T, W, H, S = self.ctx.handle, self.T, self.W, self.H, self.stride
         ia, sa = self._frames(self.img, [m]), self._frames(self.second, [m])
         if self.kind == "stereo":
-            check(lib().rgbl_resident_stage_stereo(h, slot, T, ia, sa, W, H, W), h)
+            check(lib().rgbl_resident_stage_stereo(h, slot, T, ia, sa, W, H, S), h)
         elif self.kind == "rgbd":
-            check(lib().rgbl_resident_stage_rgbd(h, slot, T, ia, W, H, W, sa, W), h)
+            check(lib().rgbl_resident_stage_rgbd(h, slot, T, ia, W, H, S, sa, W), h)
         else:
-            check(lib().rgbl_resident_stage(h, slot, T, ia, W, H, W, sa, ptr(np.ascontiguousarray(self.npts[m]))), h)
+            check(lib().rgbl_resident_stage(h, slot, T, ia, W, H, S, sa, ptr(np.ascontiguousarray(self.npts[m]))), h)
 
     def _outputs(self, nb, want_frames):
         n = nb * self.T
@@ -840,7 +858,7 @@ class SequenceRunner:
         T = self.T
         o = self._outputs(n_batches, want_frames)
         io = SequenceIO()
-        io.n_batches, io.frames_per_batch, io.width, io.height, io.stride = n_batches, T, self.W, self.H, self.W
+        io.n_batches, io.frames_per_batch, io.width, io.height, io.stride = n_batches, T, self.W, self.H, self.stride
         sa = na = None
         if resident_slots > 0:
             io.n_slots = resident_slots; io.first_slot = first % resident_slots
@@ -867,7 +885,7 @@ class SequenceRunner:
 
     def h2d_bytes_per_batch(self) -> float:
         second = 16.0 * self.npts.sum() / self.M if self.kind == "rgbl" else self.T * self.second[0, 0].nbytes
-        return float(self.T * self.W * self.H + second)
+        return float(self.T * self.img[0, 0].nbytes + second)
 
     def d2h_bytes_per_batch(self, want_frames: bool) -> float:
         b = self.T * (7 * 4 + 3 * 4)
