@@ -32,6 +32,20 @@ static void release(Ctx* c) {
 template <class A>
 static bool ensure(A& a, size_t n) { return a.size() >= n || a.alloc(n) == cudaSuccess; }
 
+// the row pitch of an input-size image of ch bytes per pixel (64-byte rows)
+static int input_pitch(const Ctx* c, int ch) { return (c->input.w * ch + 63) & ~63; }
+
+// After a change of the camera-input setting: writes its derived values and drops the resident batch, which was loaded for the previous
+// setting (stereo_only: the change concerns stereo pairs only, and a batch of another kind is kept)
+static void input_changed(Ctx* c, bool stereo_only = false) {
+    InputSetting& in = c->input;
+    const int W = c->cfg.width, H = c->cfg.height;
+    in.pitch = input_pitch(c, in.ch);
+    in.depth_pitch = ((size_t)in.w * sizeof(uint16_t) + 63) / 64 * 32;
+    in.kx = in.w % W == 0 ? in.w / W : 0; in.ky = in.h % H == 0 ? in.h / H : 0;
+    if (!stereo_only || c->resident_kind == InputKind::stereo) c->resident_frames = 0;
+}
+
 static int create(const rgbl_config* cfg, Ctx** out) {
     Ctx* c = new Ctx();
     c->cfg = *cfg;
@@ -43,7 +57,7 @@ static int create(const rgbl_config* cfg, Ctx** out) {
     rc = build_geometry(cfg->width, cfg->height, c->tab, c->levels, c->cells, c->coefs, c->frame_bytes, c->err);
     if (rc) return fail(rc);
     c->n_cells = (int)c->cells.size();
-    c->in_w = cfg->width; c->in_h = cfg->height; c->in_pitch = c->levels[0].pitch;      // no input resize
+    c->input.w = cfg->width; c->input.h = cfg->height; input_changed(c);      // gray images of the context's size
     // DistributeOctTree returns at most max(quota + 2, 4 * nIni) keypoints per level (SURVEY App. C: the very
     // first subdivision pass is unguarded, later ones stop within +3 of the budget).
     c->cap_kp = 0;
@@ -185,15 +199,14 @@ void prof_collect(Ctx* c) {
 // Stage 2 (host):   quad-tree per (frame, level) on worker threads -> SelKp lists.
 // Stage 3 (device): describe.  Results stay in d_kps / d_desc (copied out by the callers).
 
-// The image planes of a batch: plane f at base + f * stride + off, rows pitch bytes apart, w x h pixels of ch bytes.  raw: the planes are the
-// source of the kernel that writes level 0 (the remap of stereo pairs with rectification on, the input resize, the gray conversion), not level 0.
+// The image planes of a batch: plane f at base + f * stride + off, rows pitch bytes apart, w x h pixels of ch bytes
 struct Planes {
-    uint8_t* base; size_t stride, off; int pitch; bool raw; int w, h; int ch = 1;
+    uint8_t* base; size_t stride, off; int pitch; int w, h; int ch = 1;
     uint8_t* at(int f) const { return base + (size_t)f * stride + off; }
 };
 
 static Planes level0_planes(const Ctx* c) {
-    return {c->d_pyr, c->frame_bytes, (size_t)c->levels[0].off, c->levels[0].pitch, false, c->cfg.width, c->cfg.height};
+    return {c->d_pyr, c->frame_bytes, (size_t)c->levels[0].off, c->levels[0].pitch, c->cfg.width, c->cfg.height};
 }
 
 // H2D of n host images into planes [first, first + n) of dst, on stream st
@@ -690,18 +703,24 @@ int rgbl_depth_from_map(rgbl_ctx* ctx, const float* depth_map, int width, int he
     return RGBL_OK;
 }
 
-// input_size: the images are camera input (the input size, rgbl_set_input_resize), else they have the context's size; ch: their bytes per pixel
-static int check_batch_args(Ctx* c, int n_frames, int width, int height, int stride, bool input_size = true, int ch = 1) {
-    if (width <= 0 || height <= 0) { c->err = "empty image"; return RGBL_E_EMPTY; }
-    const bool rs = input_size && c->resize;
-    if (ch > 1 && stride < width * ch) { c->err = "stride < width * channels (rgbl_set_input_channels)"; return RGBL_E_INVALID; }
-    if (width != (rs ? c->in_w : c->cfg.width) || height != (rs ? c->in_h : c->cfg.height) || stride < width) {
-        c->err = rs ? "image size does not match the input size (rgbl_set_input_resize)" : "image size does not match the context"; return RGBL_E_INVALID;
-    }
+// n_frames images (or pairs) in one batch
+static int check_batch(Ctx* c, int n_frames) {
     if (n_frames < 1) { c->err = "n_frames < 1"; return RGBL_E_INVALID; }
     if (n_frames > c->cfg.max_batch) { c->err = "n_frames exceeds max_batch"; return RGBL_E_CAPACITY; }
     return RGBL_OK;
 }
+
+// A batch of n_frames images of width x height pixels, rows stride bytes apart, that an entry point takes as `images` has them: camera
+// input (c->input), or gray images of the context's size (gray_images)
+static int check_images(Ctx* c, const InputSetting& images, int n_frames, int width, int height, int stride) {
+    if (width <= 0 || height <= 0) { c->err = "empty image"; return RGBL_E_EMPTY; }
+    if (images.ch > 1 && stride < width * images.ch) { c->err = "stride < width * channels (rgbl_set_input_channels)"; return RGBL_E_INVALID; }
+    if (width != images.w || height != images.h || stride < width) {
+        c->err = images.resize ? "image size does not match the input size (rgbl_set_input_resize)" : "image size does not match the context"; return RGBL_E_INVALID;
+    }
+    return check_batch(c, n_frames);
+}
+static InputSetting gray_images(const Ctx* c) { return InputSetting{c->cfg.width, c->cfg.height}; }
 
 // what each input kind is called, and the process call and sequence runner that take it (indexed by InputKind)
 struct KindNames { const char* what; const char* process; const char* runner; };
@@ -739,7 +758,7 @@ struct HostInputs {
         return {InputKind::stereo, n, left, right, stride, nullptr, nullptr, 0, nullptr, 0};
     }
     // the images are camera input, of the context's channel count (rgbl_set_input_channels)
-    HostInputs camera(const Ctx* c) const { HostInputs r = *this; r.ch = c->in_ch; return r; }
+    HostInputs camera(const Ctx* c) const { HostInputs r = *this; r.ch = c->input.ch; return r; }
     // batch b of consecutive batches of n
     HostInputs batch(int b) const {
         const size_t o = (size_t)b * n;
@@ -768,7 +787,7 @@ static int check_inputs(Ctx* c, const HostInputs& in, int* max_pts) {
     for (int f = 0; f < in.n; ++f)
         if (!in.gray[f] || (in.right && !in.right[f])) { c->err = "empty image"; return RGBL_E_EMPTY; }
     if (in.kind == InputKind::rgbd) {
-        if (!in.depth || in.depth_stride < c->in_w) { c->err = !in.depth ? "null argument" : "depth_stride < width"; return RGBL_E_INVALID; }
+        if (!in.depth || in.depth_stride < c->input.w) { c->err = !in.depth ? "null argument" : "depth_stride < width"; return RGBL_E_INVALID; }
         for (int f = 0; f < in.n; ++f) if (!in.depth[f]) { c->err = "empty depth image"; return RGBL_E_EMPTY; }
     }
     return RGBL_OK;
@@ -818,90 +837,95 @@ static int png_status(Ctx* c, cudaStream_t st) {
     return RGBL_OK;
 }
 
-// the row pitch of an input-size image of ch bytes per pixel (64-byte rows); in_pitch = input_pitch(c, in_ch)
-static int input_pitch(const Ctx* c, int ch) { return (c->in_w * ch + 63) & ~63; }
-// one image plane of a stage slot: an input-size image of the context's channel count, without the frame slot around it
-static size_t raw_plane_bytes(const Ctx* c) { return (size_t)c->in_pitch * c->in_h; }
+// The kernel that writes level 0 from a batch of `kind` with ch bytes per pixel: System::TrackStereo's remap (rectification on), else
+// TrackRGBD's / TrackStereo's resize (input resize on; RGB-D depth images too), else GrabImage*'s cvtColor of colour images, which the
+// remap and the resize also apply; direct: the upload writes level 0.  All but direct read the batch's raw planes (LoadedInput).
+enum class Level0 { direct, gray, resize, remap };
+static Level0 level0_writer(const Ctx* c, InputKind kind, int ch) {
+    if (kind == InputKind::stereo && c->input.rectify) return Level0::remap;
+    if (kind != InputKind::rgbl && c->input.resize) return Level0::resize;
+    return ch > 1 ? Level0::gray : Level0::direct;
+}
+static bool depth_resized(const Ctx* c) { return level0_writer(c, InputKind::rgbd, 1) == Level0::resize; }
 
-// the input of `kind` goes through a kernel that reads the whole image before level 0 is written: System::TrackStereo's remap (stereo
-// pairs, rectification on) or TrackRGBD's / TrackStereo's resize (input resize on)
-static bool raw_stage(const Ctx* c, InputKind kind) { return (kind == InputKind::stereo && c->rectify) || (kind != InputKind::rgbl && c->resize); }
-
-// Where the image planes (ch bytes per pixel) of the batch being loaded go: into stage slot `slot` if given, else level 0 of the frame slots.
-// With a raw stage (raw_stage) or colour images, process_* write level 0 from raw planes and nothing else writes it: the raw planes
-// (raw_src) are the planes of the slot `staged` that already holds them (base == nullptr: nothing to copy), or else d_raw_img.  Records
-// what the raw planes hold (raw_ch, raw_w0 = the context's weight, raw_pitch).
+// Where the image planes (ch bytes per pixel) of the batch being loaded go: into stage slot `slot` if given, else level 0 of the frame
+// slots.  With a level-0 writer (level0_writer), the raw planes it reads, recorded in `loaded` with the context's gray weight: the
+// planes of the slot `staged` that already holds them (base == nullptr: nothing to copy), or else d_raw_img.
 static int image_planes(Ctx* c, InputKind kind, int ch, Ctx::StageSlot* slot, const Ctx::StageSlot* staged, Planes* p) {
-    const bool raw = ch > 1 || raw_stage(c, kind);
-    if (slot) { *p = {slot->img, raw_plane_bytes(c), 0, c->in_pitch, raw, c->in_w, c->in_h, ch}; return RGBL_OK; }
-    if (!raw) { *p = level0_planes(c); c->raw_ch = 0; return RGBL_OK; }
-    const int pitch = staged ? c->in_pitch : input_pitch(c, ch);
-    if (staged) *p = {nullptr, 0, 0, 0, true, 0, 0};
-    else if (!ensure(c->d_raw_img, (size_t)c->cfg.max_batch * pitch * c->in_h)) { c->err = "device allocation failed (raw image planes)"; return RGBL_E_CUDA; }
-    else *p = {c->d_raw_img, (size_t)pitch * c->in_h, 0, pitch, true, c->in_w, c->in_h, ch};
-    c->raw_src = staged ? staged->img.get() : c->d_raw_img.get();
-    c->raw_ch = ch; c->raw_w0 = c->in_w0; c->raw_pitch = pitch;
+    const InputSetting& in = c->input;
+    if (slot) { *p = {slot->img, in.plane_bytes(), 0, in.pitch, in.w, in.h, ch}; return RGBL_OK; }
+    if (level0_writer(c, kind, ch) == Level0::direct) { *p = level0_planes(c); c->loaded.ch = 0; return RGBL_OK; }
+    const int pitch = staged ? in.pitch : input_pitch(c, ch);
+    if (staged) *p = {};
+    else if (!ensure(c->d_raw_img, (size_t)c->cfg.max_batch * pitch * in.h)) { c->err = "device allocation failed (raw image planes)"; return RGBL_E_CUDA; }
+    else *p = {c->d_raw_img, (size_t)pitch * in.h, 0, pitch, in.w, in.h, ch};
+    c->loaded = {staged ? staged->img.get() : c->d_raw_img.get(), ch, in.w0, pitch, c->loaded.depth};
     return RGBL_OK;
 }
 
-// n PNG streams into the image planes of the batch being loaded (image_planes).  Without a raw stage the unfilter kernel converts to gray
-// and writes level 0.  With one, the reference remaps or resizes the image imread returned and converts it to gray afterwards, which differs
+// n PNG streams into the image planes of the batch being loaded (image_planes).  Without a level-0 writer the unfilter kernel converts to
+// gray and writes level 0.  With the remap or the resize, the reference converts the image imread returned to gray after it, which differs
 // for colour images: the raw planes then take the reconstructed pixels as they are, colour streams on a colour context only (a gray
 // context refuses them).  The file's samples are in R, G, B order, imread's in B, G, R: channel 0 gets the red weight when camera_rgb is 0.
 static int decode_png_gray(Ctx* c, InputKind kind, int n_frames, const uint8_t* const* png, const size_t* png_bytes, int camera_rgb, cudaStream_t st) {
-    const bool raw = raw_stage(c, kind);
-    const char* gray_only = !raw || c->in_ch > 1 ? nullptr
-                          : kind == InputKind::stereo && c->rectify ? "rectified stereo takes 8-bit gray PNGs only on a gray context (the reference remaps colour images before their conversion to gray; rgbl_set_input_channels)"
-                                                                    : "with the input resize on, image PNGs must be 8-bit gray on a gray context (the reference resizes colour images before their conversion to gray; rgbl_set_input_channels)";
-    const int ch = inflate_png_batch(c, n_frames, png, png_bytes, raw ? c->in_w : c->cfg.width, raw ? c->in_h : c->cfg.height, false, st, gray_only);
+    const Level0 writer = level0_writer(c, kind, 1);
+    const bool raw = writer != Level0::direct;
+    const char* gray_only = !raw || c->input.ch > 1 ? nullptr
+                          : writer == Level0::remap ? "rectified stereo takes 8-bit gray PNGs only on a gray context (the reference remaps colour images before their conversion to gray; rgbl_set_input_channels)"
+                                                    : "with the input resize on, image PNGs must be 8-bit gray on a gray context (the reference resizes colour images before their conversion to gray; rgbl_set_input_channels)";
+    const int ch = inflate_png_batch(c, n_frames, png, png_bytes, raw ? c->input.w : c->cfg.width, raw ? c->input.h : c->cfg.height, false, st, gray_only);
     if (ch < 0) return ch;
     Planes p;
     int rc = image_planes(c, kind, raw ? ch : 1, nullptr, nullptr, &p); if (rc) return rc;
     if (p.ch > 1) {
         launch_png_unfilter_pixels(st, c->d_png_raw, c->png_raw_stride, p.w, p.h, ch, p.base, p.stride, p.pitch, c->d_png_band, c->d_png_status, n_frames);
-        c->raw_w0 = camera_rgb ? 3735 : 9798;
+        c->loaded.w0 = camera_rgb ? 3735 : 9798;
     } else {
         LevelGeom g = c->levels[0];
         g.off = p.off; g.pitch = p.pitch;
-        launch_png_unfilter_gray(st, c->d_png_raw, c->png_raw_stride, p.w, p.h, ch, p.raw ? 0 : camera_rgb, p.base, p.stride, g,
+        launch_png_unfilter_gray(st, c->d_png_raw, c->png_raw_stride, p.w, p.h, ch, raw ? 0 : camera_rgb, p.base, p.stride, g,
                                  c->d_png_band, c->d_png_status, n_frames);
     }
     return png_status(c, st);
 }
 
 static size_t depth16_frame_elems(const Ctx* c) { return c->depth16_pitch * c->cfg.height; }
-// the depth planes RGB-D input lands in (d_depth16_raw with the resize on, else d_depth16; a stage slot's planes): pitch and frame size
-static size_t depth16_in_pitch(const Ctx* c) { return c->resize ? c->depth16_raw_pitch : c->depth16_pitch; }
-static size_t depth16_in_frame_elems(const Ctx* c) { return depth16_in_pitch(c) * c->in_h; }
 
 static int ensure_depth16(Ctx* c) {
     c->depth16_pitch = ((size_t)c->cfg.width * sizeof(uint16_t) + 63) / 64 * 32;
     if (!ensure(c->d_depth16, c->depth16_pitch * c->cfg.height * c->cfg.max_batch)) { c->err = "device allocation failed (RGB-D depth planes)"; return RGBL_E_CUDA; }
-    if (c->resize && !ensure(c->d_depth16_raw, depth16_in_frame_elems(c) * c->cfg.max_batch)) { c->err = "device allocation failed (RGB-D input-size depth planes)"; return RGBL_E_CUDA; }
+    if (depth_resized(c) && !ensure(c->d_depth16_raw, c->input.depth_elems() * c->cfg.max_batch)) { c->err = "device allocation failed (RGB-D input-size depth planes)"; return RGBL_E_CUDA; }
     return RGBL_OK;
 }
 
+// Where the input-size depth images of the RGB-D batch being loaded go: into stage slot `slot` if given, else d_depth16, or with the depth
+// resize into its source, recorded in `loaded`: the slot `staged` that already holds them (nullptr: nothing to copy), or else d_depth16_raw.
+static uint16_t* depth_planes(Ctx* c, Ctx::StageSlot* slot, const Ctx::StageSlot* staged) {
+    if (slot) return slot->depth;
+    if (!depth_resized(c)) return c->d_depth16;
+    c->loaded.depth = staged ? staged->depth.get() : c->d_depth16_raw.get();
+    return staged ? nullptr : c->d_depth16_raw.get();
+}
+
 // cv::imread(depth PNG, IMREAD_UNCHANGED) of Examples/RGB-D/rgbd_kitti.cc into the uint16 depth planes of frame slots 0..n_frames-1
-// (16-bit gray only); shares the staging buffer with the image decode, one after the other.  input_size: the streams are camera input,
-// decoded at the input size (into d_depth16_raw, the depth resize's source, while the resize is on); else at the context's size.
-static int decode_png_to_depth16(Ctx* c, int n_frames, const uint8_t* const* png, const size_t* png_bytes, cudaStream_t st, bool input_size) {
+// (16-bit gray only); shares the staging buffer with the image decode, one after the other.  camera: the streams are camera input,
+// decoded at the input size into the depth planes of the batch being loaded (depth_planes); else at the context's size into d_depth16.
+static int decode_png_to_depth16(Ctx* c, int n_frames, const uint8_t* const* png, const size_t* png_bytes, cudaStream_t st, bool camera) {
     int rc = ensure_depth16(c); if (rc) return rc;
-    const bool rs = input_size && c->resize;
-    const int w = rs ? c->in_w : c->cfg.width, h = rs ? c->in_h : c->cfg.height;
+    const int w = camera ? c->input.w : c->cfg.width, h = camera ? c->input.h : c->cfg.height;
     const int ch = inflate_png_batch(c, n_frames, png, png_bytes, w, h, true, st);
     if (ch < 0) return ch;
-    uint16_t* dst = rs ? c->d_depth16_raw.get() : c->d_depth16.get();
-    launch_png_unfilter_depth16(st, c->d_png_raw, c->png_raw_stride, w, h, dst, rs ? depth16_in_frame_elems(c) : depth16_frame_elems(c),
-                                rs ? c->depth16_raw_pitch : c->depth16_pitch, c->d_png_band, c->d_png_status, n_frames);
-    if (rs) c->depth_src = dst;
+    uint16_t* dst = camera ? depth_planes(c, nullptr, nullptr) : c->d_depth16.get();
+    launch_png_unfilter_depth16(st, c->d_png_raw, c->png_raw_stride, w, h, dst, camera ? c->input.depth_elems() : depth16_frame_elems(c),
+                                camera ? c->input.depth_pitch : c->depth16_pitch, c->d_png_band, c->d_png_status, n_frames);
     return png_status(c, st);
 }
 
 // device buffers of a stage slot (allocated on first use, grown for a larger input size; a slot can hold batches of each kind in turn)
 static int stage_slot_alloc(Ctx* c, Ctx::StageSlot& sl, InputKind kind) {
     const size_t B = c->cfg.max_batch;
-    bool ok = ensure(sl.img, B * raw_plane_bytes(c));         // stereo: the left and the right planes, 2 n_pairs <= max_batch
-    if (ok && kind == InputKind::rgbd) ok = ensure(sl.depth, B * depth16_in_frame_elems(c));
+    bool ok = ensure(sl.img, B * c->input.plane_bytes());     // stereo: the left and the right planes, 2 n_pairs <= max_batch
+    if (ok && kind == InputKind::rgbd) ok = ensure(sl.depth, B * c->input.depth_elems());
     if (ok && kind == InputKind::rgbl) ok = ensure(sl.pts, B * 4 * c->cfg.max_points) && ensure(sl.n_pts, B);
     if (!ok) { c->err = "device allocation failed (stage slot)"; return RGBL_E_CUDA; }
     return RGBL_OK;
@@ -923,11 +947,10 @@ static int copy_inputs(Ctx* c, const HostInputs& in, int max_pts, Ctx::StageSlot
         CU(cudaMemcpyAsync(slot ? slot->n_pts.get() : c->d_n_pts.get(), c->h_n_pts, (size_t)in.n * sizeof(int), cudaMemcpyHostToDevice, c->st_aux));
         if (kitti && max_pts > 0) launch_deinterleave_xyzr(c->st_aux, c->d_pts_raw, c->d_pts, 4 * c->cfg.max_points, c->d_n_pts, max_pts, in.n);
     } else if (in.kind == InputKind::rgbd) {
-        uint16_t* depth = slot ? slot->depth.get() : c->resize ? c->d_depth16_raw.get() : c->d_depth16.get();
-        if (!slot && c->resize) c->depth_src = depth;
+        uint16_t* depth = depth_planes(c, slot, nullptr);
         for (int f = 0; f < in.n; ++f)
-            CU(cudaMemcpy2DAsync(depth + (size_t)f * depth16_in_frame_elems(c), depth16_in_pitch(c) * sizeof(uint16_t), in.depth[f],
-                                 (size_t)in.depth_stride * sizeof(uint16_t), (size_t)c->in_w * sizeof(uint16_t), c->in_h, cudaMemcpyHostToDevice, c->st_aux));
+            CU(cudaMemcpy2DAsync(depth + (size_t)f * c->input.depth_elems(), c->input.depth_pitch * sizeof(uint16_t), in.depth[f],
+                                 (size_t)in.depth_stride * sizeof(uint16_t), (size_t)c->input.w * sizeof(uint16_t), c->input.h, cudaMemcpyHostToDevice, c->st_aux));
     }
     if (!in.gray) return RGBL_OK;          // level 0 was written by a PNG decode
     Planes p;
@@ -961,46 +984,44 @@ static int stage_inputs(Ctx* c, int slot, const HostInputs& in) {
     rc = copy_inputs(c, in, max_pts, &sl); if (rc) return rc;
     CU(cudaStreamSynchronize(c->st));
     CU(cudaStreamSynchronize(c->st_aux));
-    sl.n_frames = in.n; sl.max_pts = max_pts; sl.kind = in.kind; sl.in_w = c->in_w; sl.in_h = c->in_h; sl.ch = in.ch;
+    sl.n_frames = in.n; sl.max_pts = max_pts; sl.kind = in.kind; sl.input = c->input;
     return RGBL_OK;
 }
 
-// The level0 step of run_extract for the n images of the uploaded batch (stereo: n / 2 pairs, left then right), on the main stream: the raw
-// planes remapped (System::TrackStereo's cv::remap, stereo pairs with rectification on), else resized (TrackRGBD's / TrackStereo's
-// cv::resize, input resize on), else converted to gray (Tracking::GrabImage*'s cvtColor of colour input) into level 0 of frame slots
-// [0, n); colour planes are converted to gray after the remap or the resize, in the same kernel.  *step = nullptr when the upload wrote
-// level 0 itself.  With the rectification and the resize both on, the remap alone reads the input-size planes: the maps have the
-// context's size and their coordinates index the input-size images (Settings builds them with initUndistortRectifyMap(..., newImSize_, ...)).
+// The level0 step of run_extract for the n images of the loaded batch (stereo: n / 2 pairs, left then right): its level-0 writer on the
+// main stream (nullptr: direct).  With both the rectification and the resize on, the remap reads the input-size planes: its maps have the
+// context's size and index the input-size images (Settings builds them with initUndistortRectifyMap(..., newImSize_, ...)).
 static int level0_step(Ctx* c, InputKind kind, int n, std::function<int()>* step) {
-    const bool remap = kind == InputKind::stereo && c->rectify, resize = raw_stage(c, kind) && !remap;
+    const Level0 writer = level0_writer(c, kind, c->loaded.ch);
     *step = nullptr;
-    if (!remap && !resize && !c->raw_ch) return RGBL_OK;
-    if (!c->raw_src || !c->raw_ch) { c->err = remap ? "no raw stereo planes to rectify" : "no input-size planes to resize"; return RGBL_E_INVALID; }
-    *step = [c, n, remap, resize]() {
-        const size_t stride = (size_t)c->raw_pitch * c->in_h;
+    if (writer == Level0::direct) return RGBL_OK;
+    if (!c->loaded.img || !c->loaded.ch) { c->err = writer == Level0::remap ? "no raw stereo planes to rectify" : "no input-size planes to resize"; return RGBL_E_INVALID; }
+    *step = [c, n, writer]() {
+        const LoadedInput& ld = c->loaded;
+        const size_t stride = (size_t)ld.pitch * c->input.h;
         LevelGeom src{};
-        src.w = c->in_w; src.h = c->in_h; src.pitch = c->raw_pitch;
-        if (remap) {
+        src.w = c->input.w; src.h = c->input.h; src.pitch = ld.pitch;
+        if (writer == Level0::remap) {
             const LevelGeom& l0 = c->levels[0];
             RectifyDev r{};
             r.xy = c->d_rect_xy; r.a = c->d_rect_a; r.map_pitch = c->rect_pitch;
-            r.W = c->cfg.width; r.H = c->cfg.height; r.src_W = c->in_w; r.src_H = c->in_h;
-            r.src = c->raw_src; r.src_stride = stride; r.src_pitch = c->raw_pitch; r.ch = c->raw_ch; r.w0 = c->raw_w0;
+            r.W = c->cfg.width; r.H = c->cfg.height; r.src_W = c->input.w; r.src_H = c->input.h;
+            r.src = ld.img; r.src_stride = stride; r.src_pitch = ld.pitch; r.ch = ld.ch; r.w0 = ld.w0;
             r.dst = c->d_pyr; r.dst_stride = c->frame_bytes; r.dst_off = l0.off; r.dst_pitch = l0.pitch;
             launch_rectify(c->st, r, n / 2);
-        } else if (resize) {
-            launch_resize_planes(c->st, c->raw_src, stride, src, c->d_pyr, c->frame_bytes, c->levels[0], c->d_resize_coefs,
-                                 c->d_resize_coefs + c->cfg.width, n, c->raw_ch, c->raw_w0);
+        } else if (writer == Level0::resize) {
+            launch_resize_planes(c->st, ld.img, stride, src, c->d_pyr, c->frame_bytes, c->levels[0], c->d_resize_coefs,
+                                 c->d_resize_coefs + c->cfg.width, n, ld.ch, ld.w0);
         } else {
-            launch_gray_planes(c->st, c->raw_src, stride, src, c->d_pyr, c->frame_bytes, c->levels[0], c->raw_ch, c->raw_w0, n);
+            launch_gray_planes(c->st, ld.img, stride, src, c->d_pyr, c->frame_bytes, c->levels[0], ld.ch, ld.w0, n);
         }
         return 1;
     };
     return RGBL_OK;
 }
 
-// Everything of Frame::Frame (RGB-L) after the inputs are in HBM: (colour input: the gray conversion into level 0), depth maps (aux
-// stream) || extraction, then gather.
+// Everything of Frame::Frame (RGB-L) after the inputs are in HBM: (colour input: the gray conversion into level 0, level0_step), depth
+// maps (aux stream) || extraction, then gather.
 static int process_rgbl(Ctx* c, int n_frames, int max_pts, const float P[12], const rgbl_depth_params* prm) {
     DepthDev dd;
     int rc = setup_depth(c, P, prm, dd); if (rc) return rc;
@@ -1016,18 +1037,17 @@ static int process_rgbl(Ctx* c, int n_frames, int max_pts, const float P[12], co
 
 // Everything of the RGB-D Frame constructor (src/Frame.cc:200-237) after the inputs are in HBM: extraction, UndistortKeyPoints (context's
 // camera, rgbl_set_camera_distortion), then ComputeStereoFromRGBD as the gather of the uint16 depth plane, scaled per pixel like
-// GrabImageRGBD's convertTo.  With the input resize on, System::TrackRGBD's two cv::resize run first (src/System.cc, TrackRGBD): the images
-// into level 0 (main stream, billed to the pyramid stage), the depth images into d_depth16 (aux stream, behind the blur and overlapping the
-// quad-tree, billed to the depth_gather stage); the gather waits for both through run_extract's ev_blur.
+// GrabImageRGBD's convertTo.  With the input resize on, System::TrackRGBD's cv::resize of the depth images (src/System.cc) writes d_depth16
+// on the aux stream, behind the blur and overlapping the quad-tree (billed to depth_gather); the gather waits for it through ev_blur.
 static int process_rgbd(Ctx* c, int n_frames, float depth_scale, float bf) {
     std::function<int()> level0;
     std::function<void()> depth_resize;
     int rc = level0_step(c, InputKind::rgbd, n_frames, &level0); if (rc) return rc;
-    if (c->resize) {
-        if (!c->depth_src) { c->err = "no input-size planes to resize"; return RGBL_E_INVALID; }
+    if (depth_resized(c)) {
+        if (!c->loaded.depth) { c->err = "no input-size planes to resize"; return RGBL_E_INVALID; }
         depth_resize = [&]() {
             if (c->prof_on) cudaEventRecord(c->ev_rsd_b, c->st_aux);
-            launch_resize_depth16(c->st_aux, c->depth_src, depth16_in_frame_elems(c), c->depth16_raw_pitch, c->resize_kx, c->resize_ky, c->d_depth16,
+            launch_resize_depth16(c->st_aux, c->loaded.depth, c->input.depth_elems(), c->input.depth_pitch, c->input.kx, c->input.ky, c->d_depth16,
                                   depth16_frame_elems(c), c->depth16_pitch, c->cfg.width, c->cfg.height, n_frames);
             if (c->prof_on) { cudaEventRecord(c->ev_rsd_e, c->st_aux); c->rsd_used = true; }
             c->total_launches += 1;
@@ -1055,10 +1075,7 @@ static int check_rgbd_params(Ctx* c, float depth_scale, float bf) {
 // both extracted as one batch of 2n frames (the reference's two ORBextractor threads), then ComputeStereoMatches.  The left frames are
 // then the batch (last_frames = n) for download, ComputeBoW and the tracking chain.  The capacity-overflow flags cover all 2n frames,
 // so an overflow in a right frame, which changes the left frame's depths, fails the chain's _end2 like a left-frame overflow.
-// With rectification on, the raw planes of the pairs (raw_src) are first remapped into level 0 of the slots, in one launch billed to the
-// pyramid stage: System::TrackStereo's cv::remap of both images (src/System.cc:251 ff.).  Else, with the input resize on, they are resized
-// into level 0 in the same way (TrackStereo's cv::resize, the branch after the rectification's); colour pairs are converted to gray
-// after either, or alone (level0_step).
+// The pairs' level-0 writer (TrackStereo's cv::remap or cv::resize, src/System.cc:251 ff.) runs first, billed to the pyramid stage.
 static int process_stereo(Ctx* c, int n_pairs, float mb, float mbf) {
     std::function<int()> level0;
     int rc = level0_step(c, InputKind::stereo, 2 * n_pairs, &level0); if (rc) return rc;
@@ -1080,15 +1097,13 @@ static int check_stereo(Ctx* c, int n_pairs) {
 // RGB-L input is never resized: the reference's Settings do not handle RGB-L (System::TrackRGBL's resize branch never runs), and the LiDAR
 // projection P describes the original image
 static int check_rgbl_input(Ctx* c) {
-    if (c->resize) { c->err = "RGB-L input is never resized: clear the input resize (rgbl_set_input_resize(ctx, 0, 0))"; return RGBL_E_UNSUPPORTED; }
+    if (c->input.resize) { c->err = "RGB-L input is never resized: clear the input resize (rgbl_set_input_resize(ctx, 0, 0))"; return RGBL_E_UNSUPPORTED; }
     return RGBL_OK;
 }
 
 // RGB-D input with the resize on: the depth resize restates OpenCV's 16-bit INTER_LINEAR at integer factors only
 static int check_rgbd_input(Ctx* c) {
-    if (c->resize && !(c->resize_kx && c->resize_ky)) {
-        c->err = "RGB-D input resize needs integer factors (input width / width and input height / height)"; return RGBL_E_UNSUPPORTED;
-    }
+    if (depth_resized(c) && !(c->input.kx && c->input.ky)) { c->err = "RGB-D input resize needs integer factors (input width / width and input height / height)"; return RGBL_E_UNSUPPORTED; }
     return RGBL_OK;
 }
 
@@ -1141,7 +1156,7 @@ int rgbl_frame_rgbl_batch(rgbl_ctx* ctx, int n_frames, const uint8_t* const* gra
     if (!c) return RGBL_E_INVALID;
     if (!gray || !pts4xn || !n_pts || !P || !prm || !kps || !desc || !depth || !uright || !n_out) { c->err = "null argument"; return RGBL_E_INVALID; }
     int rc = check_rgbl_input(c); if (rc) return rc;
-    rc = check_batch_args(c, n_frames, width, height, stride); if (rc) return rc;
+    rc = check_images(c, gray_images(c), n_frames, width, height, stride); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     rc = upload_inputs(c, HostInputs::rgbl(n_frames, gray, stride, pts4xn, n_pts)); if (rc) return rc;
     rc = process_rgbl(c, n_frames, c->resident_max_pts, P, prm); if (rc < 0) return rc;
@@ -1156,7 +1171,7 @@ int rgbl_resident_upload(rgbl_ctx* ctx, int n_frames, const uint8_t* const* gray
     if (!c) return RGBL_E_INVALID;
     if (!gray || !pts4xn || !n_pts) { c->err = "null argument"; return RGBL_E_INVALID; }
     int rc = check_rgbl_input(c); if (rc) return rc;
-    rc = check_batch_args(c, n_frames, width, height, stride, true, c->in_ch); if (rc) return rc;
+    rc = check_images(c, c->input, n_frames, width, height, stride); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     return upload_inputs_sync(c, HostInputs::rgbl(n_frames, gray, stride, pts4xn, n_pts).camera(c));
 }
@@ -1167,7 +1182,7 @@ int rgbl_resident_upload_kitti(rgbl_ctx* ctx, int n_frames, const uint8_t* const
     if (!c) return RGBL_E_INVALID;
     if (!gray || !xyzr || !n_pts) { c->err = "null argument"; return RGBL_E_INVALID; }
     int rc = check_rgbl_input(c); if (rc) return rc;
-    rc = check_batch_args(c, n_frames, width, height, stride, true, c->in_ch); if (rc) return rc;
+    rc = check_images(c, c->input, n_frames, width, height, stride); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     return upload_inputs_sync(c, HostInputs::rgbl(n_frames, gray, stride, xyzr, n_pts, 1).camera(c));
 }
@@ -1178,7 +1193,7 @@ int rgbl_resident_upload_kitti_png(rgbl_ctx* ctx, int n_frames, const uint8_t* c
     if (!c) return RGBL_E_INVALID;
     if (!png || !png_bytes || !xyzr || !n_pts) { c->err = "null argument"; return RGBL_E_INVALID; }
     int rc = check_rgbl_input(c); if (rc) return rc;
-    rc = check_batch_args(c, n_frames, c->cfg.width, c->cfg.height, c->cfg.width); if (rc) return rc;
+    rc = check_batch(c, n_frames); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     rc = decode_png_gray(c, InputKind::rgbl, n_frames, png, png_bytes, camera_rgb, c->st); if (rc) return rc;
     return upload_inputs_sync(c, HostInputs::rgbl(n_frames, nullptr, 0, xyzr, n_pts, 1));
@@ -1189,7 +1204,7 @@ int rgbl_decode_png_gray(rgbl_ctx* ctx, int n_frames, const uint8_t* const* png,
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
     if (!png || !png_bytes || !gray_out) { c->err = "null argument"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_frames, c->cfg.width, c->cfg.height, stride, false); if (rc) return rc;
+    int rc = check_images(c, gray_images(c), n_frames, c->cfg.width, c->cfg.height, stride); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     rc = decode_png_gray(c, InputKind::rgbl, n_frames, png, png_bytes, camera_rgb, c->st); if (rc) return rc;
     const Planes l0 = level0_planes(c);
@@ -1226,7 +1241,7 @@ int rgbl_resident_stage(rgbl_ctx* ctx, int slot, int n_frames, const uint8_t* co
     if (slot < 0 || slot >= Ctx::kMaxStageSlots) { c->err = "stage slot out of range"; return RGBL_E_INVALID; }
     if (!c->d_pts) { c->err = "context was created with max_points == 0"; return RGBL_E_INVALID; }
     int rc = check_rgbl_input(c); if (rc) return rc;
-    rc = check_batch_args(c, n_frames, width, height, stride, true, c->in_ch); if (rc) return rc;
+    rc = check_images(c, c->input, n_frames, width, height, stride); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     return stage_inputs(c, slot, HostInputs::rgbl(n_frames, gray, stride, pts4xn, n_pts).camera(c));
 }
@@ -1238,7 +1253,7 @@ int rgbl_resident_stage_rgbd(rgbl_ctx* ctx, int slot, int n_frames, const uint8_
     if (!gray || !depth) { c->err = "null argument"; return RGBL_E_INVALID; }
     if (slot < 0 || slot >= Ctx::kMaxStageSlots) { c->err = "stage slot out of range"; return RGBL_E_INVALID; }
     int rc = check_rgbd_input(c); if (rc) return rc;
-    rc = check_batch_args(c, n_frames, width, height, stride, true, c->in_ch); if (rc) return rc;
+    rc = check_images(c, c->input, n_frames, width, height, stride); if (rc) return rc;
     if (depth_stride < width) { c->err = "depth_stride < width"; return RGBL_E_INVALID; }
     CU(cudaSetDevice(c->cfg.device));
     return stage_inputs(c, slot, HostInputs::rgbd(n_frames, gray, stride, depth, depth_stride).camera(c));
@@ -1250,7 +1265,7 @@ int rgbl_resident_stage_stereo(rgbl_ctx* ctx, int slot, int n_pairs, const uint8
     if (!c) return RGBL_E_INVALID;
     if (!left || !right) { c->err = "null argument"; return RGBL_E_INVALID; }
     if (slot < 0 || slot >= Ctx::kMaxStageSlots) { c->err = "stage slot out of range"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_pairs, width, height, stride, true, c->in_ch); if (rc) return rc;
+    int rc = check_images(c, c->input, n_pairs, width, height, stride); if (rc) return rc;
     rc = check_stereo(c, n_pairs); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     return stage_inputs(c, slot, HostInputs::stereo(n_pairs, left, right, stride).camera(c));
@@ -1266,18 +1281,17 @@ static int restage(Ctx* c, int slot, InputKind kind) {
         c->err = std::string("stage slot holds ") + k.what + " (" + k.runner + ")";
         return RGBL_E_INVALID;
     }
-    if (sl.in_w != c->in_w || sl.in_h != c->in_h) { c->err = "stage slot was staged at another input size (rgbl_set_input_resize)"; return RGBL_E_INVALID; }
-    if (sl.ch != c->in_ch) { c->err = "stage slot was staged with another channel count (rgbl_set_input_channels)"; return RGBL_E_INVALID; }
+    if (sl.input.w != c->input.w || sl.input.h != c->input.h) { c->err = "stage slot was staged at another input size (rgbl_set_input_resize)"; return RGBL_E_INVALID; }
+    if (sl.input.ch != c->input.ch) { c->err = "stage slot was staged with another channel count (rgbl_set_input_channels)"; return RGBL_E_INVALID; }
     Planes dst;
-    int rc = image_planes(c, kind, sl.ch, nullptr, &sl, &dst); if (rc) return rc;
-    const size_t img_bytes = raw_plane_bytes(c);
+    int rc = image_planes(c, kind, sl.input.ch, nullptr, &sl, &dst); if (rc) return rc;
+    const size_t img_bytes = sl.input.plane_bytes();
     const int n_img = kind == InputKind::stereo ? 2 * sl.n_frames : sl.n_frames;
     if (dst.base)
         for (int f = 0; f < n_img; ++f) CU(cudaMemcpyAsync(dst.at(f), sl.img + (size_t)f * img_bytes, img_bytes, cudaMemcpyDeviceToDevice, c->st));
-    if (kind == InputKind::rgbd && c->resize) {
-        c->depth_src = sl.depth;          // read in place by the depth resize
-    } else if (kind == InputKind::rgbd) {
-        CU(cudaMemcpyAsync(c->d_depth16, sl.depth, (size_t)sl.n_frames * depth16_frame_elems(c) * sizeof(uint16_t), cudaMemcpyDeviceToDevice, c->st_aux));
+    if (kind == InputKind::rgbd) {
+        uint16_t* depth = depth_planes(c, nullptr, &sl);
+        if (depth) CU(cudaMemcpyAsync(depth, sl.depth, (size_t)sl.n_frames * sl.input.depth_elems() * sizeof(uint16_t), cudaMemcpyDeviceToDevice, c->st_aux));
     } else if (kind == InputKind::rgbl) {
         CU(cudaMemcpyAsync(c->d_pts, sl.pts, (size_t)sl.n_frames * 4 * c->cfg.max_points * sizeof(float), cudaMemcpyDeviceToDevice, c->st_aux));
         CU(cudaMemcpyAsync(c->d_n_pts, sl.n_pts, (size_t)sl.n_frames * sizeof(int), cudaMemcpyDeviceToDevice, c->st_aux));
@@ -1293,7 +1307,7 @@ static int check_sequence_io(Ctx* c, const rgbl_chain_params* chain, const rgbl_
     if (T < 1 || T > c->cfg.max_batch || nb < 1) { c->err = "bad batch geometry"; return RGBL_E_INVALID; }
     if (const int rc = require_idle(c)) return rc;
     if (io->gray) {
-        int rc = check_batch_args(c, T, io->width, io->height, io->stride, true, c->in_ch); if (rc) return rc;
+        int rc = check_images(c, c->input, T, io->width, io->height, io->stride); if (rc) return rc;
     } else if (io->n_slots < 1 || io->n_slots > Ctx::kMaxStageSlots) { c->err = "resident mode needs 1..8 staged slots"; return RGBL_E_INVALID; }
     if (io->kps && (!io->desc || !io->depth || !io->uright || !io->n_kp || io->cap != c->cap_kp)) {
         c->err = "frame outputs need kps, desc, depth, uright, n_kp and cap == rgbl_keypoint_capacity()"; return RGBL_E_INVALID;
@@ -1400,7 +1414,7 @@ int rgbl_resident_upload_rgbd(rgbl_ctx* ctx, int n_frames, const uint8_t* const*
     if (!c) return RGBL_E_INVALID;
     if (!gray || !depth) { c->err = "null argument"; return RGBL_E_INVALID; }
     int rc = check_rgbd_input(c); if (rc) return rc;
-    rc = check_batch_args(c, n_frames, width, height, stride, true, c->in_ch); if (rc) return rc;
+    rc = check_images(c, c->input, n_frames, width, height, stride); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     return upload_inputs_sync(c, HostInputs::rgbd(n_frames, gray, stride, depth, depth_stride).camera(c));
 }
@@ -1411,7 +1425,7 @@ int rgbl_resident_upload_rgbd_png(rgbl_ctx* ctx, int n_frames, const uint8_t* co
     if (!c) return RGBL_E_INVALID;
     if (!png || !png_bytes || !depth_png || !depth_png_bytes) { c->err = "null argument"; return RGBL_E_INVALID; }
     int rc = check_rgbd_input(c); if (rc) return rc;
-    rc = check_batch_args(c, n_frames, c->in_w, c->in_h, c->in_w); if (rc) return rc;
+    rc = check_batch(c, n_frames); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     rc = decode_png_gray(c, InputKind::rgbd, n_frames, png, png_bytes, camera_rgb, c->st); if (rc) return rc;
     rc = decode_png_to_depth16(c, n_frames, depth_png, depth_png_bytes, c->st, true); if (rc) return rc;
@@ -1423,7 +1437,7 @@ int rgbl_decode_png_depth16(rgbl_ctx* ctx, int n_frames, const uint8_t* const* p
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
     if (!png || !png_bytes || !depth_out) { c->err = "null argument"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_frames, c->cfg.width, c->cfg.height, stride, false); if (rc) return rc;
+    int rc = check_images(c, gray_images(c), n_frames, c->cfg.width, c->cfg.height, stride); if (rc) return rc;
     for (int f = 0; f < n_frames; ++f) if (!depth_out[f]) { c->err = "null output image"; return RGBL_E_INVALID; }
     CU(cudaSetDevice(c->cfg.device));
     rc = decode_png_to_depth16(c, n_frames, png, png_bytes, c->st, false); if (rc) return rc;
@@ -1449,7 +1463,7 @@ int rgbl_resident_upload_stereo(rgbl_ctx* ctx, int n_pairs, const uint8_t* const
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
     if (!left || !right) { c->err = "null argument"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_pairs, width, height, stride, true, c->in_ch); if (rc) return rc;
+    int rc = check_images(c, c->input, n_pairs, width, height, stride); if (rc) return rc;
     rc = check_stereo(c, n_pairs); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     return upload_inputs_sync(c, HostInputs::stereo(n_pairs, left, right, stride).camera(c));
@@ -1460,7 +1474,7 @@ int rgbl_resident_upload_stereo_png(rgbl_ctx* ctx, int n_pairs, const uint8_t* c
     Ctx* c = reinterpret_cast<Ctx*>(ctx);
     if (!c) return RGBL_E_INVALID;
     if (!left_png || !left_bytes || !right_png || !right_bytes) { c->err = "null argument"; return RGBL_E_INVALID; }
-    int rc = check_batch_args(c, n_pairs, c->in_w, c->in_h, c->in_w); if (rc) return rc;
+    int rc = check_batch(c, n_pairs); if (rc) return rc;
     rc = check_stereo(c, n_pairs); if (rc) return rc;
     CU(cudaSetDevice(c->cfg.device));
     // one decode of 2n streams: every stream must have the input size, so left and right sizes that differ are an error
@@ -1492,11 +1506,7 @@ int rgbl_set_stereo_rectification(rgbl_ctx* ctx, const float* m1l, const float* 
     const float* maps[4] = {m1l, m2l, m1r, m2r};
     int n_null = 0;
     for (const float* m : maps) n_null += m == nullptr;
-    if (n_null == 4) {
-        c->rectify = false;
-        if (c->resident_kind == InputKind::stereo) c->resident_frames = 0;      // the uploaded pairs were staged for the other setting
-        return RGBL_OK;
-    }
+    if (n_null == 4) { c->input.rectify = false; input_changed(c, true); return RGBL_OK; }
     if (n_null) { c->err = "the four rectification maps are all given or all NULL"; return RGBL_E_INVALID; }
     const int W = c->cfg.width, H = c->cfg.height;
     if (map_stride < W) { c->err = "map_stride < width"; return RGBL_E_INVALID; }
@@ -1516,8 +1526,7 @@ int rgbl_set_stereo_rectification(rgbl_ctx* ctx, const float* m1l, const float* 
     launch_rectify_maps(c->st, staged, W, H, c->d_rect_xy, c->d_rect_a, c->rect_pitch);
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(c->st));
-    c->rectify = true;
-    if (c->resident_kind == InputKind::stereo) c->resident_frames = 0;
+    c->input.rectify = true; input_changed(c, true);
     return RGBL_OK;
 }
 
@@ -1546,13 +1555,8 @@ int rgbl_set_input_resize(rgbl_ctx* ctx, int src_width, int src_height) {
         CU(cudaStreamSynchronize(c->st));         // a batch in flight may still read the previous tables
         CU(cudaMemcpy(c->d_resize_coefs, tab.data(), tab.size() * sizeof(LinCoef), cudaMemcpyHostToDevice));
     }
-    c->resize = on;
-    c->in_w = on ? src_width : W; c->in_h = on ? src_height : H;
-    c->in_pitch = input_pitch(c, c->in_ch);
-    c->resize_kx = c->in_w % W == 0 ? c->in_w / W : 0;
-    c->resize_ky = c->in_h % H == 0 ? c->in_h / H : 0;
-    c->depth16_raw_pitch = ((size_t)c->in_w * sizeof(uint16_t) + 63) / 64 * 32;
-    c->resident_frames = 0;                   // the uploaded batch was loaded for the other setting
+    c->input.resize = on; c->input.w = on ? src_width : W; c->input.h = on ? src_height : H;
+    input_changed(c);
     return RGBL_OK;
 }
 
@@ -1564,10 +1568,8 @@ int rgbl_set_input_channels(rgbl_ctx* ctx, int channels, int camera_rgb) {
     if ((channels != 1 && channels != 3 && channels != 4) || (camera_rgb != 0 && camera_rgb != 1)) {
         c->err = "channels must be 1, 3 or 4 and camera_rgb 0 or 1"; return RGBL_E_INVALID;
     }
-    c->in_ch = channels;
-    c->in_w0 = camera_rgb ? 9798 : 3735;      // mbRGB: COLOR_RGB2GRAY weights channel 0 as red, COLOR_BGR2GRAY as blue
-    c->in_pitch = input_pitch(c, channels);
-    c->resident_frames = 0;                   // the uploaded batch was loaded for the other setting
+    c->input.ch = channels; c->input.w0 = camera_rgb ? 9798 : 3735;      // mbRGB: COLOR_RGB2GRAY weights channel 0 as red, COLOR_BGR2GRAY as blue
+    input_changed(c);
     return RGBL_OK;
 }
 

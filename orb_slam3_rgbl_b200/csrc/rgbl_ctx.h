@@ -24,6 +24,23 @@ constexpr int kMatchListCap = 512;    // admissible candidates kept per map poin
 // right image of a pair: rectified, or raw when the context rectifies them)
 enum class InputKind { rgbl, rgbd, stereo };
 
+// The camera-input setting (rgbl_set_input_resize / _channels, rgbl_set_stereo_rectification): images of w x h (Settings' original camera
+// size; the context's unless `resize`, which resizes RGB-D and stereo input to it) and ch bytes per pixel (1, or 3 / 4 interleaved) whose
+// channel 0 has the gray weight w0 (gray_of: 9798 with Camera.RGB = 1, else 3735); unrectified stereo pairs with `rectify`.  Derived by
+// input_changed (api.cu): the row pitches of an image (bytes) and an input-size depth image (elements), the depth resize's integer factors.
+struct InputSetting {
+    int w = 0, h = 0, ch = 1, w0 = 3735; bool resize = false, rectify = false;
+    int pitch = 0, kx = 0, ky = 0; size_t depth_pitch = 0;
+    size_t plane_bytes() const { return (size_t)pitch * h; }     // one input image, without the frame slot around it
+    size_t depth_elems() const { return depth_pitch * h; }       // one input-size depth image
+};
+
+// What the loaded batch holds for the kernels that write level 0 (api.cu: level0_writer): its images as raw planes at img (plane z at
+// img + z * pitch * input.h, ch bytes per pixel, gray weight w0 of channel 0; ch = 0: the upload wrote level 0 itself), recorded per
+// upload as a PNG stream may be gray or in R, G, B order, and depth, the input-size depth images the depth resize reads.  Each is a
+// working buffer (d_raw_img, d_depth16_raw) or a staged slot's planes, read in place.
+struct LoadedInput { const uint8_t* img = nullptr; int ch = 0, w0 = 0, pitch = 0; const uint16_t* depth = nullptr; };
+
 // Words of TrackBufs::scalars (device, 16 ints) the tracking entry points use: the frame size FrameDev::n points at, a search's match
 // count and resolution rounds (adjacent: read back as one pair), PoseOptimization's inlier count.
 constexpr int kDevFrameN = 0, kDevMatches = 1, kDevRounds = 2, kDevPoseInliers = 8;
@@ -133,36 +150,16 @@ struct Ctx {
     // referenced by the chain's CUDA graphs, so it needs no scratch_generation bump.
     DeviceArray<int> d_stereo_row_start, d_stereo_row_idx, d_stereo_sad;
     int stereo_idx_cap = 0;
-    // stereo rectification (rgbl_set_stereo_rectification, stereo_kernels.cu).  d_rect_xy / d_rect_a: OpenCV's fixed-point form of the
-    // left and right maps, H rows of rect_pitch entries per camera, allocated by the first setting and never reallocated.
-    bool rectify = false;
+    InputSetting input;
+    // stereo rectification (stereo_kernels.cu).  d_rect_xy / d_rect_a: OpenCV's fixed-point form of the left and right maps, H rows of
+    // rect_pitch entries per camera, allocated by the first setting and never reallocated.
     DeviceArray<uint32_t> d_rect_xy; DeviceArray<uint16_t> d_rect_a;
     int rect_pitch = 0;
-    // input resize (rgbl_set_input_resize): RGB-D and stereo images (and RGB-D depth images) arrive at in_w x in_h, Settings' original
-    // camera size, and are resized to the context's size before the extraction.  in_w / in_h / in_pitch are the context's width, height
-    // and level 0's pitch while the resize is off.  d_resize_coefs: the cv::resize tables of the two axes (x: W entries, then y: H entries).
-    // resize_kx / resize_ky: the integer factors of the depth resize (0: not an integer, refused for RGB-D).
-    bool resize = false;
-    int in_w = 0, in_h = 0, in_pitch = 0, resize_kx = 0, resize_ky = 0;
-    DeviceArray<LinCoef> d_resize_coefs;
-    // colour camera input (rgbl_set_input_channels): the camera-input entry points take images of in_ch bytes per pixel (1, or 3 / 4
-    // interleaved), whose channel 0 has the gray weight in_w0 (gray_of: 9798 with Camera.RGB = 1, else 3735).  in_pitch: the row pitch of
-    // an input-size image of in_ch bytes per pixel (64-byte rows).
-    int in_ch = 1, in_w0 = 3735;
-    // Raw image planes: the images of the uploaded batch before the conditioning kernel (rectification, resize or gray conversion) writes
-    // level 0 of the frame slots.  d_raw_img: max_batch planes of in_h rows, allocated by the first upload that needs them (and reallocated
-    // when a later one needs more); host uploads and PNG decodes write there instead of level 0.  raw_src: the raw planes of the uploaded
-    // batch (d_raw_img, or a staged slot's planes); raw_ch / raw_w0 / raw_pitch: what they hold (bytes per pixel, the gray weight of channel
-    // 0, row pitch; plane z at raw_src + z * raw_pitch * in_h), raw_ch = 0: the upload wrote level 0 itself.  A colour context can receive
-    // gray PNG streams, and a PNG file's samples are in R, G, B order, so these are recorded per upload.  d_depth16_raw / depth_src: the same
-    // for RGB-D depth images with the resize on (row pitch depth16_raw_pitch elements).  No chain graph references these buffers, so they
-    // need no scratch_generation bump.
-    DeviceArray<uint8_t> d_raw_img;
-    const uint8_t* raw_src = nullptr;
-    int raw_ch = 0, raw_w0 = 0, raw_pitch = 0;
-    DeviceArray<uint16_t> d_depth16_raw;
-    size_t depth16_raw_pitch = 0;
-    const uint16_t* depth_src = nullptr;
+    DeviceArray<LinCoef> d_resize_coefs;      // the input resize's cv::resize tables of the two axes (x: W entries, then y: H entries)
+    // The raw planes of uploads and PNG decodes (LoadedInput): max_batch input-size images or depth images, allocated by the first upload
+    // that needs them and reallocated when a later one needs more.  No chain graph references them, so they need no scratch_generation bump.
+    DeviceArray<uint8_t> d_raw_img; DeviceArray<uint16_t> d_depth16_raw;
+    LoadedInput loaded;
     DeviceArray<int> d_n_pts;
     DeviceArray<uint32_t> d_idx_map;
     DeviceArray<float> d_raw, d_processed, d_depth, d_uright;
@@ -239,10 +236,9 @@ struct Ctx {
     // rgbl_track_sequence_rgbd, rgbl_resident_stage_stereo / rgbl_track_sequence_stereo): level-0 planes + clouds (RGB-L), uint16 depth
     // planes (RGB-D) or the left then the right level-0 planes (stereo: n_frames pairs, 2 n_frames planes) of whole batches
     static constexpr int kMaxStageSlots = 8;
-    // (in_w x in_h, ch: the input size and channel count the slot was staged with)
     struct StageSlot {
         DeviceArray<uint8_t> img; DeviceArray<float> pts; DeviceArray<int> n_pts; DeviceArray<uint16_t> depth;
-        int n_frames = 0, max_pts = 0, in_w = 0, in_h = 0, ch = 1; InputKind kind = InputKind::rgbl;
+        int n_frames = 0, max_pts = 0; InputKind kind = InputKind::rgbl; InputSetting input;   // input: the setting it was staged with
     };
     StageSlot stage[kMaxStageSlots];
 
