@@ -25,6 +25,7 @@ extern "C" {
 
 #define RGBL_MAX_LEVELS 16
 #define RGBL_DESC_BYTES 32
+#define RGBL_MAX_SEQUENCES 16    /* sequence lanes of one context (rgbl_set_sequences) */
 
 typedef enum {
     RGBL_OK = 0,
@@ -354,6 +355,23 @@ int rgbl_resident_track_begin2(rgbl_ctx* ctx, const rgbl_chain_params* prm);
  * n_inliers = inliers of the frame's last PoseOptimization.  Fails with RGBL_E_CAPACITY when the frame construction of the tracked
  * batch overflowed a capacity (the keypoint sets were truncated) or a matcher candidate list overflowed.                        */
 int rgbl_resident_track_end2(rgbl_ctx* ctx, float* poses_out, int* n_matches, int* n_inliers, int* n_local_matches, int* n_inliers_first);
+
+/* Sequence lanes: the frames of every batch hold n_sequences independent sequences of m = n / n_sequences consecutive frames each
+ * (lane s = frames [s*m, (s+1)*m) of the batch; stereo: the left frames, pairs laid out the same way).  The tracking chain
+ * (rgbl_resident_track_begin2 / _end2) and the three sequence runners track every lane as its own sequence in lockstep: lane s
+ * continues from lane s's last frame, pose, velocity and local-map ring, and never reads another lane's state.  Every launch of the
+ * chain serves all lanes, so S lanes cost about one chain's launches per frame step instead of S chains'.
+ * pose0 (nullable): n_sequences x 7, the start pose of each lane for a chain with continue_sequence == 0 (NULL: every lane starts at
+ * rgbl_chain_params.pose0).  n_sequences 1 (the default) is today's behaviour; at most RGBL_MAX_SEQUENCES.
+ * Outputs stay in batch order: _end2's per-frame arrays hold lane s at [s*m, (s+1)*m) (frame 0 of every lane of a chain that starts
+ * a sequence = (pose0[s], 0 matches, 0 inliers)); the runners' io arrays hold batch b, lane s, frame k at b*frames_per_batch + s*m + k.
+ * RGBL_E_INVALID: n_sequences out of range, a non-finite pose0 value, a chain in flight (the previous setting stays); later, a batch or
+ * frames_per_batch that is not a multiple of n_sequences, or continue_sequence after a chain with another lane count.  A matcher list
+ * overflow names its lane in the error text.  Uploads and staged slots are unaffected: a batch is still just frames.               */
+int rgbl_set_sequences(rgbl_ctx* ctx, int n_sequences, const float* pose0);
+/* Sequence lanes whose pose optimisation (one 16-CTA cluster per lane) the device runs at once (cudaOccupancyMaxActiveClusters); lanes
+ * beyond it run in waves, which is correct and only slower.                                                                          */
+int rgbl_sequence_lanes_resident(rgbl_ctx* ctx, int* n_lanes);
 
 /* ---- Sequence runner: the loop of Examples/RGB-L/rgbl_kitti.cc:84-133 (load frame -> SLAM.TrackRGBL -> pose) for many frames per
  * call, entirely native.  Per batch of frames_per_batch consecutive frames: inputs -> frame construction -> tracking chain

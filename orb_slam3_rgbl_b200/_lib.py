@@ -120,6 +120,8 @@ SYMBOLS = {
     "rgbl_set_stereo_rectification": (_i, [_vp, _vp, _vp, _vp, _vp, _i]),
     "rgbl_set_input_resize": (_i, [_vp, _i, _i]),
     "rgbl_set_input_channels": (_i, [_vp, _i, _i]),
+    "rgbl_set_sequences": (_i, [_vp, _i, _vp]),
+    "rgbl_sequence_lanes_resident": (_i, [_vp, _ip]),
     "rgbl_resident_track_end2": (_i, [_vp, _vp, _vp, _vp, _vp, _vp]),
     "rgbl_set_camera_distortion": (_i, [_vp, _f, _f, _f, _f, _vp, _i, _vp]),
     "rgbl_resident_download_keys_un": (_i, [_vp, _vp, _i, _vp]),

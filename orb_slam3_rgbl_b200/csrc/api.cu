@@ -254,7 +254,7 @@ static int run_extract(Ctx* c, int n_frames, const std::function<void()>& aux_wo
         // Fully on-device keypoint distribution: no host round trip between FAST and describe.
         stage_begin(c, ST_QUADTREE, c->st);
         if (launch_quadtree(c->st, c->d_dense, c->d_level_cnt, c->d_frame_total, c->d_levels, nl, c->qt_scr, c->d_sel_lvl, c->d_n_sel_lvl,
-                            c->d_lvl_region, c->cap_kp, c->d_overflow + 1, c->d_sel, c->d_n_sel, n_frames, c->qt_max_nodes) != 0) {
+                            c->d_lvl_region, c->cap_kp, c->d_overflow + 1, c->d_sel, c->d_n_sel, n_frames, c->qt_max_nodes, c->dense_cap) != 0) {
             c->err = "quad-tree kernel needs more shared memory than this device allows"; return RGBL_E_CUDA;
         }
         stage_end(c, ST_QUADTREE, c->st, 2);
@@ -1306,6 +1306,7 @@ static int check_sequence_io(Ctx* c, const rgbl_chain_params* chain, const rgbl_
     const int T = io->frames_per_batch, nb = io->n_batches;
     if (T < 1 || T > c->cfg.max_batch || nb < 1) { c->err = "bad batch geometry"; return RGBL_E_INVALID; }
     if (const int rc = require_idle(c)) return rc;
+    if (T % c->lanes) { c->err = "frames_per_batch is not a multiple of the sequence count (rgbl_set_sequences)"; return RGBL_E_INVALID; }
     if (io->gray) {
         int rc = check_images(c, c->input, T, io->width, io->height, io->stride); if (rc) return rc;
     } else if (io->n_slots < 1 || io->n_slots > Ctx::kMaxStageSlots) { c->err = "resident mode needs 1..8 staged slots"; return RGBL_E_INVALID; }

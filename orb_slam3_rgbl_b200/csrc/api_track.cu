@@ -179,7 +179,7 @@ int rgbl_search_by_projection_last(rgbl_ctx* ctx, const rgbl_frame_view* cur, co
     }
     LastFrameDev lf{n_last, t.q_u8a, t.q_f3a, t.q_desc, t.q_i, t.q_f[0], t.q_u8b};
     if (n_last == 0) CU(clear_search_outputs(c, cur->n));
-    launch_search_last(c->st, f, t.cell_start, t.csr_idx, lf, prm, scratch(c), t.state, t.match, t.scalars + kDevMatches);
+    launch_search_last(c->st, f, t.cell_start.get(), t.csr_idx.get(), lf, prm, scratch(c), t.state.get(), t.match.get(), t.scalars + kDevMatches);
     return finish_search(c, cur->n, match, n_matches);
 }
 
@@ -247,7 +247,7 @@ int rgbl_search_by_projection_local(rgbl_ctx* ctx, const rgbl_frame_view* cur, i
     prm.keep_max = keep_max(100.f, nn_ratio);                                     // TH_HIGH
     LocalPointsDev lp{n, nullptr, t.q_u8a, t.q_f[0], t.q_f[1], t.q_f[2], t.q_f[3], t.q_i, t.q_f[4], t.q_desc, t.q_u8b};
     if (n == 0) CU(clear_search_outputs(c, cur->n));
-    launch_search_local(c->st, f, t.cell_start, t.csr_idx, lp, prm, scratch(c), t.state, t.match, t.scalars + kDevMatches);
+    launch_search_local(c->st, f, t.cell_start.get(), t.csr_idx.get(), lp, prm, scratch(c), t.state.get(), t.match.get(), t.scalars + kDevMatches);
     return finish_search(c, cur->n, match, n_matches);
 }
 
@@ -272,7 +272,7 @@ int rgbl_pose_optimize(rgbl_ctx* ctx, const float pose_in[7], int n, const float
     p.fx = fx; p.fy = fy; p.cx = cx; p.cy = cy; p.bf = bf; p.n_dev = nullptr; p.pose_in_dev = nullptr;
     std::memcpy(p.pose_in, pose_in, 7 * sizeof(float));
     stage_begin(c, ST_POSE, c->st);
-    launch_pose_optimize(c->st, p, t.pose_work, t.q_u8b, t.resolved, t.q_f[1], t.scalars + kDevPoseInliers);
+    launch_pose_optimize(c->st, p, t.pose_work.get(), t.q_u8b.get(), t.resolved.get(), t.q_f[1].get(), t.scalars + kDevPoseInliers);
     stage_end(c, ST_POSE, c->st, 1);
     CU(cudaGetLastError());
     CU(d2h(c, pose_out, t.q_f[1], 7));
@@ -462,7 +462,11 @@ static int check_chain(Ctx* c, const rgbl_chain_params& P, ChainPlan& p) {
     const bool cont = P.continue_sequence != 0;
     if (cont && !c->chain_has_carry) { c->err = "continue_sequence without a previous chain on this context"; return RGBL_E_INVALID; }
     if (cont && (c->carry_K != K || c->carry_cap != cap)) { c->err = "continue_sequence: local_map_frames / keypoint capacity differ from the previous chain"; return RGBL_E_INVALID; }
+    const int S = c->lanes;
+    if (nF % S) { c->err = "the batch's frame count is not a multiple of the sequence count (rgbl_set_sequences)"; return RGBL_E_INVALID; }
+    if (cont && c->carry_lanes != S) { c->err = "continue_sequence: the sequence count differs from the previous chain's (rgbl_set_sequences)"; return RGBL_E_INVALID; }
     p.nF = nF; p.cap = cap; p.mono = P.mono; p.cont = cont ? 1 : 0; p.K = K; p.prev_valid = (cont && c->carry_prev_valid) ? 1 : 0;
+    p.lanes = S; p.m = nF / S;
     p.th = P.th_last; p.th_local = P.th_local; p.nn_local = P.nn_ratio_local;
     p.fx = P.fx; p.fy = P.fy; p.cx = P.cx; p.cy = P.cy; p.bf = P.bf;
     std::memcpy(p.bounds, c->frame_bounds, sizeof(p.bounds));      // ComputeImageBounds of the frames' camera
@@ -488,32 +492,39 @@ static int ensure_chain_resources(Ctx* c, const ChainPlan& p) {
     if (c->chain_timing_on) for (Event& e : c->chain_tev) CU(have(e, 0));
     if (c->h_chain_cap < (size_t)nF) {
         if (c->chain_pending) { c->err = "batch size grew while a chain is in flight"; return RGBL_E_INVALID; }
-        const size_t capF = slot_frames(c), nf = 2 * chain_pose_floats(capF), ni = 2 * chain_count_ints(capF);
+        const size_t capF = slot_frames(c), nf = 2 * chain_pose_floats(capF), ni = 2 * chain_count_ints(capF, kMaxLanes);
         c->h_chain_cap = 0;
         if (!c->h_chain_f.grow(nf, c->scratch_generation, nf) || !c->h_chain_i.grow(ni, c->scratch_generation, ni)) {
             c->err = "pinned allocation failed (chain result staging)"; return RGBL_E_CUDA;
         }
         c->h_chain_cap = capF;
     }
-    int rc = ensure_frame(c, cap); if (rc) return rc;
-    rc = ensure_queries(c, std::max(cap, n_lq)); if (rc) return rc;
+    // every lane buffer: lanes x its lane stride (ChainLaneStrides)
+    const size_t S = (size_t)p.lanes;
+    const ChainLaneStrides ls = chain_lane_strides(p);
     TrackBufs& t = c->trk;
-    GROW(t.pose_work, (size_t)cap * 3);
-    GROW(t.ch_poses, (size_t)nF * 7 + 14); GROW(t.ch_counts, chain_count_ints(nF));      // poses | pose after TrackWithMotionModel | predicted pose
-    GROW(t.e_xw, (size_t)cap * 3); GROW(t.e_obs, (size_t)cap * 3); GROW(t.e_info, cap);
-    GROW(t.e_st, cap); GROW(t.e_lvl, cap); GROW(t.e_out, cap); GROW(t.e_idx, cap);
-    // carried last frame of the sequence + the local map ring (persist across chains of this context)
-    GROW(t.c_kps, cap); GROW(t.c_desc, (size_t)cap * 32); GROW(t.c_depth, cap);
-    GROW(t.carry, 1);
+    GROW(t.state, S * ls.kp); GROW(t.match, S * ls.kp); GROW(t.minq, S * ls.kp); GROW(t.scalars, S * ls.scalars);
+    if (S * ls.inv > t.inv_cnt.size()) {                  // per-feature entry counters + entry total of each lane: zero between launches
+        GROW(t.inv_cnt, S * ls.inv);
+        CU(cudaMemsetAsync(t.inv_cnt, 0, t.inv_cnt.size() * sizeof(int), c->st));
+    }
+    int rc = ensure_queries(c, (int)(S * ls.q)); if (rc) return rc;
+    GROW(t.pose_work, S * ls.kp * 3);
+    GROW(t.ch_poses, (size_t)nF * 7 + S * ls.pose_tmp); GROW(t.ch_counts, chain_count_ints(nF, S));      // poses | per lane: pose after TrackWithMotionModel, predicted pose
+    GROW(t.e_xw, S * ls.kp * 3); GROW(t.e_obs, S * ls.kp * 3); GROW(t.e_info, S * ls.kp);
+    GROW(t.e_st, S * ls.kp); GROW(t.e_lvl, S * ls.kp); GROW(t.e_out, S * ls.kp); GROW(t.e_idx, S * ls.kp);
+    // carried last frame of each lane's sequence + the local map rings (persist across chains of this context)
+    GROW(t.c_kps, S * ls.kp); GROW(t.c_desc, S * ls.kp * 32); GROW(t.c_depth, S * ls.kp);
+    GROW(t.carry, S);
     if (K > 0) {
-        const size_t nr = (size_t)K * cap;
+        const size_t nr = S * ls.ring;
         if (p.cont && t.r_valid.size() < nr) { c->err = "local map ring missing"; return RGBL_E_INVALID; }
         GROW(t.r_valid, nr); GROW(t.r_xw, nr * 3); GROW(t.r_normal, nr * 3);
         GROW(t.r_min, nr); GROW(t.r_max, nr); GROW(t.r_desc, nr * 32);
-        GROW(t.lq_u8, kLqU8Planes * (size_t)n_lq); GROW(t.lq_f, kLqFPlanes * (size_t)n_lq); GROW(t.lq_i, kLqIPlanes * (size_t)n_lq);
-        GROW(t.lq_desc, (size_t)n_lq * 32); GROW(t.match_local, cap);
-        if (!t.lookback) {
-            GROW(t.lookback, tlm_lookback_ints());
+        GROW(t.lq_u8, S * kLqU8Planes * ls.lq); GROW(t.lq_f, S * kLqFPlanes * ls.lq); GROW(t.lq_i, S * kLqIPlanes * ls.lq);
+        GROW(t.lq_desc, S * ls.lq * 32); GROW(t.match_local, S * ls.kp);
+        if (t.lookback.size() < S * ls.lookback) {
+            GROW(t.lookback, S * ls.lookback);
             CU(cudaMemsetAsync(t.lookback, 0, t.lookback.size() * sizeof(int), c->st));     // ordered before the chain by ev_snap (snapshot_batch)
         }
         if ((n_lq + 255) / 256 + 1 > 1024) { c->err = "local map too large for the compaction slots (local_map_frames x keypoint capacity > 261 k)"; return RGBL_E_UNSUPPORTED; }
@@ -546,12 +557,54 @@ static int snapshot_batch(Ctx* c, const ChainPlan& p, int slot, const ChainSlot&
     return RGBL_OK;
 }
 
+// Lane s's view of the chain's buffers: the single-sequence chain's buffers, each offset by s times its ChainLaneStrides stride.
+struct ChainLane {
+    uint8_t *q_u8a, *q_u8b, *state, *e_st, *e_lvl, *e_out, *c_desc;
+    float *q_f3a, *q_f0, *e_xw, *e_obs, *e_info, *c_depth, *pose_tmp, *pose_pred;
+    int *q_i, *match, *match_local, *e_idx, *scalars, *lookback;
+    double* pose_work; rgbl_keypoint* c_kps; ChainCarry* carry;
+    MatchScratch ms; ChainCounts cnt; LocalRingDev ring; LocalQueriesDev lq;
+    size_t f0;                        // the lane's first frame in the batch (s * m)
+};
+static ChainLane chain_lane(Ctx* c, const ChainPlan& p, int s) {
+    TrackBufs& t = c->trk;
+    const ChainLaneStrides st = chain_lane_strides(p);
+    const size_t kp = s * st.kp, q = s * st.q, ring = s * st.ring, lq = s * st.lq;
+    ChainLane L;
+    L.q_u8a = t.q_u8a + q; L.q_u8b = t.q_u8b + q; L.q_f3a = t.q_f3a + 3 * q; L.q_f0 = t.q_f[0] + q; L.q_i = t.q_i + q;
+    L.state = t.state + kp; L.match = t.match + kp; L.match_local = p.K > 0 ? t.match_local + kp : nullptr;
+    L.e_xw = t.e_xw + 3 * kp; L.e_obs = t.e_obs + 3 * kp; L.e_info = t.e_info + kp; L.e_st = t.e_st + kp; L.e_lvl = t.e_lvl + kp;
+    L.e_out = t.e_out + kp; L.e_idx = t.e_idx + kp; L.pose_work = t.pose_work + 3 * kp;
+    L.c_kps = t.c_kps + kp; L.c_desc = t.c_desc + 32 * kp; L.c_depth = t.c_depth + kp; L.carry = t.carry + s;
+    L.scalars = t.scalars + s * st.scalars;
+    L.pose_tmp = t.ch_poses + 7 * (size_t)p.nF + s * st.pose_tmp; L.pose_pred = L.pose_tmp + 7;
+    L.cnt = chain_counts(t.ch_counts, p.nF, p.m, s);
+    L.f0 = (size_t)s * p.m;
+    MatchScratch& m = L.ms;
+    m.lists = t.lists + q * kMatchListCap; m.slots = t.list_slots + q * kMatchListCap; m.list_cap = kMatchListCap; m.list_n = t.list_n + q;
+    m.dense = t.dense + q * kMatchListCap; m.dense_slot = t.dense_slot + q * kMatchListCap; m.dense_q = t.dense_q + q * kMatchListCap; m.base = t.list_base + q;
+    m.inv_cnt = t.inv_cnt + s * st.inv; m.total = m.inv_cnt + p.cap;
+    m.minq = t.minq + kp; m.choice = t.choice + q; m.resolved = t.resolved + q; m.overflow = L.cnt.overflow; m.rounds = L.scalars + kDevRounds;
+    if (p.K > 0) {
+        L.ring = LocalRingDev{p.K, p.cap, t.r_valid + ring, t.r_xw + 3 * ring, t.r_normal + 3 * ring, t.r_min + ring, t.r_max + ring, t.r_desc + 32 * ring,
+                              &L.carry->ring_count};
+        L.lq = local_queries(t.lq_u8 + kLqU8Planes * lq, t.lq_f + kLqFPlanes * lq, t.lq_i + kLqIPlanes * lq, t.lq_desc + 32 * lq, (int)st.lq, L.cnt.n_queries);
+        L.lookback = t.lookback + s * st.lookback;
+    } else {
+        L.ring = LocalRingDev{p.K, p.cap, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, &L.carry->ring_count};
+        L.lq = LocalQueriesDev{}; L.lookback = nullptr;
+    }
+    return L;
+}
+
 // Everything the chain does on the tracking stream.  It is captured ONCE per slot into a CUDA graph and
 // replayed: the launch commands then live in device memory, so the dependent-kernel sequence no longer fetches a command
 // packet from the host over PCIe per launch (which the concurrent H2D uploads of the next batch were slowing down) and
 // _begin costs one graph launch instead of hundreds of kernel launches on the host.
 // It reads the plan, the slot's buffers and the context (its scratch, whose addresses scratch_generation stands for, and settings fixed
 // at rgbl_create) and nothing else: the graph's key is the plan and that generation.
+// Sequence lanes: step k of the loop tracks frame k of every lane (batch frame s * m + k), each launch serving all lanes (Laned arguments
+// built from chain_lane(s)), so the launch count per step does not depend on the lane count.
 static int enqueue_chain(Ctx* c, const ChainPlan& p, const ChainSlot& s, int& n_launches) {
     struct PdlScope {      // programmatic dependent launches between the chain's kernels (rgbl_device.cuh: pdl_wait)
         explicit PdlScope(bool on) { chain_launch_pdl() = on; }
@@ -559,107 +612,151 @@ static int enqueue_chain(Ctx* c, const ChainPlan& p, const ChainSlot& s, int& n_
     } pdl(c->chain_pdl_on);
     TrackBufs& t = c->trk;
     const cudaStream_t cs = c->st_trk;
-    const int nF = p.nF, cap = p.cap, K = p.K, n_lq = local_query_cap(p);
+    const int nF = p.nF, cap = p.cap, K = p.K, S = p.lanes, m = p.m, n_lq = local_query_cap(p);
     const bool cont = p.cont != 0, chain_timing = c->chain_timing_on;
     const Event* tev = c->chain_tev;
-    ChainCarry* carry = t.carry;
     n_launches = 0;
-    float* poses = t.ch_poses;                 // frame k -> poses + 7 k
-    float* pose_tmp = t.ch_poses + 7 * (size_t)nF;      // pose after TrackWithMotionModel (input of the second PoseOptimization)
-    float* pose_pred = pose_tmp + 7;                    // the motion model's pose of the frame being tracked (written when the previous frame's pose is final)
-    const ChainCounts cnt = chain_counts(t.ch_counts, nF);
-    CU(cudaMemsetAsync(t.ch_counts, 0, chain_count_ints(nF) * sizeof(int), cs));
+    std::vector<ChainLane> lanes;
+    for (int l = 0; l < S; ++l) lanes.push_back(chain_lane(c, p, l));
+    const ChainLane& L0 = lanes[0];
+    float* poses = t.ch_poses;                 // batch frame j -> poses + 7 j
+    auto pose_of = [&](int l, int k) { return poses + 7 * (lanes[l].f0 + (size_t)k); };
+    auto laned = [&](auto make) { return laned_of(S, make); };
+    CU(cudaMemsetAsync(t.ch_counts, 0, chain_count_ints(nF, S) * sizeof(int), cs));
     if (!cont) {
-        CU(cudaMemcpyAsync(poses, s.h_f, 7 * sizeof(float), cudaMemcpyHostToDevice, cs));
-        if (K > 0) { CU(cudaMemsetAsync(t.r_valid, 0, (size_t)K * cap, cs)); CU(cudaMemsetAsync(&carry->ring_count, 0, sizeof(int), cs)); }
+        // frame 0 of every lane: its start pose (the slot's pose0 block, one 7-float record per lane)
+        CU(cudaMemcpy2DAsync(poses, 7 * sizeof(float) * m, s.h_f, 7 * sizeof(float), 7 * sizeof(float), S, cudaMemcpyHostToDevice, cs));
+        if (K > 0) {
+            CU(cudaMemsetAsync(t.r_valid, 0, (size_t)S * K * cap, cs));
+            for (const ChainLane& L : lanes) CU(cudaMemsetAsync(&L.carry->ring_count, 0, sizeof(int), cs));
+        }
     }
-    FrameDev f{};
-    set_camera(f, p.bounds, p.fx, p.fy, p.cx, p.cy, p.bf);
-    f.n_levels = c->tab.nlevels;
-    for (int l = 0; l < f.n_levels; ++l) f.scale[l] = c->tab.scale[l];
-    f.log_scale_factor = std::log(c->cfg.orb.scale_factor);
-    MatchScratch ms = scratch(c);
-    ms.overflow = cnt.overflow;
-    // the 64x48 grids do not depend on the poses: all frames in one launch (one CTA per frame)
-    f.n = s.s_nsel; f.keys = s.s_kps;
-    launch_grid_build_batch(cs, f, nF, cap, s.b_cell_start, s.b_csr_idx, s.b_kp_cell); ++n_launches;
-    // unprojection of frame j's keypoints (map points of the search in frame j + 1); j == -1: the carried frame
-    auto prep_of = [&](int j) {
+    FrameDev f0{};
+    set_camera(f0, p.bounds, p.fx, p.fy, p.cx, p.cy, p.bf);
+    f0.n_levels = c->tab.nlevels;
+    for (int l = 0; l < f0.n_levels; ++l) f0.scale[l] = c->tab.scale[l];
+    f0.log_scale_factor = std::log(c->cfg.orb.scale_factor);
+    // the 64x48 grids do not depend on the poses: all frames of all lanes in one launch (one CTA per frame)
+    {
+        FrameDev f = f0;
+        f.n = s.s_nsel; f.keys = s.s_kps;
+        launch_grid_build_batch(cs, f, nF, cap, s.b_cell_start, s.b_csr_idx, s.b_kp_cell); ++n_launches;
+    }
+    // unprojection of lane l's frame j (map points of the search in frame j + 1); j == -1: the lane's carried frame
+    auto prep_of = [&](int l, int j) {
+        const ChainLane& L = lanes[l];
         ChainPrepDev cp{};
-        if (j < 0) { cp.kps = t.c_kps; cp.depth = t.c_depth; cp.n_ptr = &carry->n_sel; }
-        else { cp.kps = s.s_kps + (size_t)j * cap; cp.depth = s.s_depth + (size_t)j * cap; cp.n_ptr = s.s_nsel + j; }
-        cp.fx = f.fx; cp.fy = f.fy; cp.cx = f.cx; cp.cy = f.cy; cp.mb = f.mb; cp.mono = p.mono; cp.cap = cap;
-        cp.valid = t.q_u8a; cp.xw = t.q_f3a; cp.octave = t.q_i; cp.angle = t.q_f[0]; cp.obs_pos = t.q_u8b; cp.flags = cnt.flags; cp.state_clear = t.state;
+        if (j < 0) { cp.kps = L.c_kps; cp.depth = L.c_depth; cp.n_ptr = &L.carry->n_sel; }
+        else { cp.kps = s.s_kps + (L.f0 + j) * cap; cp.depth = s.s_depth + (L.f0 + j) * cap; cp.n_ptr = s.s_nsel + L.f0 + j; }
+        cp.fx = f0.fx; cp.fy = f0.fy; cp.cx = f0.cx; cp.cy = f0.cy; cp.mb = f0.mb; cp.mono = p.mono; cp.cap = cap;
+        cp.valid = L.q_u8a; cp.xw = L.q_f3a; cp.octave = L.q_i; cp.angle = L.q_f0; cp.obs_pos = L.q_u8b; cp.flags = L.cnt.flags; cp.state_clear = L.state;
         // constant-velocity motion model: the pose of the frame before frame j (nullptr at the start of a sequence)
-        if (j >= 1) cp.prev_pose = poses + 7 * (size_t)(j - 1);
-        else if (j == 0) cp.prev_pose = cont ? carry->pose : nullptr;
-        else cp.prev_pose = p.prev_valid ? carry->prev_pose : nullptr;      // the pose of the frame before the carried one
-        cp.pred_pose = pose_pred;
+        if (j >= 1) cp.prev_pose = pose_of(l, j - 1);
+        else if (j == 0) cp.prev_pose = cont ? L.carry->pose : nullptr;
+        else cp.prev_pose = p.prev_valid ? L.carry->prev_pose : nullptr;      // the pose of the frame before the carried one
+        cp.pred_pose = L.pose_pred;
         return cp;
     };
-    LocalRingDev ring{K, cap, t.r_valid, t.r_xw, t.r_normal, t.r_min, t.r_max, t.r_desc, &carry->ring_count};
-    const LocalQueriesDev lq = K > 0 ? local_queries(t, n_lq, cnt.n_queries) : LocalQueriesDev{};
     const int k0 = cont ? 0 : 1;
-    for (int k = k0; k < nF; ++k) {
-        const bool tm = chain_timing && k == std::max(1, nF / 2);
-        const size_t cu = (size_t)k * cap;
-        const float* last_pose = (k == 0) ? carry->pose : poses + 7 * (size_t)(k - 1);
-        const uint8_t* last_desc = (k == 0) ? t.c_desc.get() : s.s_desc + (size_t)(k - 1) * cap * 32;
+    for (int k = k0; k < m; ++k) {
+        const bool tm = chain_timing && k == std::max(1, m / 2);
+        const Laned<const float*> last_pose = laned([&](int l) -> const float* { return (k == 0) ? lanes[l].carry->pose : pose_of(l, k - 1); });
+        const Laned<const uint8_t*> last_desc = laned([&](int l) -> const uint8_t* {
+            return (k == 0) ? lanes[l].c_desc : s.s_desc + (lanes[l].f0 + k - 1) * cap * 32;
+        });
         if (tm) cudaEventRecord(tev[0], cs);
-        if (k == k0) { launch_chain_prep(cs, prep_of(k - 1), last_pose); ++n_launches; }   // later frames: prepared by the previous pose kernel
-        f.n = s.s_nsel + k; f.keys = s.s_kps + cu; f.uright = s.s_uright + cu; f.desc = s.s_desc + cu * 32;
-        const int* cell_start = s.b_cell_start + (size_t)k * (kGridCols * kGridRows + 1);
-        const int* csr_idx = s.b_csr_idx + cu;
+        if (k == k0) { launch_chain_prep(cs, laned([&](int l) { return prep_of(l, k - 1); }), last_pose, S); ++n_launches; }   // later frames: prepared by the previous pose kernel
+        const Laned<FrameDev> f = laned([&](int l) {
+            const size_t cu = (lanes[l].f0 + k) * cap;
+            FrameDev fl = f0;
+            fl.n = s.s_nsel + lanes[l].f0 + k; fl.keys = s.s_kps + cu; fl.uright = s.s_uright + cu; fl.desc = s.s_desc + cu * 32;
+            return fl;
+        });
+        const Laned<const int*> cell_start = laned([&](int l) -> const int* { return s.b_cell_start + (lanes[l].f0 + k) * (kGridCols * kGridRows + 1); });
+        const Laned<const int*> csr_idx = laned([&](int l) -> const int* { return s.b_csr_idx + (lanes[l].f0 + k) * cap; });
+        const Laned<MatchScratch> ms = laned([&](int l) { return lanes[l].ms; });
+        const Laned<uint8_t*> state = laned([&](int l) { return lanes[l].state; });
         if (tm) cudaEventRecord(tev[1], cs);
-        SearchLastParams prm{};
-        prm.th = p.th; prm.check_orientation = 1; prm.cur_pose_dev = pose_pred; prm.flags_dev = cnt.flags;      // projected with the motion model's pose (src/Tracking.cc:2904)
-        LastFrameDev lf{cap, t.q_u8a, t.q_f3a, last_desc, t.q_i, t.q_f[0], t.q_u8b};
-        const ChainEdgesOut eo{t.e_xw, t.e_obs, t.e_info, t.e_st, t.e_idx, cnt.n_edges};
-        launch_search_last(cs, f, cell_start, csr_idx, lf, prm, ms, t.state, t.match, cnt.n_matches + k, &eo); n_launches += 2;   // + edges of the matches
+        const Laned<SearchLastParams> prm = laned([&](int l) {
+            SearchLastParams pr{};
+            pr.th = p.th; pr.check_orientation = 1; pr.cur_pose_dev = lanes[l].pose_pred; pr.flags_dev = lanes[l].cnt.flags;      // projected with the motion model's pose (src/Tracking.cc:2904)
+            return pr;
+        });
+        const Laned<LastFrameDev> lf = laned([&](int l) {
+            const ChainLane& L = lanes[l];
+            return LastFrameDev{cap, L.q_u8a, L.q_f3a, lane_value(last_desc, l), L.q_i, L.q_f0, L.q_u8b};
+        });
+        const Laned<ChainEdgesOut> eo = laned([&](int l) {
+            const ChainLane& L = lanes[l];
+            return ChainEdgesOut{L.e_xw, L.e_obs, L.e_info, L.e_st, L.e_idx, L.cnt.n_edges};
+        });
+        launch_search_last(cs, f, cell_start, csr_idx, lf, prm, ms, state, laned([&](int l) { return lanes[l].match; }),
+                           laned([&](int l) { return lanes[l].cnt.n_matches + k; }), &eo, S); n_launches += 2;   // + edges of the matches
         if (tm) cudaEventRecord(tev[2], cs);
-        PoseProblemDev pp{};
-        pp.n = 0; pp.n_dev = cnt.n_edges; pp.pose_in_dev = pose_pred;
-        pp.xw = t.e_xw; pp.obs = t.e_obs; pp.inv_sigma2 = t.e_info; pp.stereo = t.e_st;
-        pp.fx = p.fx; pp.fy = p.fy; pp.cx = p.cx; pp.cy = p.cy; pp.bf = p.bf;
-        const ChainPrepDev nxt = prep_of(k);
+        auto pose_problem = [&](int l, bool second) {
+            const ChainLane& L = lanes[l];
+            PoseProblemDev pp{};
+            pp.n = 0; pp.n_dev = second ? L.cnt.n_edges2 : L.cnt.n_edges; pp.pose_in_dev = second ? L.pose_tmp : L.pose_pred;
+            pp.xw = L.e_xw; pp.obs = L.e_obs; pp.inv_sigma2 = L.e_info; pp.stereo = L.e_st;
+            pp.fx = p.fx; pp.fy = p.fy; pp.cx = p.cx; pp.cy = p.cy; pp.bf = p.bf;
+            return pp;
+        };
+        const Laned<ChainPrepDev> nxt = laned([&](int l) { return prep_of(l, k); });
+        const Laned<double*> work = laned([&](int l) { return lanes[l].pose_work; });
+        const Laned<uint8_t*> e_lvl = laned([&](int l) { return lanes[l].e_lvl; });
+        const Laned<uint8_t*> e_out = laned([&](int l) { return lanes[l].e_out; });
+        const Laned<float*> pose_final = laned([&](int l) { return pose_of(l, k); });
+        const Laned<int*> n_inliers = laned([&](int l) { return lanes[l].cnt.n_inliers + k; });
         if (K == 0) {
-            launch_pose_optimize(cs, pp, t.pose_work, t.e_lvl, t.e_out, poses + 7 * (size_t)k, cnt.n_inliers + k, (k + 1 < nF) ? &nxt : nullptr); ++n_launches;
+            launch_pose_optimize(cs, laned([&](int l) { return pose_problem(l, false); }), work, e_lvl, e_out, pose_final, n_inliers, (k + 1 < m) ? &nxt : nullptr, S); ++n_launches;
             if (tm) { cudaEventRecord(tev[3], cs); cudaEventRecord(tev[4], cs); cudaEventRecord(tev[5], cs); cudaEventRecord(tev[6], cs); }
         } else {
-            launch_pose_optimize(cs, pp, t.pose_work, t.e_lvl, t.e_out, pose_tmp, cnt.n_inliers_first + k, nullptr); ++n_launches;
+            const Laned<float*> pose_tmp = laned([&](int l) { return lanes[l].pose_tmp; });
+            launch_pose_optimize(cs, laned([&](int l) { return pose_problem(l, false); }), work, e_lvl, e_out, pose_tmp,
+                                 laned([&](int l) { return lanes[l].cnt.n_inliers_first + k; }), nullptr, S); ++n_launches;
             if (tm) cudaEventRecord(tev[3], cs);
             // TrackLocalMap: outlier discard + isInFrustum + ordered compaction, local search, edges of all map points, second optimisation
-            launch_tlm_prepare(cs, f, pose_tmp, ring, 0.5f, cnt.n_edges, t.e_idx, t.e_out, t.state, t.match, lq, t.lookback, cnt.overflow); ++n_launches;
-            LocalPointsDev lp{n_lq, cnt.n_queries, lq.in_view, lq.proj_x, lq.proj_y, lq.proj_xr, lq.depth, lq.level, lq.view_cos, lq.desc, lq.obs_pos};
+            launch_tlm_prepare(cs, f, laned([&](int l) -> const float* { return lanes[l].pose_tmp; }), laned([&](int l) { return lanes[l].ring; }), 0.5f,
+                               laned([&](int l) -> const int* { return lanes[l].cnt.n_edges; }), laned([&](int l) -> const int* { return lanes[l].e_idx; }),
+                               laned([&](int l) -> const uint8_t* { return lanes[l].e_out; }), state, laned([&](int l) { return lanes[l].match; }),
+                               laned([&](int l) { return lanes[l].lq; }), L0.lookback, laned([&](int l) { return lanes[l].cnt.overflow; }), S); ++n_launches;
+            const Laned<LocalPointsDev> lp = laned([&](int l) {
+                const LocalQueriesDev& lq = lanes[l].lq;
+                return LocalPointsDev{n_lq, lanes[l].cnt.n_queries, lq.in_view, lq.proj_x, lq.proj_y, lq.proj_xr, lq.depth, lq.level, lq.view_cos, lq.desc, lq.obs_pos};
+            });
             SearchLocalParams sl{};
             sl.th = p.th_local; sl.nn_ratio = p.nn_local; sl.th_far = 0.f; sl.use_factor = (p.th_local != 1.0f) ? 1 : 0; sl.far_points = 0;
             sl.keep_max = keep_max(100.f, p.nn_local);                                    // TH_HIGH
             // the resolution kernel of the local search also writes the edge list of the second optimisation and hands the last frame's points to the ring
-            const ChainEdgesOut eo2{t.e_xw, t.e_obs, t.e_info, t.e_st, t.e_idx, cnt.n_edges2};
-            const ChainTlmTail tail{t.match, t.q_f3a, lq.xw, ring, eo2, cnt.n_local_matches + k, cap, t.q_u8a, t.q_i, last_desc, last_pose};
-            launch_search_local(cs, f, cell_start, csr_idx, lp, sl, ms, t.state, t.match_local, t.scalars + kDevMatches, &tail); n_launches += 2;
+            const Laned<ChainTlmTail> tail = laned([&](int l) {
+                const ChainLane& L = lanes[l];
+                const ChainEdgesOut eo2{L.e_xw, L.e_obs, L.e_info, L.e_st, L.e_idx, L.cnt.n_edges2};
+                return ChainTlmTail{L.match, L.q_f3a, L.lq.xw, L.ring, eo2, L.cnt.n_local_matches + k, cap, L.q_u8a, L.q_i, lane_value(last_desc, l),
+                                    lane_value(last_pose, l)};
+            });
+            launch_search_local(cs, f, cell_start, csr_idx, lp, sl, ms, state, laned([&](int l) { return lanes[l].match_local; }),
+                                laned([&](int l) { return lanes[l].scalars + kDevMatches; }), &tail, S); n_launches += 2;
             if (tm) cudaEventRecord(tev[4], cs);
             if (tm) cudaEventRecord(tev[5], cs);
-            PoseProblemDev pp2 = pp;
-            pp2.n_dev = cnt.n_edges2; pp2.pose_in_dev = pose_tmp;
-            launch_pose_optimize(cs, pp2, t.pose_work, t.e_lvl, t.e_out, poses + 7 * (size_t)k, cnt.n_inliers + k, (k + 1 < nF) ? &nxt : nullptr); ++n_launches;
+            launch_pose_optimize(cs, laned([&](int l) { return pose_problem(l, true); }), work, e_lvl, e_out, pose_final, n_inliers, (k + 1 < m) ? &nxt : nullptr, S); ++n_launches;
             if (tm) cudaEventRecord(tev[6], cs);
         }
     }
-    // carry the last frame of this batch (keypoints, depths, descriptors, pose) for a continuing chain
-    const size_t lo = (size_t)(nF - 1) * cap;
-    CU(cudaMemcpyAsync(t.c_kps, s.s_kps + lo, (size_t)cap * sizeof(rgbl_keypoint), cudaMemcpyDeviceToDevice, cs));
-    CU(cudaMemcpyAsync(t.c_desc, s.s_desc + lo * 32, (size_t)cap * 32, cudaMemcpyDeviceToDevice, cs));
-    CU(cudaMemcpyAsync(t.c_depth, s.s_depth + lo, (size_t)cap * sizeof(float), cudaMemcpyDeviceToDevice, cs));
-    CU(cudaMemcpyAsync(&carry->n_sel, s.s_nsel + (nF - 1), sizeof(int), cudaMemcpyDeviceToDevice, cs));
-    // ... and the pose before it (motion model of the next chain's first frame): frame nF - 2, or the previously carried pose for a one-frame batch
-    if (nF >= 2) CU(cudaMemcpyAsync(carry->prev_pose, poses + 7 * (size_t)(nF - 2), 7 * sizeof(float), cudaMemcpyDeviceToDevice, cs));
-    else if (cont) CU(cudaMemcpyAsync(carry->prev_pose, carry->pose, 7 * sizeof(float), cudaMemcpyDeviceToDevice, cs));
-    CU(cudaMemcpyAsync(carry->pose, poses + 7 * (size_t)(nF - 1), 7 * sizeof(float), cudaMemcpyDeviceToDevice, cs));
+    // carry each lane's last frame (keypoints, depths, descriptors, pose) for a continuing chain: one strided copy per array over the lanes
+    const size_t lo = (size_t)(m - 1) * cap, kpb = (size_t)cap * sizeof(rgbl_keypoint), cb = sizeof(ChainCarry), pb = 7 * sizeof(float);
+    CU(cudaMemcpy2DAsync(t.c_kps, kpb, s.s_kps + lo, m * kpb, kpb, S, cudaMemcpyDeviceToDevice, cs));
+    CU(cudaMemcpy2DAsync(t.c_desc, (size_t)cap * 32, s.s_desc + lo * 32, (size_t)m * cap * 32, (size_t)cap * 32, S, cudaMemcpyDeviceToDevice, cs));
+    CU(cudaMemcpy2DAsync(t.c_depth, (size_t)cap * sizeof(float), s.s_depth + lo, (size_t)m * cap * sizeof(float), (size_t)cap * sizeof(float), S, cudaMemcpyDeviceToDevice, cs));
+    CU(cudaMemcpy2DAsync(&L0.carry->n_sel, cb, s.s_nsel + (m - 1), m * sizeof(int), sizeof(int), S, cudaMemcpyDeviceToDevice, cs));
+    // ... and the pose before it (motion model of the next chain's first frame): frame m - 2, or the previously carried pose for a one-frame lane
+    if (m >= 2) CU(cudaMemcpy2DAsync(L0.carry->prev_pose, cb, pose_of(0, m - 2), m * pb, pb, S, cudaMemcpyDeviceToDevice, cs));
+    else if (cont) CU(cudaMemcpy2DAsync(L0.carry->prev_pose, cb, L0.carry->pose, cb, pb, S, cudaMemcpyDeviceToDevice, cs));
+    CU(cudaMemcpy2DAsync(L0.carry->pose, cb, pose_of(0, m - 1), m * pb, pb, S, cudaMemcpyDeviceToDevice, cs));
     if (chain_timing) c->chain_timing_recorded = true;
+    if (lane_layout_broken()) { lane_layout_broken() = false; c->err = "internal error: a sequence lane's chain arguments are not equally spaced"; return RGBL_E_CUDA; }
     CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(s.h_f + 7, poses, (size_t)nF * 7 * sizeof(float), cudaMemcpyDeviceToHost, cs));
-    CU(cudaMemcpyAsync(s.h_i, t.ch_counts, chain_count_ints(nF) * sizeof(int), cudaMemcpyDeviceToHost, cs));
+    CU(cudaMemcpyAsync(s.h_f + kChainPose0Floats, poses, (size_t)nF * 7 * sizeof(float), cudaMemcpyDeviceToHost, cs));
+    CU(cudaMemcpyAsync(s.h_i, t.ch_counts, chain_count_ints(nF, S) * sizeof(int), cudaMemcpyDeviceToHost, cs));
     return RGBL_OK;
 }
 
@@ -701,7 +798,8 @@ static int chain_begin(Ctx* c, const rgbl_chain_params& P) {
     const int slot = (c->chain_head + c->chain_pending) & 1;
     const ChainSlot s = chain_slot(c, slot);
     rc = snapshot_batch(c, p, slot, s); if (rc) return rc;
-    for (int i = 0; i < 7; ++i) s.h_f[i] = P.pose0[i];
+    for (int l = 0; l < p.lanes; ++l)
+        for (int i = 0; i < 7; ++i) s.h_f[7 * l + i] = c->lane_pose0_set ? c->lane_pose0[l][i] : P.pose0[i];
     // stage timing events stay outside the graph (events recorded by graph nodes cannot be used for cudaEventElapsedTime)
     if (c->prof_on) CU(cudaEventRecord(c->ev_chain_b[slot], c->st_trk));
     int n_launches = 0;
@@ -709,11 +807,12 @@ static int chain_begin(Ctx* c, const rgbl_chain_params& P) {
     if (c->prof_on) CU(cudaEventRecord(c->ev_chain_e[slot], c->st_trk));
     CU(cudaEventRecord(c->ev_chain_done[slot], c->st_trk));
     c->chain_frames[slot] = p.nF;
+    c->chain_lanes[slot] = p.lanes;
     c->chain_first[slot] = p.cont ? 0 : 1;
     c->chain_launches[slot] = n_launches;
     c->chain_pending += 1;
-    c->chain_has_carry = true; c->carry_K = p.K; c->carry_cap = p.cap;
-    c->carry_prev_valid = (p.nF >= 2) || p.cont;
+    c->chain_has_carry = true; c->carry_K = p.K; c->carry_cap = p.cap; c->carry_lanes = p.lanes;
+    c->carry_prev_valid = (p.m >= 2) || p.cont;
     return RGBL_OK;
 }
 
@@ -747,22 +846,22 @@ int rgbl_resident_track_end2(rgbl_ctx* ctx, float* poses_out, int* n_matches, in
     c->chain_head ^= 1;
     c->chain_pending -= 1;
     CU(cudaEventSynchronize(c->ev_chain_done[slot]));            // the oldest chain only: a younger one may still be running
-    const int nF = c->chain_frames[slot];
+    const int nF = c->chain_frames[slot], S = c->chain_lanes[slot];
     const ChainSlot s = chain_slot(c, slot);
-    const ChainCounts cnt = chain_counts(s.h_i, nF);
+    const ChainCounts cnt = chain_counts(s.h_i, nF, nF / S, 0);
     if (c->chain_timing_recorded && c->chain_pending == 0) {
         const Event* e = c->chain_tev;
         const char* names[6] = {"chain_prep (first frame only)", "search_last (collect+resolve+edges)", "pose_optimize #1", "tlm_prepare + search_local (+edges, hand-over)", "-", "pose_optimize #2"};
         for (int i = 0; i < 6; ++i) { float ms = 0; if (cudaEventElapsedTime(&ms, e[i], e[i + 1]) == cudaSuccess) std::fprintf(stderr, "[chain timing] %-36s %8.2f us\n", names[i], ms * 1e3f); }
         cudaGetLastError();
     }
-    std::memcpy(poses_out, s.h_f + 7, (size_t)nF * 7 * sizeof(float));
+    std::memcpy(poses_out, s.h_f + kChainPose0Floats, (size_t)nF * 7 * sizeof(float));
     std::memcpy(n_matches, cnt.n_matches, (size_t)nF * sizeof(int));
     std::memcpy(n_inliers, cnt.n_inliers, (size_t)nF * sizeof(int));
     if (n_local_matches) std::memcpy(n_local_matches, cnt.n_local_matches, (size_t)nF * sizeof(int));
     if (n_inliers_first) std::memcpy(n_inliers_first, cnt.n_inliers_first, (size_t)nF * sizeof(int));
     c->total_launches += c->chain_launches[slot];
-    c->chain_tracked_frames += nF - c->chain_first[slot];
+    c->chain_tracked_frames += nF - S * c->chain_first[slot];
     if (c->prof_on) {
         float ms = 0.f;
         if (cudaEventElapsedTime(&ms, c->ev_chain_b[slot], c->ev_chain_e[slot]) == cudaSuccess) {
@@ -771,11 +870,38 @@ int rgbl_resident_track_end2(rgbl_ctx* ctx, float* poses_out, int* n_matches, in
             cudaGetLastError();
         }
     }
-    if (*cnt.overflow == kTlmWaitFailed) { c->err = "TrackLocalMap compaction: a CTA waited in vain for its predecessors (chain_kernels.cu)"; return RGBL_E_CUDA; }
-    if (*cnt.overflow) { c->err = "matcher candidate list overflow"; return RGBL_E_CAPACITY; }
+    for (int l = 0; l < S; ++l) {      // the overflow word of each lane
+        const int ovf = *chain_counts(s.h_i, nF, nF / S, l).overflow;
+        const std::string lane = S > 1 ? " (sequence lane " + std::to_string(l) + ")" : "";
+        if (ovf == kTlmWaitFailed) { c->err = "TrackLocalMap compaction: a CTA waited in vain for its predecessors (chain_kernels.cu)" + lane; return RGBL_E_CUDA; }
+        if (ovf) { c->err = "matcher candidate list overflow" + lane; return RGBL_E_CAPACITY; }
+    }
     // capacity overflow of the frame construction that produced this batch (FAST cell slots, candidate buffer, quad-tree): the chain
     // ran on truncated keypoint sets
     if (c->h_chain_ovf[2 * slot] || c->h_chain_ovf[2 * slot + 1]) { c->err = "frame-construction capacity overflow in the batch this chain tracked"; return RGBL_E_CAPACITY; }
+    return RGBL_OK;
+}
+
+int rgbl_set_sequences(rgbl_ctx* ctx, int n_sequences, const float* pose0) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (const int rc = require_idle(c)) return rc;
+    if (n_sequences < 1 || n_sequences > RGBL_MAX_SEQUENCES) { c->err = "n_sequences must be 1.." + std::to_string(RGBL_MAX_SEQUENCES); return RGBL_E_INVALID; }
+    if (pose0)
+        for (int i = 0; i < 7 * n_sequences; ++i)
+            if (!std::isfinite(pose0[i])) { c->err = "pose0 holds a non-finite value"; return RGBL_E_INVALID; }
+    c->lanes = n_sequences;
+    c->lane_pose0_set = pose0 != nullptr;
+    if (pose0) for (int l = 0; l < n_sequences; ++l) std::memcpy(c->lane_pose0[l], pose0 + 7 * l, 7 * sizeof(float));
+    return RGBL_OK;
+}
+
+int rgbl_sequence_lanes_resident(rgbl_ctx* ctx, int* n_lanes) {
+    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+    if (!c) return RGBL_E_INVALID;
+    if (!n_lanes) { c->err = "null argument"; return RGBL_E_INVALID; }
+    if (const char* why = pose_cluster_unsupported(c->cfg.device)) { c->err = why; return RGBL_E_UNSUPPORTED; }
+    *n_lanes = pose_max_active_clusters(c->cfg.device);
+    if (*n_lanes < 1) { c->err = "cudaOccupancyMaxActiveClusters failed"; return RGBL_E_CUDA; }
     return RGBL_OK;
 }
 

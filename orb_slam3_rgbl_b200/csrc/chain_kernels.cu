@@ -69,11 +69,25 @@ __device__ __forceinline__ int block_rank(int flag, int* s_wsum, int& total) {
 }
 
 // grid = n_blocks frustum CTAs (one ring point per thread) + ONE extra CTA (the last) for the slot states of the local search.
-__global__ void __launch_bounds__(kTlmThreads) tlm_prepare_kernel(FrameDev f, const float* __restrict__ pose, LocalRingDev ring, float cos_limit,
-                                                                  const int* __restrict__ n_edges, const int* __restrict__ e_idx,
-                                                                  const uint8_t* __restrict__ e_outlier, uint8_t* __restrict__ state,
-                                                                  int* __restrict__ match_last, LocalQueriesDev lq, Lookback lb) {
+// Sequence lanes: lane s = blockIdx.y with its own slot array.  CTAs are dispatched in linear order (lane-major), and a CTA waits only for
+// CTAs of its own lane with a smaller x, so still only for CTAs with a smaller linear index.
+template <bool kLanes>
+__global__ void __launch_bounds__(kTlmThreads) tlm_prepare_kernel(Laned<FrameDev> f_l, Laned<const float*> pose_l, Laned<LocalRingDev> ring_l, float cos_limit,
+                                                                  Laned<const int*> n_edges_l, Laned<const int*> e_idx_l,
+                                                                  Laned<const uint8_t*> e_outlier_l, Laned<uint8_t*> state_l,
+                                                                  Laned<int*> match_last_l, Laned<LocalQueriesDev> lq_l, Laned<Lookback> lb_l) {
     pdl_wait(); pdl_trigger();
+    const unsigned ln_ = blockIdx.y;
+    const FrameDev& f = lane_arg<kLanes>(f_l, ln_);
+    const float* __restrict__ pose = lane_arg<kLanes>(pose_l, ln_);
+    const LocalRingDev& ring = lane_arg<kLanes>(ring_l, ln_);
+    const int* __restrict__ n_edges = lane_arg<kLanes>(n_edges_l, ln_);
+    const int* __restrict__ e_idx = lane_arg<kLanes>(e_idx_l, ln_);
+    const uint8_t* __restrict__ e_outlier = lane_arg<kLanes>(e_outlier_l, ln_);
+    uint8_t* __restrict__ state = lane_arg<kLanes>(state_l, ln_);
+    int* __restrict__ match_last = lane_arg<kLanes>(match_last_l, ln_);
+    const LocalQueriesDev& lq = lane_arg<kLanes>(lq_l, ln_);
+    const Lookback& lb = lane_arg<kLanes>(lb_l, ln_);
     __shared__ int s_wsum[kTlmThreads / 32];
     __shared__ int s_base;
     const int tid = threadIdx.x;
@@ -140,11 +154,15 @@ __global__ void __launch_bounds__(kTlmThreads) tlm_prepare_kernel(FrameDev f, co
 // lb: kLbSlots + 8 zero-initialised ints owned by the caller; fail: the chain's overflow flag
 int tlm_lookback_ints() { return kLbSlots + 8; }
 
-void launch_tlm_prepare(cudaStream_t st, const FrameDev& f, const float* pose, const LocalRingDev& ring, float cos_limit, const int* n_edges,
-                        const int* e_idx, const uint8_t* e_outlier, uint8_t* state, int* match_last, const LocalQueriesDev& lq, int* lb, int* fail) {
-    const int n_part = (ring.K * ring.cap + kTlmThreads - 1) / kTlmThreads;
-    const Lookback l{lb, lb + kLbSlots, fail};
-    launch_kernel(tlm_prepare_kernel, dim3(n_part + 1), dim3(kTlmThreads), 0, st, chain_launch_pdl(), f, pose, ring, cos_limit, n_edges, e_idx, e_outlier, state, match_last, lq, l);
+void launch_tlm_prepare(cudaStream_t st, const Laned<FrameDev>& f, const Laned<const float*>& pose, const Laned<LocalRingDev>& ring, float cos_limit,
+                        const Laned<const int*>& n_edges, const Laned<const int*>& e_idx, const Laned<const uint8_t*>& e_outlier, const Laned<uint8_t*>& state,
+                        const Laned<int*>& match_last, const Laned<LocalQueriesDev>& lq, int* lb, const Laned<int*>& fail, int lanes) {
+    const int n_part = (ring.base.K * ring.base.cap + kTlmThreads - 1) / kTlmThreads;
+    const Laned<Lookback> l = laned_of(lanes, [&](int s) {
+        int* slots = lb + (size_t)s * tlm_lookback_ints();
+        return Lookback{slots, slots + kLbSlots, lane_value(fail, s)};
+    });
+    launch_kernel(lanes > 1 ? tlm_prepare_kernel<true> : tlm_prepare_kernel<false>, dim3(n_part + 1, lanes), dim3(kTlmThreads), 0, st, chain_launch_pdl(), f, pose, ring, cos_limit, n_edges, e_idx, e_outlier, state, match_last, lq, l);
 }
 
 }  // namespace rgbl

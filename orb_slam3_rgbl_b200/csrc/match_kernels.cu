@@ -252,10 +252,17 @@ __device__ __forceinline__ int warp_finish_list(const ListOut& lo, int q, int co
 }
 
 // ---- SearchByProjection(CurrentFrame, LastFrame): candidate phase --------------------------------
-__global__ void __launch_bounds__(256) search_last_collect_kernel(FrameDev f, const int* __restrict__ cell_start,
-                                                                  const int* __restrict__ csr_idx, LastFrameDev lf,
-                                                                  SearchLastParams prm, ListOut out) {
+template <bool kLanes>
+__global__ void __launch_bounds__(256) search_last_collect_kernel(Laned<FrameDev> f_l, Laned<const int*> cell_start_l, Laned<const int*> csr_idx_l,
+                                                                  Laned<LastFrameDev> lf_l, Laned<SearchLastParams> prm_l, Laned<ListOut> out_l) {
     pdl_wait(); pdl_trigger();
+    const unsigned ln_ = blockIdx.y;
+    const FrameDev& f = lane_arg<kLanes>(f_l, ln_);
+    const int* __restrict__ cell_start = lane_arg<kLanes>(cell_start_l, ln_);
+    const int* __restrict__ csr_idx = lane_arg<kLanes>(csr_idx_l, ln_);
+    const LastFrameDev& lf = lane_arg<kLanes>(lf_l, ln_);
+    const SearchLastParams& prm = lane_arg<kLanes>(prm_l, ln_);
+    const ListOut& out = lane_arg<kLanes>(out_l, ln_);
     const int q = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (q >= lf.n) return;
     int count = 0;
@@ -310,10 +317,18 @@ struct RingHandOverDev {
     LocalRingDev ring; const float* last_xw; int n_last_cap; const uint8_t* last_valid; const int* last_octave; const uint8_t* last_desc; const float* last_pose;
 };
 
-__global__ void __launch_bounds__(256) search_local_collect_kernel(FrameDev f, const int* __restrict__ cell_start,
-                                                                   const int* __restrict__ csr_idx, LocalPointsDev lp,
-                                                                   SearchLocalParams prm, ListOut out, RingHandOverDev ho) {
+template <bool kLanes>
+__global__ void __launch_bounds__(256) search_local_collect_kernel(Laned<FrameDev> f_l, Laned<const int*> cell_start_l, Laned<const int*> csr_idx_l,
+                                                                   Laned<LocalPointsDev> lp_l, SearchLocalParams prm, Laned<ListOut> out_l,
+                                                                   Laned<RingHandOverDev> ho_l) {
     pdl_wait(); pdl_trigger();
+    const unsigned ln_ = blockIdx.y;
+    const FrameDev& f = lane_arg<kLanes>(f_l, ln_);
+    const int* __restrict__ cell_start = lane_arg<kLanes>(cell_start_l, ln_);
+    const int* __restrict__ csr_idx = lane_arg<kLanes>(csr_idx_l, ln_);
+    const LocalPointsDev& lp = lane_arg<kLanes>(lp_l, ln_);
+    const ListOut& out = lane_arg<kLanes>(out_l, ln_);
+    const RingHandOverDev& ho = lane_arg<kLanes>(ho_l, ln_);
     if (ho.ring.valid) {
         const int j = blockIdx.x * 256 + threadIdx.x;
         if (j < ho.ring.cap) {
@@ -396,17 +411,35 @@ struct ChainTlmDev {
     int* n_local_matches;
 };
 
-__global__ void __launch_bounds__(1024) resolve_kernel(int mode, int n_q, const int* __restrict__ n_q_dev, FrameDev f,
-                                                       ListOut lo,
-                                                       const uint8_t* __restrict__ obs_pos,
-                                                       const float* __restrict__ q_angle, float nn_ratio,
+// One CTA per lane (blockIdx.y); the lane's arguments are read once into registers (Laned, rgbl_kernels.h).
+template <bool kLanes>
+__global__ void __launch_bounds__(1024) resolve_kernel(int mode, int n_q, Laned<const int*> n_q_dev_l, Laned<FrameDev> f_l,
+                                                       Laned<ListOut> lo_l,
+                                                       Laned<const uint8_t*> obs_pos_l,
+                                                       Laned<const float*> q_angle_l, float nn_ratio,
                                                        int check_orientation, int th_accept,
-                                                       const float* __restrict__ f_angle, uint8_t* __restrict__ state,
-                                                       int* __restrict__ minq, int* __restrict__ choice,
-                                                       uint8_t* __restrict__ resolved, int* __restrict__ match,
-                                                       int* __restrict__ n_matches, int* __restrict__ rounds_out, int dyn_bytes,
-                                                       ChainEdgesDev ce, ChainTlmDev tl) {
+                                                       Laned<const float*> f_angle_l, Laned<uint8_t*> state_l,
+                                                       Laned<int*> minq_l, Laned<int*> choice_l,
+                                                       Laned<uint8_t*> resolved_l, Laned<int*> match_l,
+                                                       Laned<int*> n_matches_l, Laned<int*> rounds_out_l, int dyn_bytes,
+                                                       Laned<ChainEdgesDev> ce_l, Laned<ChainTlmDev> tl_l) {
     pdl_wait(); pdl_trigger();
+    const unsigned ln_ = blockIdx.y;
+    const int* __restrict__ n_q_dev = lane_arg<kLanes>(n_q_dev_l, ln_);
+    const FrameDev& f = lane_arg<kLanes>(f_l, ln_);
+    const ListOut& lo = lane_arg<kLanes>(lo_l, ln_);
+    const uint8_t* __restrict__ obs_pos = lane_arg<kLanes>(obs_pos_l, ln_);
+    const float* __restrict__ q_angle = lane_arg<kLanes>(q_angle_l, ln_);
+    const float* __restrict__ f_angle = lane_arg<kLanes>(f_angle_l, ln_);
+    uint8_t* __restrict__ state = lane_arg<kLanes>(state_l, ln_);
+    int* __restrict__ minq = lane_arg<kLanes>(minq_l, ln_);
+    int* __restrict__ choice = lane_arg<kLanes>(choice_l, ln_);
+    uint8_t* __restrict__ resolved = lane_arg<kLanes>(resolved_l, ln_);
+    int* __restrict__ match = lane_arg<kLanes>(match_l, ln_);
+    int* __restrict__ n_matches = lane_arg<kLanes>(n_matches_l, ln_);
+    int* __restrict__ rounds_out = lane_arg<kLanes>(rounds_out_l, ln_);
+    const ChainEdgesDev& ce = lane_arg<kLanes>(ce_l, ln_);
+    const ChainTlmDev& tl = lane_arg<kLanes>(tl_l, ln_);
     const MatchEntry* __restrict__ lists = lo.lists;
     const int list_cap = lo.list_cap;
     const int* __restrict__ list_n = lo.list_n;
@@ -1086,7 +1119,10 @@ __global__ void __launch_bounds__(256) search_reloc_collect_kernel(FrameDev f, c
 // ---- resident tracking chain (TrackWithMotionModel-style glue between the reference functions) ----------------
 // Every keypoint of the last frame that has a LiDAR depth acts as a map point: Frame::UnprojectStereo
 // (src/Frame.cc:1137-1150) with the last pose, descriptor = the keypoint's own descriptor.
-__global__ void __launch_bounds__(256) chain_prep_kernel(ChainPrepDev cp, const float* __restrict__ last_pose) {
+template <bool kLanes>
+__global__ void __launch_bounds__(256) chain_prep_kernel(Laned<ChainPrepDev> cp_l, Laned<const float*> last_pose_l) {
+    const ChainPrepDev& cp = lane_arg<kLanes>(cp_l, blockIdx.y);
+    const float* __restrict__ last_pose = lane_arg<kLanes>(last_pose_l, blockIdx.y);
     const int i = blockIdx.x * 256 + threadIdx.x;
     if (i == 0) chain_prep_motion(cp, last_pose);
     float Rwc[9], Ow[3];
@@ -1103,7 +1139,8 @@ static int resolve_dyn_bytes() {
     int dev = 0;
     cudaGetDevice(&dev);
     if (dev >= 0 && dev < 64 && !done[dev]) {
-        cudaFuncSetAttribute(resolve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kBytes);
+        cudaFuncSetAttribute(resolve_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBytes);
+        cudaFuncSetAttribute(resolve_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBytes);
         done[dev] = true;
     }
     return kBytes;
@@ -1121,34 +1158,62 @@ void launch_grid_build_batch(cudaStream_t st, const FrameDev& f, int n_frames, i
     grid_build_kernel<<<n_frames, 1024, 0, st>>>(f, kp_stride, cell_start, csr_idx, kp_cell);
 }
 
-void launch_search_last(cudaStream_t st, const FrameDev& f, const int* cell_start, const int* csr_idx, const LastFrameDev& lf,
-                        const SearchLastParams& prm, MatchScratch s, uint8_t* state, int* match, int* n_matches,
-                        const ChainEdgesOut* edges) {
-    if (lf.n <= 0) return;
-    const bool pdl = chain_launch_pdl();
-    launch_kernel(search_last_collect_kernel, dim3((lf.n + 7) / 8), dim3(256), 0, st, pdl, f, cell_start, csr_idx, lf, prm, ListOut{s.lists, s.slots, s.list_cap, s.list_n, s.dense, s.dense_slot, s.dense_q, s.base, s.total, s.inv_cnt, s.overflow});
-    launch_kernel(resolve_kernel, dim3(1), dim3(1024), (size_t)resolve_dyn_bytes(), st, pdl, 0, lf.n, (const int*)nullptr, f, ListOut{s.lists, s.slots, s.list_cap, s.list_n, s.dense, s.dense_slot, s.dense_q, s.base, s.total, s.inv_cnt, s.overflow}, lf.obs_pos, lf.angle, 0.f,
-                                       prm.check_orientation, kThHigh, (const float*)nullptr, state, s.minq, s.choice, s.resolved, match, n_matches, s.rounds, resolve_dyn_bytes(),
-                                       edges ? ChainEdgesDev{f.keys, f.uright, lf.xw, edges->exw, edges->eobs, edges->einfo, edges->est, edges->eidx, edges->n_edges} : ChainEdgesDev{}, ChainTlmDev{});
+static ListOut list_out(const MatchScratch& s) {
+    return ListOut{s.lists, s.slots, s.list_cap, s.list_n, s.dense, s.dense_slot, s.dense_q, s.base, s.total, s.inv_cnt, s.overflow};
 }
 
-void launch_search_local(cudaStream_t st, const FrameDev& f, const int* cell_start, const int* csr_idx, const LocalPointsDev& lp,
-                         const SearchLocalParams& prm, MatchScratch s, uint8_t* state, int* match, int* n_matches, const ChainTlmTail* tail) {
-    if (lp.n <= 0) return;
-    RingHandOverDev ho{};
-    if (tail) ho = RingHandOverDev{tail->ring, tail->last_xw, tail->n_last_cap, tail->last_valid, tail->last_octave, tail->last_desc, tail->last_pose};
-    const int n_q_cta = (lp.n + 7) / 8, n_ho_cta = tail ? (tail->ring.cap + 255) / 256 : 0;
+void launch_search_last(cudaStream_t st, const Laned<FrameDev>& f, const Laned<const int*>& cell_start, const Laned<const int*>& csr_idx,
+                        const Laned<LastFrameDev>& lf, const Laned<SearchLastParams>& prm, const Laned<MatchScratch>& s, const Laned<uint8_t*>& state,
+                        const Laned<int*>& match, const Laned<int*>& n_matches, const Laned<ChainEdgesOut>* edges, int lanes) {
+    const LastFrameDev lf0 = lf.base;
+    if (lf0.n <= 0) return;
+    const bool pdl = chain_launch_pdl();
+    const Laned<ListOut> lo = laned_of(lanes, [&](int l) { return list_out(lane_value(s, l)); });
+    launch_kernel(lanes > 1 ? search_last_collect_kernel<true> : search_last_collect_kernel<false>, dim3((lf0.n + 7) / 8, lanes), dim3(256), 0, st, pdl, f, cell_start, csr_idx, lf, prm, lo);
+    const auto ls = [&](int l) { return lane_value(s, l); };
+    const Laned<ChainEdgesDev> ce = laned_of(lanes, [&](int l) {
+        if (!edges) return ChainEdgesDev{};
+        const FrameDev fl = lane_value(f, l); const LastFrameDev ll = lane_value(lf, l); const ChainEdgesOut e = lane_value(*edges, l);
+        return ChainEdgesDev{fl.keys, fl.uright, ll.xw, e.exw, e.eobs, e.einfo, e.est, e.eidx, e.n_edges};
+    });
+    launch_kernel(lanes > 1 ? resolve_kernel<true> : resolve_kernel<false>, dim3(1, lanes), dim3(1024), (size_t)resolve_dyn_bytes(), st, pdl, 0, lf0.n, Laned<const int*>(), f, lo,
+                  laned_of(lanes, [&](int l) { return lane_value(lf, l).obs_pos; }), laned_of(lanes, [&](int l) { return lane_value(lf, l).angle; }), 0.f,
+                  prm.base.check_orientation, kThHigh, Laned<const float*>(), state, laned_of(lanes, [&](int l) { return ls(l).minq; }),
+                  laned_of(lanes, [&](int l) { return ls(l).choice; }), laned_of(lanes, [&](int l) { return ls(l).resolved; }), match, n_matches,
+                  laned_of(lanes, [&](int l) { return ls(l).rounds; }), resolve_dyn_bytes(), ce, Laned<ChainTlmDev>());
+}
+
+void launch_search_local(cudaStream_t st, const Laned<FrameDev>& f, const Laned<const int*>& cell_start, const Laned<const int*>& csr_idx,
+                         const Laned<LocalPointsDev>& lp, const SearchLocalParams& prm, const Laned<MatchScratch>& s, const Laned<uint8_t*>& state,
+                         const Laned<int*>& match, const Laned<int*>& n_matches, const Laned<ChainTlmTail>* tail, int lanes) {
+    const int n_lp = lp.base.n;
+    if (n_lp <= 0) return;
+    const Laned<RingHandOverDev> ho = laned_of(lanes, [&](int l) {
+        if (!tail) return RingHandOverDev{};
+        const ChainTlmTail t = lane_value(*tail, l);
+        return RingHandOverDev{t.ring, t.last_xw, t.n_last_cap, t.last_valid, t.last_octave, t.last_desc, t.last_pose};
+    });
+    const int n_q_cta = (n_lp + 7) / 8, n_ho_cta = tail ? (tail->base.ring.cap + 255) / 256 : 0;
     const int n_cta = n_q_cta > n_ho_cta ? n_q_cta : n_ho_cta;
     const bool pdl = chain_launch_pdl();
-    launch_kernel(search_local_collect_kernel, dim3(n_cta), dim3(256), 0, st, pdl, f, cell_start, csr_idx, lp, prm, ListOut{s.lists, s.slots, s.list_cap, s.list_n, s.dense, s.dense_slot, s.dense_q, s.base, s.total, s.inv_cnt, s.overflow}, ho);
-    ChainEdgesDev ce{};
-    ChainTlmDev tl{};
-    if (tail) {
-        ce = ChainEdgesDev{f.keys, f.uright, tail->last_xw, tail->edges.exw, tail->edges.eobs, tail->edges.einfo, tail->edges.est, tail->edges.eidx, tail->edges.n_edges};
-        tl = ChainTlmDev{tail->match_last, tail->lq_xw, tail->ring.count, tail->n_local_matches};
-    }
-    launch_kernel(resolve_kernel, dim3(1), dim3(1024), (size_t)resolve_dyn_bytes(), st, pdl, 1, lp.n, lp.n_dev, f, ListOut{s.lists, s.slots, s.list_cap, s.list_n, s.dense, s.dense_slot, s.dense_q, s.base, s.total, s.inv_cnt, s.overflow}, lp.obs_pos, (const float*)nullptr, prm.nn_ratio,
-                                       0, kThHigh, (const float*)nullptr, state, s.minq, s.choice, s.resolved, match, n_matches, s.rounds, resolve_dyn_bytes(), ce, tl);
+    const auto ls = [&](int l) { return lane_value(s, l); };
+    const Laned<ListOut> lo = laned_of(lanes, [&](int l) { return list_out(ls(l)); });
+    launch_kernel(lanes > 1 ? search_local_collect_kernel<true> : search_local_collect_kernel<false>, dim3(n_cta, lanes), dim3(256), 0, st, pdl, f, cell_start, csr_idx, lp, prm, lo, ho);
+    const Laned<ChainEdgesDev> ce = laned_of(lanes, [&](int l) {
+        if (!tail) return ChainEdgesDev{};
+        const FrameDev fl = lane_value(f, l); const ChainTlmTail t = lane_value(*tail, l);
+        return ChainEdgesDev{fl.keys, fl.uright, t.last_xw, t.edges.exw, t.edges.eobs, t.edges.einfo, t.edges.est, t.edges.eidx, t.edges.n_edges};
+    });
+    const Laned<ChainTlmDev> tl = laned_of(lanes, [&](int l) {
+        if (!tail) return ChainTlmDev{};
+        const ChainTlmTail t = lane_value(*tail, l);
+        return ChainTlmDev{t.match_last, t.lq_xw, t.ring.count, t.n_local_matches};
+    });
+    launch_kernel(lanes > 1 ? resolve_kernel<true> : resolve_kernel<false>, dim3(1, lanes), dim3(1024), (size_t)resolve_dyn_bytes(), st, pdl, 1, n_lp,
+                  laned_of(lanes, [&](int l) { return lane_value(lp, l).n_dev; }), f, lo, laned_of(lanes, [&](int l) { return lane_value(lp, l).obs_pos; }),
+                  Laned<const float*>(), prm.nn_ratio, 0, kThHigh, Laned<const float*>(), state, laned_of(lanes, [&](int l) { return ls(l).minq; }),
+                  laned_of(lanes, [&](int l) { return ls(l).choice; }), laned_of(lanes, [&](int l) { return ls(l).resolved; }), match, n_matches,
+                  laned_of(lanes, [&](int l) { return ls(l).rounds; }), resolve_dyn_bytes(), ce, tl);
 }
 
 void launch_search_bow(cudaStream_t st, const FrameDev& f, int n_q, const int* q_feat, const int* q_cbeg, const int* q_cend,
@@ -1158,7 +1223,7 @@ void launch_search_bow(cudaStream_t st, const FrameDev& f, int n_q, const int* q
     if (n_q <= 0) return;
     bow_collect_kernel<<<(n_q + 7) / 8, 256, 0, st>>>(n_q, q_feat, q_cbeg, q_cend, kf_desc, f_desc, f_node_feat, q_angle, f_angle, check_orientation, keep_max,
                                                     ListOut{s.lists, s.slots, s.list_cap, s.list_n, s.dense, s.dense_slot, s.dense_q, s.base, s.total, s.inv_cnt, s.overflow});
-    resolve_kernel<<<1, 1024, resolve_dyn_bytes(), st>>>(2, n_q, nullptr, f, ListOut{s.lists, s.slots, s.list_cap, s.list_n, s.dense, s.dense_slot, s.dense_q, s.base, s.total, s.inv_cnt, s.overflow}, obs_pos, q_angle, nn_ratio,
+    resolve_kernel<false><<<1, 1024, resolve_dyn_bytes(), st>>>(2, n_q, nullptr, f, ListOut{s.lists, s.slots, s.list_cap, s.list_n, s.dense, s.dense_slot, s.dense_q, s.base, s.total, s.inv_cnt, s.overflow}, obs_pos, q_angle, nn_ratio,
                                        check_orientation, 50 /* TH_LOW */, f_angle, state, s.minq, s.choice, s.resolved, match, n_matches, s.rounds, resolve_dyn_bytes(), ChainEdgesDev{}, ChainTlmDev{});
 }
 
@@ -1166,7 +1231,7 @@ void launch_search_reloc(cudaStream_t st, const FrameDev& f, const int* cell_sta
                          const SearchRelocParams& prm, const uint8_t* obs_pos, MatchScratch s, uint8_t* state, int* match, int* n_matches) {
     if (rp.n <= 0) return;
     search_reloc_collect_kernel<<<(rp.n + 7) / 8, 256, 0, st>>>(f, cell_start, csr_idx, rp, prm, ListOut{s.lists, s.slots, s.list_cap, s.list_n, s.dense, s.dense_slot, s.dense_q, s.base, s.total, s.inv_cnt, s.overflow});
-    resolve_kernel<<<1, 1024, resolve_dyn_bytes(), st>>>(0, rp.n, nullptr, f, ListOut{s.lists, s.slots, s.list_cap, s.list_n, s.dense, s.dense_slot, s.dense_q, s.base, s.total, s.inv_cnt, s.overflow}, obs_pos, rp.angle, 0.f,
+    resolve_kernel<false><<<1, 1024, resolve_dyn_bytes(), st>>>(0, rp.n, nullptr, f, ListOut{s.lists, s.slots, s.list_cap, s.list_n, s.dense, s.dense_slot, s.dense_q, s.base, s.total, s.inv_cnt, s.overflow}, obs_pos, rp.angle, 0.f,
                                        prm.check_orientation, prm.orb_dist, nullptr, state, s.minq, s.choice, s.resolved, match, n_matches, s.rounds, resolve_dyn_bytes(), ChainEdgesDev{}, ChainTlmDev{});
 }
 
@@ -1178,8 +1243,9 @@ void launch_fuse_search(cudaStream_t st, const FrameDev& f, const int* cell_star
                                                   best_idx, best_dist);
 }
 
-void launch_chain_prep(cudaStream_t st, const ChainPrepDev& cp, const float* last_pose) {
-    chain_prep_kernel<<<(cp.cap + 255) / 256, 256, 0, st>>>(cp, last_pose);
+void launch_chain_prep(cudaStream_t st, const Laned<ChainPrepDev>& cp, const Laned<const float*>& last_pose, int lanes) {
+    if (lanes > 1) chain_prep_kernel<true><<<dim3((cp.base.cap + 255) / 256, lanes), 256, 0, st>>>(cp, last_pose);
+    else chain_prep_kernel<false><<<dim3((cp.base.cap + 255) / 256, 1), 256, 0, st>>>(cp, last_pose);
 }
 
 void launch_frustum(cudaStream_t st, const FrameDev& f, const FrustumParams& prm, int n, const float* xw, const float* normal,

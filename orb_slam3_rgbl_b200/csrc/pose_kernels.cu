@@ -337,9 +337,9 @@ __device__ constexpr bool kJnz[3][6] = {{true, true, true, true, false, true}, {
 
 }  // namespace
 
-__global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads) pose_optimize_kernel(PoseProblemDev p, double* __restrict__ work, uint8_t* __restrict__ level,
-                                                            uint8_t* __restrict__ outlier, float* __restrict__ pose_out,
-                                                            int* __restrict__ n_inliers, ChainPrepDev next) {
+__global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads) pose_optimize_kernel(Laned<PoseProblemDev> p_l, Laned<double*> work_l, Laned<uint8_t*> level_l,
+                                                            Laned<uint8_t*> outlier_l, Laned<float*> pose_out_l,
+                                                            Laned<int*> n_inliers_l, Laned<ChainPrepDev> next_l) {
     __shared__ double red[kPoseWarps * kXchg];
     __shared__ double acc[kXchg];         // the cluster totals of the last exchange: the system the next solves start from + one value
     __shared__ __align__(16) double xchg_buf[2][kPoseCtas][32];      // partial sums of the CTAs (written remotely by st.async)
@@ -355,6 +355,15 @@ __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads
     __shared__ Se3d s_est, s_init, s_cand[kMaxTrials];
     __shared__ double s_cinv[kMaxTrials], s_lambda, s_ni, s_current, s_ini;
     __shared__ int s_build, s_nbad_lm, s_ok, s_cok[kMaxTrials], s_continue;
+    // sequence lane = the cluster's y (the exchange and the next frame's preparation stay inside the lane's cluster)
+    const unsigned ln_ = blockIdx.y;
+    const PoseProblemDev p = lane_value(p_l, ln_);
+    double* __restrict__ work = lane_value(work_l, ln_);
+    uint8_t* __restrict__ level = lane_value(level_l, ln_);
+    uint8_t* __restrict__ outlier = lane_value(outlier_l, ln_);
+    float* __restrict__ pose_out = lane_value(pose_out_l, ln_);
+    int* __restrict__ n_inliers = lane_value(n_inliers_l, ln_);
+    const ChainPrepDev next = lane_value(next_l, ln_);
     const int tid = threadIdx.x, n = p.n_dev ? *p.n_dev : p.n;
     const int gtid = (int)rank * kPoseThreads + tid;
 #ifdef POSE_TIMING
@@ -677,9 +686,20 @@ const char* pose_cluster_unsupported(int device) {
     return state[device] == 1 ? nullptr : why.c_str();
 }
 
-void launch_pose_optimize(cudaStream_t st, const PoseProblemDev& p, double* work, uint8_t* level, uint8_t* outlier,
-                          float* pose_out, int* n_inliers, const ChainPrepDev* next) {
-    launch_kernel(pose_optimize_kernel, dim3(kPoseCtas), dim3(kPoseThreads), 0, st, chain_launch_pdl(), p, work, level, outlier, pose_out, n_inliers, next ? *next : ChainPrepDev{});
+int pose_max_active_clusters(int device) {
+    if (pose_cluster_unsupported(device)) return 0;
+    int n = 0;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(kPoseCtas); cfg.blockDim = dim3(kPoseThreads);
+    if (cudaSetDevice(device) != cudaSuccess || cudaOccupancyMaxActiveClusters(&n, pose_optimize_kernel, &cfg) != cudaSuccess) { cudaGetLastError(); return 0; }
+    return n;
+}
+
+void launch_pose_optimize(cudaStream_t st, const Laned<PoseProblemDev>& p, const Laned<double*>& work, const Laned<uint8_t*>& level,
+                          const Laned<uint8_t*>& outlier, const Laned<float*>& pose_out, const Laned<int*>& n_inliers, const Laned<ChainPrepDev>* next,
+                          int lanes) {
+    launch_kernel(pose_optimize_kernel, dim3(kPoseCtas, lanes), dim3(kPoseThreads), 0, st, chain_launch_pdl(), p, work, level, outlier, pose_out, n_inliers,
+                  next ? *next : Laned<ChainPrepDev>());
 }
 
 }  // namespace rgbl

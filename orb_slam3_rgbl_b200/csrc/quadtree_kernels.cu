@@ -14,7 +14,7 @@
 namespace rgbl {
 
 template <int MAXN>
-__global__ void __launch_bounds__(512, MAXN <= 512 ? 2 : 1) quadtree_kernel(const uint32_t* __restrict__ dense, const int* __restrict__ level_cnt,
+__global__ void __launch_bounds__(512, MAXN <= 512 ? 2 : 1) quadtree_kernel(const uint32_t* __restrict__ dense, int dense_cap, const int* __restrict__ level_cnt,
                                                        const int* __restrict__ frame_total, const LevelGeom* __restrict__ levels,
                                                        int n_levels, QtScratchDev scr, uint32_t* __restrict__ sel_lvl,
                                                        int* __restrict__ n_sel_lvl, const int* __restrict__ lvl_region,
@@ -28,7 +28,11 @@ __global__ void __launch_bounds__(512, MAXN <= 512 ? 2 : 1) quadtree_kernel(cons
     int off = 0;
     for (int k = 0; k < f; ++k) off += frame_total[k];
     for (int k = 0; k < l; ++k) off += level_cnt[f * RGBL_MAX_LEVELS + k];
-    const int n = level_cnt[f * RGBL_MAX_LEVELS + l];
+    int n = level_cnt[f * RGBL_MAX_LEVELS + l];
+    // after a candidate-buffer overflow (flagged by the gather, reported as RGBL_E_CAPACITY) the counts run past the buffer: the trees
+    // beyond its end are empty and the one across it is cut, so no tree reads or writes outside the candidate and scratch arrays
+    off = min(off, dense_cap);
+    n = max(0, min(n, dense_cap - off));
     const LevelGeom lg = levels[l];
     qt::Scratch g;
     const int so = off + (f * n_levels + l);          // one extra scan slot per preceding tree
@@ -104,7 +108,7 @@ static int quadtree_dyn_bytes(int ctas_per_sm) {
 
 int launch_quadtree(cudaStream_t st, const uint32_t* dense, const int* level_cnt, const int* frame_total, const LevelGeom* d_levels,
                     int n_levels, const QtScratchDev& scr, uint32_t* sel_lvl, int* n_sel_lvl, const int* lvl_region, int cap_kp,
-                    int* status, SelKp* sel, int* n_sel, int n_frames, int max_nodes) {
+                    int* status, SelKp* sel, int* n_sel, int n_frames, int max_nodes, int dense_cap) {
     // max_nodes = the largest node list any level of the context needs (max(quota + 3, 4 nIni)): <= 512 selects the half-size tree state
     // with two CTAs per SM
     static int dyn512 = 0, dyn1024 = 0;
@@ -113,10 +117,10 @@ int launch_quadtree(cudaStream_t st, const uint32_t* dense, const int* level_cnt
     if (!dyn_bytes) dyn_bytes = small ? quadtree_dyn_bytes<512>(2) : quadtree_dyn_bytes<1024>(1);
     if (dyn_bytes <= 0) return -1;
     if (small)
-        quadtree_kernel<512><<<dim3(n_frames, n_levels), 512, dyn_bytes, st>>>(dense, level_cnt, frame_total, d_levels, n_levels, scr, sel_lvl, n_sel_lvl,
+        quadtree_kernel<512><<<dim3(n_frames, n_levels), 512, dyn_bytes, st>>>(dense, dense_cap, level_cnt, frame_total, d_levels, n_levels, scr, sel_lvl, n_sel_lvl,
                                                                              lvl_region, cap_kp, status, dyn_bytes);
     else
-        quadtree_kernel<1024><<<dim3(n_frames, n_levels), 512, dyn_bytes, st>>>(dense, level_cnt, frame_total, d_levels, n_levels, scr, sel_lvl, n_sel_lvl,
+        quadtree_kernel<1024><<<dim3(n_frames, n_levels), 512, dyn_bytes, st>>>(dense, dense_cap, level_cnt, frame_total, d_levels, n_levels, scr, sel_lvl, n_sel_lvl,
                                                                               lvl_region, cap_kp, status, dyn_bytes);
     sel_pack_kernel<<<n_frames, 256, 0, st>>>(sel_lvl, n_sel_lvl, lvl_region, n_levels, cap_kp, sel, n_sel);
     return 0;

@@ -19,6 +19,7 @@ static const char* const kStageNames[kNumStages] = {"pyramid", "fast", "compact"
                                               "depth_resolve_dilate", "depth_gather", "match", "pose", "quadtree"};
 
 constexpr int kMatchListCap = 512;    // admissible candidates kept per map point (overflow is reported)
+static_assert(RGBL_MAX_SEQUENCES == kMaxLanes, "the header's sequence bound is the chain's lane bound");
 
 // the inputs of a resident upload or a staged slot: RGB-L (image + point cloud), RGB-D (image + uint16 depth plane), stereo (left and
 // right image of a pair: rectified, or raw when the context rectifies them)
@@ -57,23 +58,46 @@ struct ChainCarry { int n_sel; float pose[7]; int ring_count; float prev_pose[7]
 static_assert(sizeof(ChainCarry) == 16 * 4 && offsetof(ChainCarry, pose) == 4 && offsetof(ChainCarry, ring_count) == 32 &&
               offsetof(ChainCarry, prev_pose) == 36, "ChainCarry is 16 packed 32-bit words");
 
-// Counters of one chain over nF frames: TrackBufs::ch_counts on the device, a slot of Ctx::h_chain_i on the host (one copy brings all of
-// them back).  Four blocks of nF ints, then the tail: edges of the first and the second PoseOptimization, the forward / backward flags of the
-// last-frame search, the overflow word (matcher list overflow, or kTlmWaitFailed), the local search's query count.
+// Counters of one chain over nF frames in `lanes` sequence lanes of m = nF / lanes frames: TrackBufs::ch_counts on the device, a slot of
+// Ctx::h_chain_i on the host (one copy brings all of them back).  Four blocks of nF ints in batch order (lane s's frame k at s * m + k), then
+// one tail of 8 ints per lane: edges of the first and the second PoseOptimization, the forward / backward flags of the last-frame search,
+// the overflow word (matcher list overflow, or kTlmWaitFailed), the local search's query count.
 struct ChainCounts { int *n_matches, *n_inliers, *n_local_matches, *n_inliers_first, *n_edges, *n_edges2, *flags, *overflow, *n_queries; };
-constexpr size_t chain_count_ints(size_t nF) { return 4 * nF + 8; }
-inline ChainCounts chain_counts(int* base, size_t nF) {
-    int* tail = base + 4 * nF;
-    return {base, base + nF, base + 2 * nF, base + 3 * nF, tail, tail + 1, tail + 2, tail + 4, tail + 5};
+constexpr size_t chain_count_ints(size_t nF, size_t lanes) { return 4 * nF + 8 * lanes; }
+// lane s's counters (its frame 0 and its tail)
+inline ChainCounts chain_counts(int* base, size_t nF, size_t m, size_t s) {
+    int* head = base + s * m;
+    int* tail = base + 4 * nF + 8 * s;
+    return {head, head + nF, head + 2 * nF, head + 3 * nF, tail, tail + 1, tail + 2, tail + 4, tail + 5};
 }
-// Poses of one chain in a slot of Ctx::h_chain_f: the pose given for frame 0 (read by a chain that starts a sequence), then the nF results
-constexpr size_t chain_pose_floats(size_t nF) { return 7 + nF * 7; }
+// Poses of one chain in a slot of Ctx::h_chain_f: the pose given for frame 0 of each lane (kMaxLanes x 7, read by a chain that starts a
+// sequence), then the nF results in batch order
+constexpr size_t kChainPose0Floats = 7 * (size_t)kMaxLanes;
+constexpr size_t chain_pose_floats(size_t nF) { return kChainPose0Floats + nF * 7; }
 
 // Launch parameters of a chain: with the context's buffers and its settings fixed at rgbl_create, everything the enqueue of the chain
 // reads (api_track.cu: enqueue_chain takes this struct and nothing else of the call).
-struct ChainPlan { int nF, cap, mono, cont, K, prev_valid; float th, th_local, nn_local, fx, fy, cx, cy, bf, bounds[4]; };
+// lanes: sequence lanes (rgbl_set_sequences), m = nF / lanes frames each.
+struct ChainPlan { int nF, cap, mono, cont, K, prev_valid, lanes, m; float th, th_local, nn_local, fx, fy, cx, cy, bf, bounds[4]; };
 // capacity of the query arrays of the chain's local search: the queries are compacted, at most every point of the local map ring
 inline int local_query_cap(const ChainPlan& p) { return std::max(p.K * p.cap, 1); }
+// The chain's per-lane layout: every TrackBufs buffer the chain writes holds plan.lanes lanes, lane s of a buffer at base + s * stride
+// (elements).  ensure_chain_resources grows each buffer to lanes x its stride and chain_lane (api_track.cu) carves lane s with these and
+// nothing else.  The batch's frames (the slot snapshot, the grids, ch_poses, ch_counts) are in batch order: lane s's frame k is s * m + k.
+struct ChainLaneStrides {
+    size_t kp;         // per keypoint of a frame (cap): state, match, match_local, minq, e_*, c_kps, c_depth; x 3: e_xw, e_obs, pose_work; x 32: c_desc
+    size_t inv;        // inv_cnt: cap per-feature counters + the dense run's entry total
+    size_t q;          // queries (max(cap, local query cap)): q_*, list_n, list_base, choice, resolved; x 3: q_f3*; x kMatchListCap: lists, dense*
+    size_t ring;       // local map ring (K x cap): r_valid, r_min, r_max; x 3: r_xw, r_normal; x 32: r_desc
+    size_t lq;         // local queries (local query cap): planes of lq_u8 / lq_f / lq_i (kLq*Planes each), x 32: lq_desc
+    size_t scalars;    // TrackBufs::scalars: 16 words
+    size_t lookback;   // tlm_prepare's slot array: tlm_lookback_ints()
+    size_t pose_tmp;   // ch_poses after the nF results: pose after TrackWithMotionModel | predicted pose (14 floats)
+};
+inline ChainLaneStrides chain_lane_strides(const ChainPlan& p) {
+    const size_t cap = (size_t)p.cap, lq = (size_t)local_query_cap(p);
+    return {cap, cap + 1, std::max(cap, lq), (size_t)p.K * cap, lq, 16, (size_t)tlm_lookback_ints(), 14};
+}
 // Key of a slot's CUDA graph: the plan, and Ctx::scratch_generation for the buffer addresses.  Compared with memcmp: value-initialise it.
 struct ChainGraphKey { ChainPlan plan; unsigned long long generation; };
 static_assert(sizeof(ChainPlan) % sizeof(unsigned long long) == 0, "no padding in ChainGraphKey");
@@ -95,7 +119,7 @@ struct TrackBufs {
     DeviceArray<int> s_nsel, b_cell_start, b_csr_idx, b_kp_cell;
     // state that persists between the chains of one sequence: the carried last frame and the local map ring (chain_kernels.cu)
     DeviceArray<rgbl_keypoint> c_kps; DeviceArray<uint8_t> c_desc; DeviceArray<float> c_depth;
-    DeviceArray<ChainCarry> carry;                       // one element
+    DeviceArray<ChainCarry> carry;                       // one element per sequence lane
     DeviceArray<uint8_t> r_valid, r_desc, lq_u8, lq_desc; DeviceArray<float> r_xw, r_normal, r_min, r_max, lq_f; DeviceArray<int> lq_i, match_local;
     DeviceArray<int> lookback;                           // slot arrays of the multi-CTA compactions (chain_kernels.cu), kept zero between launches
     // ComputeBoW
@@ -212,9 +236,12 @@ struct Ctx {
     Event ev_snap, ev_chain_b[2], ev_chain_e[2], ev_chain_done[2];
     int chain_pending = 0;       // chains in flight (0..2)
     int chain_head = 0;          // slot of the oldest chain in flight
-    int chain_frames[2] = {}, chain_launches[2] = {}, chain_first[2] = {}, chain_graph_launches[2] = {};
+    int chain_frames[2] = {}, chain_lanes[2] = {1, 1}, chain_launches[2] = {}, chain_first[2] = {}, chain_graph_launches[2] = {};
     long chain_tracked_frames = 0;               // frames that went through the chain (frame 0 of a non-continuing chain is given, not tracked)
-    bool chain_has_carry = false; int carry_K = 0, carry_cap = 0;
+    bool chain_has_carry = false; int carry_K = 0, carry_cap = 0, carry_lanes = 1;
+    // sequence lanes (rgbl_set_sequences): batches hold `lanes` sequences of consecutive frames; lane_pose0[s] = lane s's start pose when
+    // lane_pose0_set (else every lane starts at rgbl_chain_params::pose0)
+    int lanes = 1; bool lane_pose0_set = false; float lane_pose0[kMaxLanes][7] = {};
     bool carry_prev_valid = false;               // the carried sequence also holds the pose BEFORE its last frame (constant-velocity motion model)
     PinnedArray<int> h_chain_ovf;                // per slot: the two frame-construction overflow flags of the tracked batch
     // The chain's CUDA graphs hold raw pointers into the buffers of this context.  Every buffer that can be reallocated after
@@ -303,17 +330,17 @@ inline ChainSlot chain_slot(Ctx* c, int slot) {
     const size_t nF = slot_frames(c), tot = nF * c->cap_kp, cs = nF * (kGridCols * kGridRows + 1);
     return {t.s_kps + slot * tot, t.s_desc + slot * tot * 32, t.s_depth + slot * tot, t.s_uright + slot * tot, t.s_nsel + slot * nF,
             t.b_cell_start + slot * cs, t.b_csr_idx + slot * tot, t.b_kp_cell + slot * tot,
-            c->h_chain_f + slot * chain_pose_floats(c->h_chain_cap), c->h_chain_i + slot * chain_count_ints(c->h_chain_cap)};
+            c->h_chain_f + slot * chain_pose_floats(c->h_chain_cap), c->h_chain_i + slot * chain_count_ints(c->h_chain_cap, kMaxLanes)};
 }
 
-// The query arrays of the chain's local search: planes of n_lq elements in lq_u8 (2), lq_f (8: five scalars, then xyz) and lq_i (2)
+// The query arrays of the chain's local search (one lane): planes of n_lq elements in lq_u8 (2), lq_f (8: five scalars, then xyz) and lq_i (2)
 constexpr int kLqU8Planes = 2, kLqFPlanes = 8, kLqIPlanes = 2;
-inline LocalQueriesDev local_queries(TrackBufs& t, int n_lq, int* n) {
+inline LocalQueriesDev local_queries(uint8_t* u8, float* f, int* i, uint8_t* desc, int n_lq, int* n) {
     const size_t s = (size_t)n_lq;
     LocalQueriesDev lq{};
-    lq.cap = n_lq; lq.n = n; lq.in_view = t.lq_u8; lq.obs_pos = t.lq_u8 + s;
-    lq.proj_x = t.lq_f; lq.proj_y = t.lq_f + s; lq.proj_xr = t.lq_f + 2 * s; lq.depth = t.lq_f + 3 * s; lq.view_cos = t.lq_f + 4 * s; lq.xw = t.lq_f + 5 * s;
-    lq.level = t.lq_i; lq.src = t.lq_i + s; lq.desc = t.lq_desc;
+    lq.cap = n_lq; lq.n = n; lq.in_view = u8; lq.obs_pos = u8 + s;
+    lq.proj_x = f; lq.proj_y = f + s; lq.proj_xr = f + 2 * s; lq.depth = f + 3 * s; lq.view_cos = f + 4 * s; lq.xw = f + 5 * s;
+    lq.level = i; lq.src = i + s; lq.desc = desc;
     return lq;
 }
 

@@ -4,7 +4,9 @@
 
 #include <cuda_runtime.h>
 
+#include <cstring>
 #include <string>
+#include <type_traits>
 
 #include "rgbl_internal.h"
 
@@ -70,7 +72,8 @@ struct QtScratchDev { unsigned short *perm_a, *perm_b, *node_a, *node_b; unsigne
 int quadtree_smem_bytes();
 int launch_quadtree(cudaStream_t st, const uint32_t* dense, const int* level_cnt, const int* frame_total, const LevelGeom* d_levels,
                     int n_levels, const QtScratchDev& scr, uint32_t* sel_lvl, int* n_sel_lvl, const int* lvl_region, int cap_kp,
-                    int* status, SelKp* sel, int* n_sel, int n_frames, int max_nodes = 1024);      // max_nodes: largest max(quota + 3, 4 nIni) over the levels
+                    int* status, SelKp* sel, int* n_sel, int n_frames, int max_nodes = 1024,      // max_nodes: largest max(quota + 3, 4 nIni) over the levels
+                    int dense_cap = 0x7fffffff);      // entries of `dense`: the counts may run past it after a flagged candidate-buffer overflow
 int quadtree_block_host(const uint32_t* cand, int n, int width, int height, int N, uint32_t* out, int out_cap);
 
 // depth_kernels.cu
@@ -145,6 +148,67 @@ struct MatchScratch {                 // device scratch of the matchers (match_k
     int* minq; int* choice; uint8_t* resolved; int* overflow; int* rounds;
 };
 
+// Sequence lanes (rgbl_set_sequences): every launch of the resident chain serves S independent sequences, lane s = blockIdx.y (the pose
+// kernel: cluster s along y).  Each pointer-bearing argument of the chain's kernels is a Laned<T>: lane s's value is base + s * step, word
+// by word (64-bit, wrapping).  The lanes' buffers are equally spaced (rgbl_ctx.h: ChainLaneStrides), so a pointer's step is its lane
+// stride in bytes and every other field, the same in all lanes, has step zero.  A plain T converts to one lane (step zero).
+constexpr int kMaxLanes = 16;
+template <class T> struct Laned {
+    static_assert(sizeof(T) % 8 == 0 && alignof(T) >= 8, "Laned<T>: T is made of 64-bit words");
+    T base, step;
+    Laned() : base(), step() {}
+    Laned(const T& v) : base(v), step() {}
+    Laned(const T& b, const T& st) : base(b), step(st) {}
+};
+template <class T> __host__ __device__ __forceinline__ T lane_value(const Laned<T>& a, unsigned s) {
+    T r;
+#pragma unroll
+    for (size_t i = 0; i < sizeof(T) / 8; ++i) {
+        unsigned long long b, d;
+        memcpy(&b, reinterpret_cast<const char*>(&a.base) + 8 * i, 8);
+        memcpy(&d, reinterpret_cast<const char*>(&a.step) + 8 * i, 8);
+        b += (unsigned long long)s * d;
+        memcpy(reinterpret_cast<char*>(&r) + 8 * i, &b, 8);
+    }
+    return r;
+}
+// lane s's argument inside a kernel instantiated for kLanes; a one-lane launch (kLanes false) reads the argument itself, as a kernel
+// without lanes would
+template <bool kLanes, class T> __device__ __forceinline__ auto lane_arg(const Laned<T>& a, unsigned s) -> typename std::conditional<kLanes, T, const T&>::type {
+    if constexpr (kLanes) return lane_value(a, s); else return a.base;
+}
+// Set (never cleared here) when laned_of met lanes that are not base + s * step.  enqueue_chain fails the chain with it; a captured chain
+// (the default) is then never instantiated, so none of its launches runs.
+inline bool& lane_layout_broken() { static thread_local bool broken = false; return broken; }
+// host: the Laned<T> of the lanes make(s) builds (make(1) - make(0) word by word; make(0) alone when the launch has one lane).  Every lane
+// s >= 2 is checked against base + s * step in the low 32 bits of each word: all of a pointer's offset and every 4-byte field that starts a
+// word, while the high half of a word may be the padding after such a field, whose bytes are unspecified.
+template <class F> inline auto laned_of(int lanes, F make) -> Laned<decltype(make(0))> {
+    using T = decltype(make(0));
+    const T b = make(0);
+    if (lanes < 2) return Laned<T>(b);
+    const T o = make(1);
+    T d;
+    for (size_t i = 0; i < sizeof(T) / 8; ++i) {
+        unsigned long long x, y;
+        memcpy(&x, reinterpret_cast<const char*>(&o) + 8 * i, 8);
+        memcpy(&y, reinterpret_cast<const char*>(&b) + 8 * i, 8);
+        x -= y;
+        memcpy(reinterpret_cast<char*>(&d) + 8 * i, &x, 8);
+    }
+    const Laned<T> r(b, d);
+    for (int s = 2; s < lanes; ++s) {
+        const T want = make(s), got = lane_value(r, (unsigned)s);
+        for (size_t i = 0; i < sizeof(T) / 8; ++i) {
+            unsigned long long x, y;
+            memcpy(&x, reinterpret_cast<const char*>(&want) + 8 * i, 8);
+            memcpy(&y, reinterpret_cast<const char*>(&got) + 8 * i, 8);
+            if ((uint32_t)x != (uint32_t)y) lane_layout_broken() = true;
+        }
+    }
+    return r;
+}
+
 void prepare_match_kernels();
 // true while the resident chain enqueues its kernels: the chain launchers then add the programmatic-stream-serialization attribute (PDL, see
 // pdl_wait in rgbl_device.cuh).  Thread-local, set and cleared by chain_begin (api_track.cu).
@@ -165,13 +229,15 @@ void launch_grid_build(cudaStream_t st, const FrameDev& f, int* cell_start, int*
 void launch_grid_build_batch(cudaStream_t st, const FrameDev& f, int n_frames, int kp_stride, int* cell_start, int* csr_idx, int* kp_cell);
 // edges != nullptr: the resolution kernel also writes the matched features as PoseOptimization edges (resident tracking chain)
 struct ChainEdgesOut { float* exw; float* eobs; float* einfo; uint8_t* est; int* eidx; int* n_edges; };
-void launch_search_last(cudaStream_t st, const FrameDev& f, const int* cell_start, const int* csr_idx, const LastFrameDev& lf,
-                        const SearchLastParams& prm, MatchScratch s, uint8_t* state, int* match, int* n_matches,
-                        const ChainEdgesOut* edges = nullptr);
+// The chain's launchers take `lanes` sequence lanes (grid y); a plain argument is one lane.
+void launch_search_last(cudaStream_t st, const Laned<FrameDev>& f, const Laned<const int*>& cell_start, const Laned<const int*>& csr_idx,
+                        const Laned<LastFrameDev>& lf, const Laned<SearchLastParams>& prm, const Laned<MatchScratch>& s, const Laned<uint8_t*>& state,
+                        const Laned<int*>& match, const Laned<int*>& n_matches, const Laned<ChainEdgesOut>* edges = nullptr, int lanes = 1);
 struct LocalRingDev;
 struct ChainTlmTail;                 // below (chain_kernels.cu section): TrackLocalMap tail of the resolution kernel
-void launch_search_local(cudaStream_t st, const FrameDev& f, const int* cell_start, const int* csr_idx, const LocalPointsDev& lp,
-                         const SearchLocalParams& prm, MatchScratch s, uint8_t* state, int* match, int* n_matches, const ChainTlmTail* tail = nullptr);
+void launch_search_local(cudaStream_t st, const Laned<FrameDev>& f, const Laned<const int*>& cell_start, const Laned<const int*>& csr_idx,
+                         const Laned<LocalPointsDev>& lp, const SearchLocalParams& prm, const Laned<MatchScratch>& s, const Laned<uint8_t*>& state,
+                         const Laned<int*>& match, const Laned<int*>& n_matches, const Laned<ChainTlmTail>* tail = nullptr, int lanes = 1);
 void launch_search_bow(cudaStream_t st, const FrameDev& f, int n_q, const int* q_feat, const int* q_cbeg, const int* q_cend,
                        const uint8_t* kf_desc, const uint8_t* f_desc, const float* q_angle, const float* f_angle, const int* f_node_feat,
                        float nn_ratio, int keep_max, int check_orientation, const uint8_t* obs_pos, MatchScratch s, uint8_t* state, int* match,
@@ -183,7 +249,7 @@ void launch_fuse_search(cudaStream_t st, const FrameDev& f, const int* cell_star
                         const float* Ow /*3, device*/, float th, int* best_idx, int* best_dist);
 // ChainPrepDev (rgbl_device.cuh): unprojection of one frame's LiDAR-depth keypoints with its pose = the map points of the next search
 struct ChainPrepDev;
-void launch_chain_prep(cudaStream_t st, const ChainPrepDev& cp, const float* last_pose);
+void launch_chain_prep(cudaStream_t st, const Laned<ChainPrepDev>& cp, const Laned<const float*>& last_pose, int lanes = 1);
 void launch_frustum(cudaStream_t st, const FrameDev& f, const FrustumParams& prm, int n, const float* xw, const float* normal,
                     const float* mf_min, const float* mf_max, uint8_t* in_view, float* px, float* py, float* pxr, float* depth,
                     int* level, float* view_cos);
@@ -199,8 +265,10 @@ struct LocalQueriesDev {             // the in-frustum local map points, compact
     uint8_t* in_view; uint8_t* obs_pos; float *proj_x, *proj_y, *proj_xr, *depth; int* level; float* view_cos; uint8_t* desc; int* src;
     float* xw;                       // world coordinates of the compacted points (read by the edge-list tail instead of the ring)
 };
-void launch_tlm_prepare(cudaStream_t st, const FrameDev& f, const float* pose, const LocalRingDev& ring, float cos_limit, const int* n_edges,
-                        const int* e_idx, const uint8_t* e_outlier, uint8_t* state, int* match_last, const LocalQueriesDev& lq, int* lookback, int* fail);
+// lanes: one compaction per lane (grid y), lane s's look-back slots at lookback + s * tlm_lookback_ints()
+void launch_tlm_prepare(cudaStream_t st, const Laned<FrameDev>& f, const Laned<const float*>& pose, const Laned<LocalRingDev>& ring, float cos_limit,
+                        const Laned<const int*>& n_edges, const Laned<const int*>& e_idx, const Laned<const uint8_t*>& e_outlier, const Laned<uint8_t*>& state,
+                        const Laned<int*>& match_last, const Laned<LocalQueriesDev>& lq, int* lookback, const Laned<int*>& fail, int lanes = 1);
 // TrackLocalMap tail of the local search's resolution kernel (match_kernels.cu): the edge list of the second PoseOptimization from (inliers
 // of the first search) + (local matches), and the hand-over of the last frame's points into the ring.  *n_local_matches is written.
 struct ChainTlmTail {
@@ -257,8 +325,12 @@ struct PoseProblemDev {
 // callers check it before launch_pose_optimize
 const char* pose_cluster_unsupported(int device);
 // next != nullptr: after the pose is final the kernel also runs the chain preparation of the NEXT frame's search with it
-void launch_pose_optimize(cudaStream_t st, const PoseProblemDev& p, double* work /* n*4 doubles */, uint8_t* level, uint8_t* outlier,
-                          float* pose_out /*7*/, int* n_inliers, const ChainPrepDev* next = nullptr);
+// lanes: one cluster per lane (cluster s = CTAs [0, kPoseCtas) x {s})
+void launch_pose_optimize(cudaStream_t st, const Laned<PoseProblemDev>& p, const Laned<double*>& work /* n*4 doubles */, const Laned<uint8_t*>& level,
+                          const Laned<uint8_t*>& outlier, const Laned<float*>& pose_out /*7*/, const Laned<int*>& n_inliers,
+                          const Laned<ChainPrepDev>* next = nullptr, int lanes = 1);
+// clusters of pose_optimize_kernel the device holds at once (cudaOccupancyMaxActiveClusters; 0: the query failed)
+int pose_max_active_clusters(int device);
 
 // bow_kernels.cu ------------------------------------------------------------------------------------
 struct VocabDev {                    // DBoW2 vocabulary, flattened (node 0 = root)

@@ -84,6 +84,21 @@ class Context:
         to gray on the device.  camera_rgb = Camera.RGB (True: channel 0 is red).  channels 1: gray images (the default)."""
         check(lib().rgbl_set_input_channels(self.handle, int(channels), int(bool(camera_rgb))), self.handle)
 
+    def set_sequences(self, n: int = 1, pose0=None):
+        """Track n independent sequences in lockstep (rgbl_set_sequences): every batch holds n lanes of m = batch / n consecutive frames
+        (lane s = frames [s*m, (s+1)*m)), and the tracking chain and the sequence runners track each lane as its own sequence, one launch
+        serving all lanes.  pose0: None (every lane starts at the chain's pose0) or n x 7 start poses.  Outputs stay in batch order."""
+        p = None if pose0 is None else np.ascontiguousarray(pose0, np.float32).reshape(-1)
+        if p is not None and p.size != 7 * int(n):
+            raise ValueError(f"pose0 must hold {int(n)} x 7 floats")
+        check(lib().rgbl_set_sequences(self.handle, int(n), None if p is None else ptr(p)), self.handle)
+
+    def sequence_lanes_resident(self) -> int:
+        """Sequence lanes whose pose clusters the device runs at once (rgbl_sequence_lanes_resident); more lanes run in waves."""
+        n = C.c_int()
+        check(lib().rgbl_sequence_lanes_resident(self.handle, C.byref(n)), self.handle)
+        return n.value
+
     def set_host_quadtree(self, on: bool):
         check(lib().rgbl_set_host_quadtree(self.handle, int(on)), self.handle)
 
