@@ -18,6 +18,8 @@
 //     stop when (ini - cur) * 1e3 < ini three times in a row;
 //   * every round restarts from the frame's initial pose; inlier edges are classified with the error of
 //     the LAST evaluated trial (g2o does not recompute it), outlier edges are recomputed.
+// A round that would repeat the previous one bit for bit (no level changed, and the same robust flag or no Huber linear-region
+// evaluation) is not run: its estimate, errors and classification are already in place (end of the round loop).
 #include <atomic>
 #include <cfloat>
 #include <string>
@@ -216,8 +218,13 @@ __device__ __forceinline__ void huber(double e2, double delta, float dsqr, doubl
     rho1 = in ? 1.0 : delta * rs;
 }
 
-constexpr int kAcc = 28;      // 21 H + 6 b + 1 chi
-constexpr int kXchg = kAcc + 1;   // + the trial's chi2 in evaluation order, or the classification's outlier count
+// Huber's linear region (huber's `in` is false; a NaN e2 counts as linear): where a robust and a non-robust evaluation differ
+__device__ __forceinline__ bool huber_linear(double e2, float dsqr) { return !(e2 <= (double)dsqr); }
+
+constexpr int kAcc = 28;      // 21 H + 6 b + 1 chi; a build's and a trial's exchange add one value (the trial's chi2 in evaluation order)
+// the classification's exchange: + the outlier count, the number of edges whose level changed, and the threads that evaluated an
+// active edge in Huber's linear region during the round and during the next round's first build
+constexpr int kXchgClass = kAcc + 4;
 // Cluster shape, measured on an H100 SXM (700 W) through the whole resident chain (tools/pose_variants.sh, bench.py config B,
 // us per tracked frame incl. both searches): 4 x 256: 324   8 x 128: 257   8 x 256: 328   16 x 64: 239   16 x 128: 269.
 // The build / evaluation passes are bound by one SM's FP64 issue rate (~400 DFMA per edge), so more SMs with fewer threads each
@@ -308,28 +315,39 @@ __device__ __forceinline__ void butterfly_step(double* v, int lane) {
 // with a halving butterfly: at distance h every lane keeps one half of its slots and ships the other half to its partner, so
 // 16+8+4+2+1 = 31 exchanges replace 28 x 5 and lane L ends up with the warp total of slot L.  `last` is folded with shfl_down into
 // lane 0, the order the trial chi2 of the rho test is summed in (the build's chi2, slot 27, has its own order: both are kept, each
-// feeds its own LM decision).  The warp totals are added in warp order, the CTA totals go through ClusterXchg: out[0..kAcc].
-__device__ __forceinline__ void cluster_reduce(ClusterXchg& xc, double* v /* 32 slots, 28..31 zero */, double last, double* smem /* warps*kXchg */,
-                                               double* out /* kXchg, shared */) {
+// feeds its own LM decision).  The warp totals are added in warp order, the CTA totals go through ClusterXchg: out[0..kAcc + NL).
+// The classification folds NL = 4 such values (counts, exact in any order) into its exchange.
+template <int NL>
+__device__ __forceinline__ void cluster_reduce(ClusterXchg& xc, double* v /* 32 slots, 28..31 zero */, double (&last)[NL],
+                                               double* smem /* warps*32 */, double* out /* kAcc + NL, shared */) {
+    static_assert(kAcc + NL <= 32, "ClusterXchg slots");
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     butterfly_step<16>(v, lane); butterfly_step<8>(v, lane); butterfly_step<4>(v, lane); butterfly_step<2>(v, lane); butterfly_step<1>(v, lane);
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) last += __shfl_down_sync(0xffffffffu, last, o);
-    if (lane < kAcc) smem[warp * kXchg + lane] = v[0];
-    if (lane == 0) smem[warp * kXchg + kAcc] = last;
+    for (int j = 0; j < NL; ++j)
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) last[j] += __shfl_down_sync(0xffffffffu, last[j], o);
+    if (lane < kAcc) smem[warp * 32 + lane] = v[0];
+    if (lane == 0)
+#pragma unroll
+        for (int j = 0; j < NL; ++j) smem[warp * 32 + kAcc + j] = last[j];
     __syncthreads();
     double s = 0;
-    if (threadIdx.x < kXchg) {
+    if (threadIdx.x < kAcc + NL) {
         double t[kPoseWarps];
 #pragma unroll
-        for (int w = 0; w < kPoseWarps; ++w) t[w] = smem[w * kXchg + threadIdx.x];
+        for (int w = 0; w < kPoseWarps; ++w) t[w] = smem[w * 32 + threadIdx.x];
 #pragma unroll
         for (int st = 1; st < kPoseWarps; st <<= 1)
 #pragma unroll
             for (int w = 0; w + st < kPoseWarps; w += 2 * st) t[w] += t[w + st];
         s = t[0];
     }
-    xc.sum(s, kXchg, out);
+    xc.sum(s, kAcc + NL, out);
+}
+__device__ __forceinline__ void cluster_reduce(ClusterXchg& xc, double* v, double last, double* smem, double* out) {
+    double l[1] = {last};
+    cluster_reduce<1>(xc, v, l, smem, out);
 }
 
 // structural zeros shared by the mono and the stereo Jacobian (d(u)/d(ty) = d(v)/d(tx) = d(ur)/d(ty) = 0)
@@ -340,8 +358,8 @@ __device__ constexpr bool kJnz[3][6] = {{true, true, true, true, false, true}, {
 __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads) pose_optimize_kernel(Laned<PoseProblemDev> p_l, Laned<double*> work_l, Laned<uint8_t*> level_l,
                                                             Laned<uint8_t*> outlier_l, Laned<float*> pose_out_l,
                                                             Laned<int*> n_inliers_l, Laned<ChainPrepDev> next_l) {
-    __shared__ double red[kPoseWarps * kXchg];
-    __shared__ double acc[kXchg];         // the cluster totals of the last exchange: the system the next solves start from + one value
+    __shared__ double red[kPoseWarps * 32];
+    __shared__ double acc[kXchgClass];    // the cluster totals of the last exchange: the system the next solves start from + 1 or 4 values
     __shared__ __align__(16) double xchg_buf[2][kPoseCtas][32];      // partial sums of the CTAs (written remotely by st.async)
     __shared__ __align__(8) unsigned long long xchg_mbar[2];
     __shared__ float s_posef[7];
@@ -367,7 +385,7 @@ __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads
     const int tid = threadIdx.x, n = p.n_dev ? *p.n_dev : p.n;
     const int gtid = (int)rank * kPoseThreads + tid;
 #ifdef POSE_TIMING
-    long long tm[6] = {0, 0, 0, 0, 0, 0}; int tc[3] = {0, 0, 0}; long long t0_ = clock64(), tA_;
+    long long tm[6] = {0, 0, 0, 0, 0, 0}; int tc[4] = {0, 0, 0, 0}; long long t0_ = clock64(), tA_;
 #define TM_START() tA_ = clock64()
 #define TM_ADD(i) do { long long tB_ = clock64(); tm[i] += tB_ - tA_; tA_ = tB_; } while (0)
 #else
@@ -409,6 +427,7 @@ __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads
     for (int k = gtid; k < n; k += kPoseStride) { level[k] = 0; outlier[k] = 0; }       // every edge belongs to one thread of the cluster for the whole kernel
     __syncthreads();
     bool robust = true;
+    bool lin = false;                     // this thread evaluated an active edge of the round in Huber's linear region (robust rounds)
     int n_bad = 0;
 
     // One edge at pose T: camera-frame point, 1/z and the reprojection error, one code path for both edge types (no warp
@@ -433,8 +452,9 @@ __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads
     };
 
     // computeActiveErrors + activeRobustChi2 + buildSystem for one active edge at the pose its camera-frame point and errors E were
-    // computed at: adds its robust chi2 to v[27], rho' J^T Omega J to v[0..20] (upper triangle) and -rho' J^T Omega e to v[21..26]
-    auto accumulate = [&](const Edge& E, bool rob, double (&v)[32]) {
+    // computed at: adds its robust chi2 to v[27], rho' J^T Omega J to v[0..20] (upper triangle) and -rho' J^T Omega e to v[21..26];
+    // sets lin when a robust evaluation falls in Huber's linear region
+    auto accumulate = [&](const Edge& E, bool rob, double (&v)[32], bool& lin) {
         const bool st = E.st;
         const double info = E.info, x = E.pc[0], y = E.pc[1], invz = E.invz, invz_2 = invz * invz;
         const double e[3] = {E.e[0], E.e[1], E.e[2]};
@@ -453,7 +473,7 @@ __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads
 #pragma unroll
         for (int r = 0; r < 3; ++r) chi += e[r] * (info * e[r]);
         double w = 1.0, r0 = chi;
-        if (rob) huber(chi, st ? ds : dm, st ? dsqr_s : dsqr_m, r0, w);
+        if (rob) { lin |= huber_linear(chi, st ? dsqr_s : dsqr_m); huber(chi, st ? ds : dm, st ? dsqr_s : dsqr_m, r0, w); }
         v[27] += r0;
         const double wi = w * info;
         double WJ[3][6], we[3];
@@ -479,10 +499,11 @@ __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads
         }
     };
 
-    for (int it = 0; it < 4; ++it) {
+    bool first_build = true;              // the round's iteration-0 system needs a build pass of its own
+    for (int it = 0; it < 4;) {
         // round 0 starts with a build pass at the initial pose; every later round's iteration-0 system was built by the previous
-        // round's classification pass
-        if (tid == 0) { s_est = s_init; s_ok = 1; s_build = it == 0; }
+        // executed round's classification pass, unless that was built with the other robust flag (see the end of the round)
+        if (tid == 0) { s_est = s_init; s_ok = 1; s_build = first_build; }
         __syncthreads();
         for (int iter = 0; iter < 10; ++iter) {
             if (!s_ok) break;
@@ -497,7 +518,7 @@ __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads
                 for (int k = gtid; k < n; k += kPoseStride) {
                     Edge E;
                     load_edge(T, k, E);
-                    if (E.active) accumulate(E, robust, v);
+                    if (E.active) accumulate(E, robust, v, lin);
                 }
                 TM_ADD(0);
                 cluster_reduce(xc, v, 0.0, red, acc);
@@ -567,9 +588,13 @@ __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads
                         if (!E.active) continue;
                         work[3 * (size_t)k] = E.e[0]; work[3 * (size_t)k + 1] = E.e[1]; work[3 * (size_t)k + 2] = E.e[2];
                         double chi = E.e[0] * (E.info * E.e[0]) + E.e[1] * (E.info * E.e[1]) + E.e[2] * (E.info * E.e[2]);
-                        if (robust) { double r0, r1; huber(chi, E.st ? ds : dm, E.st ? dsqr_s : dsqr_m, r0, r1); chi = r0; }
+                        if (robust) {
+                            double r0, r1;
+                            lin |= huber_linear(chi, E.st ? dsqr_s : dsqr_m);
+                            huber(chi, E.st ? ds : dm, E.st ? dsqr_s : dsqr_m, r0, r1); chi = r0;
+                        }
                         part += chi;
-                        accumulate(E, robust, v);
+                        accumulate(E, robust, v, lin);
                     }
                 }
                 TM_ADD(3);
@@ -611,20 +636,25 @@ __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads
                 if (!s_continue) break;
             }
         }
-        // ---- classification (src/Optimizer.cc:1014-1100).  Its pass also builds the next round's iteration-0 system at the initial
-        // pose, with the levels just decided and that round's robust flag, and its exchange carries the outlier count ----
+        // ---- classification (src/Optimizer.cc:1014-1100).  Its pass also builds round it + 1's iteration-0 system at the initial
+        // pose, with the levels just decided and that round's robust flag; its exchange carries the outlier count, the number of level
+        // changes and the linear-region flags of this round and of that build ----
+        bool changed = false, lin_round = false, lin_first = false;
+        const bool robust_next = it < 2;
+        bool lin_next = false;            // this thread's part of lin_first
         {
             const Se3d T = s_est;
-            const bool build_next = it < 3 && n >= 10, robust_next = it < 2;
+            const bool build_next = it < 3 && n >= 10;
             double v[32];
 #pragma unroll
             for (int k = 0; k < 32; ++k) v[k] = 0;
-            int bad = 0;
+            int bad = 0, moved = 0;
             for (int k = gtid; k < n; k += kPoseStride) {
                 const bool st = p.stereo[k] != 0;
                 const double info = (double)p.inv_sigma2[k];
                 double e0, e1, e2 = 0;
-                if (outlier[k]) {
+                const bool was_out = outlier[k] != 0;         // = level[k] != 0
+                if (was_out) {
                     Edge E;
                     load_edge(T, k, E);
                     e0 = E.e[0]; e1 = E.e[1]; e2 = E.e[2];
@@ -635,21 +665,43 @@ __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads
                 double chi = e0 * (info * e0) + e1 * (info * e1);
                 if (st) chi += e2 * (info * e2);
                 const float chi2 = (float)chi;
-                if (chi2 > (st ? 7.815f : 5.991f)) { outlier[k] = 1; level[k] = 1; ++bad; }
+                if (chi2 > (st ? 7.815f : 5.991f)) { outlier[k] = 1; level[k] = 1; ++bad; moved += !was_out; }
                 else {
-                    outlier[k] = 0; level[k] = 0;
+                    outlier[k] = 0; level[k] = 0; moved += was_out;
                     if (build_next) {
                         Edge E;
                         load_edge(s_init, k, E);
-                        accumulate(E, robust_next, v);
+                        accumulate(E, robust_next, v, lin_next);
                     }
                 }
             }
-            cluster_reduce(xc, v, (double)bad, red, acc);
+            double last[4] = {(double)bad, (double)moved, lin ? 1.0 : 0.0, lin_next ? 1.0 : 0.0};
+            cluster_reduce<4>(xc, v, last, red, acc);
             n_bad = (int)acc[kAcc];
+            changed = acc[kAcc + 1] != 0; lin_round = acc[kAcc + 2] != 0; lin_first = acc[kAcc + 3] != 0;
         }
-        if (it == 2) robust = false;
         if (n < 10) break;
+        // ---- rounds that repeat this one.  A round's result is a function of the initial pose, the levels and its robust flag only:
+        // the kernel is deterministic (fixed summation orders, no atomics).  So with no level changed, round it + 1 repeats round it
+        // bit for bit when its robust flag is the same, and also when it is not but no active edge of round it (its iteration-0
+        // system, build passes, every evaluated trial) fell in Huber's linear region: huber() then returns rho = e2 and weight 1.0,
+        // the non-robust values.  The repeat would classify every edge as before, so the next round repeats it too: skip them all.
+        int next = it + 1;
+#ifndef POSE_RUN_ALL_ROUNDS               // test builds only (tests/test_cuda_emu_pose_replica.py): the same kernel running every round
+        while (next < 4 && !changed && ((next < 3) == (it < 3) || !lin_round)) {
+            ++next;
+#ifdef POSE_TIMING
+            tc[3]++;
+#endif
+        }
+#endif
+        // the classification built the first system with round it + 1's robust flag; the next round to run needs the other one only
+        // after a skip from round 0 or 1 to round 3.  That system is the non-robust one too when no edge of its build fell in the
+        // linear region, otherwise the round starts with a build pass of its own.
+        robust = next < 3;
+        first_build = robust != robust_next && lin_first;
+        lin = first_build ? false : lin_next;
+        it = next;
     }
     if (tid == 0) {
         const Se3d T = s_est;
@@ -660,7 +712,7 @@ __global__ void __cluster_dims__(kPoseCtas, 1, 1) __launch_bounds__(kPoseThreads
         s_posef[4] = (float)T.tx; s_posef[5] = (float)T.ty; s_posef[6] = (float)T.tz;
         if (rank == 0) *n_inliers = n - n_bad;
 #ifdef POSE_TIMING
-        if (rank == 0) printf("pose n=%d total=%lld build=%lld(%d) breduce=%lld solve=%lld eval=%lld(%d, %d accepted) evalred=%lld solve6=%lld\n", n, clock64() - t0_, tm[0], tc[0], tm[1], tm[2], tm[3], tc[1], tc[2], tm[4], tm[5]);
+        if (rank == 0) printf("pose n=%d total=%lld build=%lld(%d) breduce=%lld solve=%lld eval=%lld(%d, %d accepted) evalred=%lld solve6=%lld skipped=%d\n", n, clock64() - t0_, tm[0], tc[0], tm[1], tm[2], tm[3], tc[1], tc[2], tm[4], tm[5], tc[3]);
 #endif
     }
     prepare_next();

@@ -1,6 +1,6 @@
 #!/bin/bash
-# Development aid (needs a GPU): rebuild pose_kernels.o with -DPOSE_TIMING (clock64 per phase, printed by rank 0 of the cluster),
-# run a short chain, restore the normal object.
+# Development aid (needs a GPU): rebuild pose_kernels.o with -DPOSE_TIMING (clock64 per phase, printed by rank 0 of the cluster, with the
+# number of build passes, evaluated / accepted trials and skipped repeat rounds of each call), run a short chain, restore the normal object.
 set -e
 cd orb_slam3_rgbl_b200/csrc
 F="-gencode arch=compute_90a,code=sm_90a --extended-lambda -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall,-ffp-contract=off -fmad=true"
