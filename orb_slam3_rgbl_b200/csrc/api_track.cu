@@ -436,6 +436,10 @@ int rgbl_search_by_projection_reloc(rgbl_ctx* ctx, const rgbl_frame_view* cur, c
     return finish_search(c, cur->n, match, n_matches);
 }
 
+#ifdef RGBL_TESTING_EXPORTS        // test hook (csrc/rgbl_testing.h): not in librgbl_b200.so
+int rgbl_last_match_rounds(const rgbl_ctx* ctx) { return reinterpret_cast<const Ctx*>(ctx)->last_match_rounds; }
+#endif
+
 }  // extern "C" (re-opened below)
 
 /* Resident tracking chain over the frames of the last rgbl_resident_process / rgbl_frame_rgbl_batch call, entirely on the

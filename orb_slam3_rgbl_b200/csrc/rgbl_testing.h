@@ -37,6 +37,10 @@ int rgbl_fast_strips_emulation(const rgbl_orb_params* orb, int width, int height
 int rgbl_describe_staged_emulation(const rgbl_orb_params* orb, const uint8_t* level_img, const uint8_t* blurred_img, int w, int h,
                                    int stride, int n, const int32_t* xy, float* angle_out, uint8_t* desc_out);
 
+/* Test hook: the resolution rounds of the last successful matcher call on this context (resolve_kernel's round counter, read back
+ * together with the match count).  Exported by the emulated library (tests/cuda_emu), which compiles api_track.cu with this flag.    */
+int rgbl_last_match_rounds(const rgbl_ctx* ctx);
+
 #ifdef __cplusplus
 }
 #endif
