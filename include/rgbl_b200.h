@@ -275,6 +275,38 @@ int rgbl_search_for_triangulation(rgbl_ctx* ctx, int n1, const uint8_t* desc1, c
                                   const float F12[9], const float ep[2], int n_levels, const float* scale_factors2, const float* level_sigma2_2,
                                   int only_stereo, int coarse, int check_orientation, int32_t* match12, int* n_matches);
 
+/* What LocalMapping::CreateNewMapPoints reads of a key frame.  Feature vector as CSR (ascending node ids, node_start[n_nodes + 1]
+ * with node_start[0] == 0, features in vector order); Tcw = GetPose() as qx qy qz qw tx ty tz.                            */
+typedef struct {
+    int32_t n;
+    const uint8_t* desc;                 /* mDescriptors, n x 32 */
+    const rgbl_keypoint* keys;           /* mvKeys (KeyFrame::UnprojectStereo reads the distorted keypoint) */
+    const rgbl_keypoint* keys_un;        /* mvKeysUn */
+    const float* uright; const float* depth;   /* mvuRight, mvDepth */
+    const uint8_t* has_mp;               /* GetMapPoint(i) != NULL */
+    int32_t n_nodes; const uint32_t* node_ids; const int32_t* node_start; const int32_t* node_feat;   /* mFeatVec as CSR */
+    float Tcw[7];
+} rgbl_keyframe_view;
+
+/* LocalMapping::CreateNewMapPoints (src/LocalMapping.cc; Nleft == -1, no IMU): for each neighbour j in order, SearchForTriangulation
+ * (kf1, kf2[j], only_stereo false, coarse) against the key-frame-1 features without a map point, then per match the parallax choice
+ * between GeometricTools::Triangulate and KeyFrame::UnprojectStereo, the depth, reprojection and scale-consistency checks.  A feature
+ * of key frame 1 given a point by neighbour j is not searched by later neighbours (the reference's `if (pMP1) continue;`).
+ * kf2 = GetBestCovisibilityKeyFrames(nn) that pass the baseline test; F12[9 j..] / ep[2 j..] = the pair constants as for
+ * rgbl_search_for_triangulation.  One camera: mb = bf / fx, ratioFactor = 1.5f * scale_factors[1] (so n_levels >= 2);
+ * th_far = mThFarPoints (0: mbFarPoints off).  Points of neighbour j: [created_start[j], created_start[j+1]) of idx1 / idx2 /
+ * x3d (world, 3 floats each), ascending idx1 = the order the reference creates them; n_matches[j] = SearchForTriangulation's
+ * return value for that pair.  Each key-frame-1 feature is created at most once, so cap >= kf1->n is always enough; more points
+ * than cap: RGBL_E_CAPACITY and no output written.  RGBL_E_INVALID (nothing written): missing arrays, a feature or octave index
+ * out of range, n_levels outside 2..RGBL_MAX_LEVELS, a non-finite pose or intrinsic.  Calling once per neighbour with has_mp
+ * of key frame 1 set for the points just created gives the same results as one call.  Billed to the `match` profiling stage. */
+int rgbl_create_new_map_points(rgbl_ctx* ctx, const rgbl_keyframe_view* kf1, int n_neighbours, const rgbl_keyframe_view* kf2,
+                               const float* F12 /* n_neighbours x 9 */, const float* ep /* n_neighbours x 2 */,
+                               float fx, float fy, float cx, float cy, float bf, int n_levels, const float* scale_factors,
+                               const float* level_sigma2, float th_far, int check_orientation, int coarse,
+                               int32_t* created_start /* n_neighbours + 1 */, int32_t* idx1, int32_t* idx2, float* x3d /* cap x 3 */,
+                               int cap, int32_t* n_matches /* nullable, [n_neighbours] */);
+
 /* ORBmatcher::Fuse(KeyFrame* pKF, const vector<MapPoint*>& vpMapPoints, float th, bool bRight = false) (src/ORBmatcher.cc:1148-1330),
  * the search part (:1176-1303).  kf = the key frame's members (a KeyFrame has the same grid / keypoint members as a Frame);
  * Tcw = pKF->GetPose(), Ow = pKF->GetCameraCenter(); valid[i] = pMP && !isBad() && !IsInKeyFrame(pKF); mf_min / mf_max =

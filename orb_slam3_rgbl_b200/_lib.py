@@ -41,6 +41,12 @@ class FrameViewC(C.Structure):
                 ("log_scale_factor", C.c_float)]
 
 
+class KeyFrameViewC(C.Structure):
+    _fields_ = [("n", C.c_int32), ("desc", C.c_void_p), ("keys", C.c_void_p), ("keys_un", C.c_void_p), ("uright", C.c_void_p),
+                ("depth", C.c_void_p), ("has_mp", C.c_void_p), ("n_nodes", C.c_int32), ("node_ids", C.c_void_p),
+                ("node_start", C.c_void_p), ("node_feat", C.c_void_p), ("Tcw", C.c_float * 7)]
+
+
 class Config(C.Structure):
     _fields_ = [("device", C.c_int32), ("width", C.c_int32), ("height", C.c_int32), ("max_batch", C.c_int32),
                 ("max_points", C.c_int32), ("max_candidates", C.c_int32), ("orb", OrbParams)]
@@ -94,6 +100,8 @@ SYMBOLS = {
     "rgbl_distinctive_descriptors": (_i, [_vp, _i, _vp, _vp, _vp]),
     "rgbl_search_for_triangulation": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp,
                                            _i, _i, _i, _vp, _ip]),
+    "rgbl_create_new_map_points": (_i, [_vp, C.POINTER(KeyFrameViewC), _i, C.POINTER(KeyFrameViewC), _vp, _vp, _f, _f, _f, _f, _f, _i, _vp, _vp, _f,
+                                        _i, _i, _vp, _vp, _vp, _vp, _i, _vp]),
     "rgbl_local_bundle_adjustment": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _f, _f, _f, _f, _f, _i, _vp, _vp, _vp, _ip]),
     "rgbl_vocabulary_create": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, C.POINTER(C.c_void_p)]),
     "rgbl_vocabulary_destroy": (None, [_vp]),

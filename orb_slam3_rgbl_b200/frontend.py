@@ -300,6 +300,42 @@ def search_for_triangulation(ctx: Context, kf1: dict, kf2: dict, F12, ep, scale_
     return nm.value, match[:len(d1)]
 
 
+class KeyFrameView:
+    """rgbl_keyframe_view over one key-frame dict: desc, keys (mvKeys), keys_un (mvKeysUn), uright, depth, has_mp,
+    fv=(node_ids, node_start, node_feat) and Tcw (qx qy qz qw tx ty tz).  Keeps the arrays alive with the struct."""
+
+    def __init__(self, kf: dict):
+        self.desc = np.ascontiguousarray(kf["desc"], np.uint8).reshape(-1, 32)
+        self.keys = np.ascontiguousarray(kf["keys"], L.KP_DTYPE); self.keys_un = np.ascontiguousarray(kf["keys_un"], L.KP_DTYPE)
+        self.uright = np.ascontiguousarray(kf["uright"], np.float32); self.depth = np.ascontiguousarray(kf["depth"], np.float32)
+        self.has_mp = np.ascontiguousarray(kf["has_mp"], np.uint8)
+        self.fv = (np.ascontiguousarray(kf["fv"][0], np.uint32), np.ascontiguousarray(kf["fv"][1], np.int32), np.ascontiguousarray(kf["fv"][2], np.int32))
+        nz = lambda a: ptr(a) if a.size else None
+        self.c = L.KeyFrameViewC(len(self.desc), nz(self.desc), nz(self.keys), nz(self.keys_un), nz(self.uright), nz(self.depth), nz(self.has_mp),
+                                 len(self.fv[0]), nz(self.fv[0]), nz(self.fv[1]), nz(self.fv[2]),
+                                 (C.c_float * 7)(*np.asarray(kf["Tcw"], np.float32).tolist()))
+
+
+def create_new_map_points(ctx: Context, kf1: dict, neighbours, F12, ep, cam, n_levels=None, scale_factors=None, level_sigma2=None, th_far=0.0,
+                          check_orientation=False, coarse=False, cap=None):
+    """LocalMapping::CreateNewMapPoints over key frame kf1 and its neighbours (dicts as KeyFrameView takes), in order.
+    cam = (fx, fy, cx, cy, bf); F12[n, 9] / ep[n, 2] = the pair constants.  -> dict(created_start[n + 1], idx1, idx2, x3d[m, 3], n_matches[n])"""
+    v1 = KeyFrameView(kf1); v2 = [KeyFrameView(k) for k in neighbours]
+    arr = (L.KeyFrameViewC * max(len(v2), 1))(*[v.c for v in v2])
+    n = len(v2)
+    F12 = np.ascontiguousarray(F12, np.float32).reshape(n * 9); ep = np.ascontiguousarray(ep, np.float32).reshape(n * 2)
+    sf = np.ascontiguousarray(scale_factors, np.float32); sg = np.ascontiguousarray(level_sigma2, np.float32)
+    cap = len(v1.desc) if cap is None else cap
+    start = np.zeros(n + 1, np.int32); nm = np.zeros(max(n, 1), np.int32)
+    i1 = np.empty(max(cap, 1), np.int32); i2 = np.empty(max(cap, 1), np.int32); x = np.empty((max(cap, 1), 3), np.float32)
+    fx, fy, cx, cy, bf = cam
+    check(lib().rgbl_create_new_map_points(ctx.handle, C.byref(v1.c), n, arr, ptr(F12) if n else None, ptr(ep) if n else None, fx, fy, cx, cy, bf,
+                                           len(sf) if n_levels is None else n_levels, ptr(sf), ptr(sg), th_far, int(check_orientation), int(coarse),
+                                           ptr(start), ptr(i1), ptr(i2), ptr(x), cap, ptr(nm)), ctx.handle)
+    m = int(start[n])
+    return dict(created_start=start, idx1=i1[:m].copy(), idx2=i2[:m].copy(), x3d=x[:m].copy(), n_matches=nm[:n].copy())
+
+
 def local_bundle_adjustment(ctx: Context, poses, pose_fixed, points, e_point, e_pose, obs, stereo, inv_sigma2, fx, fy, cx, cy, bf, iterations=10):
     """Optimizer::LocalBundleAdjustment's numerical core on a flat graph (rgbl_local_bundle_adjustment)
     -> (poses[n,7], points[m,3], erase[n_edges], iterations_run)"""
