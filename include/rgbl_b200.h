@@ -256,6 +256,22 @@ int rgbl_local_bundle_adjustment(rgbl_ctx* ctx, int n_poses, const float* poses 
                                  float cy, float bf, int iterations, float* poses_out, float* points_out, uint8_t* edge_erase,
                                  int* iterations_run /* nullable */);
 
+/* ---- Optimizer::BundleAdjustment (src/Optimizer.cc:60), numerical core; GlobalBundleAdjustemnt (:52) calls it -----------
+ * The graph in the flat form of rgbl_local_bundle_adjustment: one pose per non-bad key frame (pose_fixed = 1 for the map's
+ * initial key frame), one point per non-bad map point, one edge per observation whose key frame is in the graph (stereo =
+ * mvuRight >= 0, inv_sigma2 = mvInvLevelSigma2[octave]).  Runs the same Levenberg-Marquardt for `iterations`, with Huber
+ * kernels (deltas sqrt(5.99) mono, sqrt(7.815) stereo) only when `robust`, and no outlier pass.  `stop` (nullable) is the
+ * bool behind pbStopFlag: it is read before every iteration and after every LM trial, and a raised flag ends the run as
+ * g2o's force-stop does.  Fixed poses and points without edges come back bit for bit.  More than RGBL_GBA_MAX_FREE_POSES
+ * free poses: RGBL_E_CAPACITY with nothing written (the dense reduced system is (6 n_free)^2 doubles).  The reduced system
+ * of more than 64 free poses is factored across the whole GPU.  Recovery (SetPose / mTcwGBA by nLoopKF) stays in the shim. */
+#define RGBL_GBA_MAX_FREE_POSES 4096
+int rgbl_global_bundle_adjustment(rgbl_ctx* ctx, int n_poses, const float* poses /* n_poses x 7 */, const uint8_t* pose_fixed, int n_points,
+                                  const float* points /* n_points x 3 */, int n_edges, const int32_t* e_point, const int32_t* e_pose,
+                                  const float* obs /* n_edges x 3 */, const uint8_t* stereo, const float* inv_sigma2, float fx, float fy, float cx,
+                                  float cy, float bf, int iterations, int robust, const volatile uint8_t* stop /* nullable */,
+                                  float* poses_out, float* points_out, int* iterations_run /* nullable */);
+
 /* ---- LocalMapping-thread kernels (SURVEY 8(f) row 3) -----------------------------------------------------------------
  * MapPoint::ComputeDistinctiveDescriptors (src/MapPoint.cc:329-403) for a batch of map points: the descriptors observed for
  * point p are desc[obs_start[p] .. obs_start[p+1]) (vDescriptors in the reference's order); best[p] = index within that list of

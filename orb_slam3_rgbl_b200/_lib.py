@@ -103,6 +103,7 @@ SYMBOLS = {
     "rgbl_create_new_map_points": (_i, [_vp, C.POINTER(KeyFrameViewC), _i, C.POINTER(KeyFrameViewC), _vp, _vp, _f, _f, _f, _f, _f, _i, _vp, _vp, _f,
                                         _i, _i, _vp, _vp, _vp, _vp, _i, _vp]),
     "rgbl_local_bundle_adjustment": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _f, _f, _f, _f, _f, _i, _vp, _vp, _vp, _ip]),
+    "rgbl_global_bundle_adjustment": (_i, [_vp, _i, _vp, _vp, _i, _vp, _i, _vp, _vp, _vp, _vp, _vp, _f, _f, _f, _f, _f, _i, _i, _vp, _vp, _vp, _ip]),
     "rgbl_vocabulary_create": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, C.POINTER(C.c_void_p)]),
     "rgbl_vocabulary_destroy": (None, [_vp]),
     "rgbl_compute_bow": (_i, [_vp, _vp, _i, _vp, _i, _vp, _vp, _ip, _vp, _vp, _vp, _ip]),
@@ -154,6 +155,7 @@ TESTING_SYMBOLS = {
     "rgbl_std_sort_block_emulation": (_i, [_vp, _i, _i, _vp]),
     "rgbl_describe_staged_emulation": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "rgbl_fast_strips_emulation": (_i, [_vp, _i, _i, _i, _vp, _i, _i, _i, _vp, _i]),
+    "rgbl_testing_reduced_solve": (_i, [_i, _vp, _vp, _i, _vp, _vp]),
     "rgbl_orb_tables": None,          # plus the product's host-only table helper (same source file), bound like the product's
 }
 TESTING_LIB_PATH = LIB_PATH.with_name("librgbl_b200_testing.so")

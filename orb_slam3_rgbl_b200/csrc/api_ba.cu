@@ -1,4 +1,5 @@
-// Optimizer::LocalBundleAdjustment's numerical core (src/Optimizer.cc:1116-1499) on the device: g2o's Levenberg-Marquardt
+// Optimizer::LocalBundleAdjustment's (src/Optimizer.cc:1116-1499) and Optimizer::BundleAdjustment's (:60, global BA) numerical core on the
+// device, one LM driver (ba_run) for both entry points: g2o's Levenberg-Marquardt
 // (Thirdparty/g2o/g2o/core/optimization_algorithm_levenberg.cpp:61-201) over key-frame poses (SE3, 6 dof) and map points
 // (marginalised, 3 dof) with the Schur-complement block solver (core/block_solver.hpp:354-486), Huber kernels, the mono edge
 // of src/OptimizableTypes.cpp:139-160 and the stereo edge of types/types_six_dof_expmap.cpp:190-274.  FP64.
@@ -10,11 +11,14 @@
 // and per LM trial (lambda)
 //   ba_schur       thread per point: D^-1 = (H_ll + lambda I)^-1; S -= B_i D^-1 B_j^T for the pose pairs of the point (atomicAdd into
 //                                    the dense reduced system, 6 n_opt squared), coefficients += B_i D^-1 b_l
-//   ba_cholesky    one CTA         : dense Cholesky of S, solve for the pose increments
+//   ba_solve_reduced (ba_factor.cu) : dense Cholesky of S and the pose increments; one CTA up to 64 free poses, tiled across the GPU above
 //   ba_update      thread per point / pose: landmark increments by back substitution, trial estimates, gain denominator terms
 //   ba_errors      thread per edge : errors and robust chi2 at the trial estimates
 // The accept / reject decision needs three scalars per trial; they are read back (one small D2H + sync per trial): local BA runs
-// in the mapping thread, off the per-frame latency path.
+// in the mapping thread, global BA in the loop-closing thread, both off the per-frame latency path.  What the two entry points differ in
+// (BaOptions): the Huber kernel (always, deltas sqrt(5.991) / sqrt(7.815), for local BA; only when bRobust, sqrt(5.99) / sqrt(7.815), for
+// global BA), the stop flag (global BA's pbStopFlag, read before each iteration and after each trial), the erase test (local BA only) and
+// the free-pose capacity (global BA: RGBL_GBA_MAX_FREE_POSES).
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
@@ -89,6 +93,8 @@ struct BaDev {
     const int* pose_slot;                       // per pose: slot in the reduced system or -1 (fixed)
     const int* pt_start; const int* pt_edges;   // CSR: edges of a point
     const int* ps_start; const int* ps_edges;   // CSR: edges of a non-fixed pose (by slot)
+    int robust;                                 // Huber kernel on every edge; off: rho(e2) = e2, weight 1
+    double delta_mono, delta_stereo;            // Huber deltas (g2o's setDelta: float)
 };
 
 constexpr int kEdgeBlk = 54;                    // per-edge doubles: A(6) gl(3) B(21) gp(6) Hpl(18)
@@ -109,8 +115,9 @@ __device__ __forceinline__ void edge_error(const BaDev& g, int k, const Se3d* po
         e[2] = 0;
     }
 }
-__device__ __forceinline__ void huber(double e2, bool stereo, double& rho0, double& rho1) {
-    const double delta = stereo ? (double)(float)sqrt(7.815) : (double)(float)sqrt(5.991);
+__device__ __forceinline__ void huber(const BaDev& g, double e2, bool stereo, double& rho0, double& rho1) {
+    if (!g.robust) { rho0 = e2; rho1 = 1.0; return; }
+    const double delta = stereo ? g.delta_stereo : g.delta_mono;
     const float dsqr = (float)(delta * delta);
     if (e2 <= (double)dsqr) { rho0 = e2; rho1 = 1.0; }
     else { const double sq = sqrt(e2); rho0 = 2 * sq * delta - (double)dsqr; rho1 = delta / sq; }
@@ -142,7 +149,7 @@ __global__ void __launch_bounds__(128) ba_errors_kernel(BaDev g, const Se3d* __r
         err[3 * (size_t)k] = e[0]; err[3 * (size_t)k + 1] = e[1]; err[3 * (size_t)k + 2] = e[2];
         const double info = (double)g.info[k];
         double r1;
-        huber(info * (e[0] * e[0] + e[1] * e[1] + e[2] * e[2]), g.stereo[k] != 0, chi, r1);
+        huber(g, info * (e[0] * e[0] + e[1] * e[1] + e[2] * e[2]), g.stereo[k] != 0, chi, r1);
     }
     block_sum_to(chi, partial);
 }
@@ -158,7 +165,7 @@ __global__ void __launch_bounds__(128) ba_linearize_kernel(BaDev g, const Se3d* 
         const bool st = g.stereo[k] != 0;
         const double info = (double)g.info[k];
         double w;
-        huber(info * (e[0] * e[0] + e[1] * e[1] + e[2] * e[2]), st, chi, w);
+        huber(g, info * (e[0] * e[0] + e[1] * e[1] + e[2] * e[2]), st, chi, w);
         const Se3d T = poses[g.e_pose[k]];
         double R[3][3];
         {
@@ -327,55 +334,6 @@ __global__ void __launch_bounds__(128) ba_schur_kernel(BaDev g, const double* __
     }
 }
 
-// dense Cholesky S = L L^T on the lower triangle, then L L^T x = b_p - coef, by one CTA.  The matrix is staged in shared
-// memory when it fits (n <= 160: 6 n_opt squared doubles), else it is factored in place in global memory.  status[0] = 1 on a
-// non-positive pivot (g2o: the linear solver fails -> the LM trial is rejected).
-__global__ void __launch_bounds__(1024) ba_cholesky_kernel(int n, int use_smem, double* __restrict__ Sg, const double* __restrict__ bp, const double* __restrict__ coef,
-                                                           double* __restrict__ x, int* __restrict__ status) {
-    extern __shared__ double s_mat[];
-    const int tid = threadIdx.x, nt = blockDim.x;
-    double* S = use_smem ? s_mat : Sg;
-    double* y = use_smem ? s_mat + (size_t)n * n : x;
-    if (use_smem) for (int i = tid; i < n * n; i += nt) S[i] = Sg[i];
-    for (int i = tid; i < n; i += nt) y[i] = bp[i] - coef[i];
-    __syncthreads();
-    // two barriers per column: every thread reads the pivot itself (uniform failure test, no broadcast step)
-    bool fail = false;
-    for (int k = 0; k < n; ++k) {
-        const double d = S[(size_t)k * n + k];
-        if (!(d > 0) || !(d <= DBL_MAX)) { fail = true; break; }
-        const double sd = sqrt(d), inv = 1.0 / sd;
-        __syncthreads();                                          // everyone has read the pivot before it is overwritten
-        for (int i = k + tid; i < n; i += nt) S[(size_t)i * n + k] = (i == k) ? sd : S[(size_t)i * n + k] * inv;
-        __syncthreads();
-        // trailing update of the lower triangle (rows i > k, columns k < j <= i) on a 16-wide thread grid: no index divisions
-        const int tx = tid & 15, ty = tid >> 4, ny = nt >> 4;
-        for (int i = k + 1 + ty; i < n; i += ny) {
-            const double lik = S[(size_t)i * n + k];
-            for (int j = k + 1 + tx; j <= i; j += 16) S[(size_t)i * n + j] -= lik * S[(size_t)j * n + k];
-        }
-        __syncthreads();
-    }
-    if (fail) { if (tid == 0) status[0] = 1; for (int i = tid; i < n; i += nt) x[i] = 0; return; }
-    if (tid == 0) status[0] = 0;
-    // column-oriented substitutions, one barrier per column: every thread forms y[k] / L[k][k] itself
-    for (int k = 0; k < n; ++k) {
-        const double yk = y[k] / S[(size_t)k * n + k];
-        __syncthreads();
-        if (tid == 0) y[k] = yk;
-        for (int i = k + 1 + tid; i < n; i += nt) y[i] -= S[(size_t)i * n + k] * yk;
-        __syncthreads();
-    }
-    for (int k = n - 1; k >= 0; --k) {
-        const double yk = y[k] / S[(size_t)k * n + k];
-        __syncthreads();
-        if (tid == 0) y[k] = yk;
-        for (int i = tid; i < k; i += nt) y[i] -= S[(size_t)k * n + i] * yk;
-        __syncthreads();
-    }
-    if (use_smem) for (int i = tid; i < n; i += nt) x[i] = y[i];
-}
-
 // landmark increments, trial points, gain denominator terms of the landmarks.  After a failed factorisation (status[0] != 0) the whole
 // solution is zero: g2o's solve() (core/block_solver.hpp:354-486) returns when the reduced system cannot be solved, before the landmark
 // back substitution.  The trial points are then the current ones, so the errors the rejected trial leaves behind (the erase test reads
@@ -484,25 +442,35 @@ __global__ void ba_export_kernel(int n_poses, const Se3d* __restrict__ poses, co
     if (i < n3) pts_f[i] = (float)pts[i];
 }
 
-}  // namespace
-}  // namespace rgbl
+// What distinguishes the two entry points; the LM run itself is one (ba_run)
+struct BaOptions {
+    const char* what;                    // "local BA" / "global BA", for error messages
+    int max_opt;                         // free poses the call accepts (RGBL_E_CAPACITY above), < 0: no limit
+    bool robust;                         // Huber kernels, deltas sqrt(delta2_mono) / sqrt(delta2_stereo)
+    double delta2_mono, delta2_stereo;
+    const volatile uint8_t* stop;        // nullable: g2o's force-stop flag, read before each iteration and after each trial
+    bool want_erase;                     // the erase test per edge into edge_erase
+};
 
-using namespace rgbl;
-
-extern "C" int rgbl_local_bundle_adjustment(rgbl_ctx* ctx, int n_poses, const float* poses, const uint8_t* pose_fixed, int n_points, const float* points,
-                                            int n_edges, const int32_t* e_point, const int32_t* e_pose, const float* obs, const uint8_t* stereo,
-                                            const float* inv_sigma2, float fx, float fy, float cx, float cy, float bf, int iterations,
-                                            float* poses_out, float* points_out, uint8_t* edge_erase, int* iterations_run) {
-    Ctx* c = reinterpret_cast<Ctx*>(ctx);
+// g2o's Levenberg-Marquardt over the flat graph (optimize(iterations) of core/sparse_optimizer.cpp with
+// optimization_algorithm_levenberg.cpp's solve() per iteration)
+int ba_run(Ctx* c, const BaOptions& o, int n_poses, const float* poses, const uint8_t* pose_fixed, int n_points, const float* points, int n_edges,
+           const int32_t* e_point, const int32_t* e_pose, const float* obs, const uint8_t* stereo, const float* inv_sigma2, float fx, float fy, float cx,
+           float cy, float bf, int iterations, float* poses_out, float* points_out, uint8_t* edge_erase, int* iterations_run) {
     if (const int rc = require_idle(c)) return rc;
     if (n_poses < 0 || n_points < 0 || n_edges < 0 || iterations < 0 || (n_poses && (!poses || !pose_fixed || !poses_out)) || (n_points && (!points || !points_out)) ||
-        (n_edges && (!e_point || !e_pose || !obs || !stereo || !inv_sigma2 || !edge_erase))) { c->err = "bad local BA arguments"; return RGBL_E_INVALID; }
+        (n_edges && (!e_point || !e_pose || !obs || !stereo || !inv_sigma2 || (o.want_erase && !edge_erase)))) { c->err = std::string("bad ") + o.what + " arguments"; return RGBL_E_INVALID; }
     for (int k = 0; k < n_edges; ++k)
-        if (e_point[k] < 0 || e_point[k] >= n_points || e_pose[k] < 0 || e_pose[k] >= n_poses) { c->err = "local BA edge index out of range"; return RGBL_E_INVALID; }
+        if (e_point[k] < 0 || e_point[k] >= n_points || e_pose[k] < 0 || e_pose[k] >= n_poses) { c->err = std::string(o.what) + " edge index out of range"; return RGBL_E_INVALID; }
+    if (o.max_opt >= 0) {
+        int free_poses = 0;
+        for (int p = 0; p < n_poses; ++p) free_poses += pose_fixed[p] ? 0 : 1;
+        if (free_poses > o.max_opt) { c->err = std::string(o.what) + ": more free poses than the reduced system holds (" + std::to_string(o.max_opt) + ")"; return RGBL_E_CAPACITY; }
+    }
     if (iterations_run) *iterations_run = 0;
     if (n_poses) std::memcpy(poses_out, poses, (size_t)n_poses * 7 * sizeof(float));
     if (n_points) std::memcpy(points_out, points, (size_t)n_points * 3 * sizeof(float));
-    if (n_edges) std::memset(edge_erase, 0, n_edges);
+    if (n_edges && o.want_erase) std::memset(edge_erase, 0, n_edges);
     if (n_edges == 0 || n_points == 0) return RGBL_OK;
     CU(cudaSetDevice(c->cfg.device));
     cudaStream_t st = c->st;
@@ -525,8 +493,8 @@ extern "C" int rgbl_local_bundle_adjustment(rgbl_ctx* ctx, int n_poses, const fl
 
     // ---- device arena ----
     ArenaCarve a(c, (size_t)n_edges * (kEdgeBlk * 8 + 3 * 8 + 4 + 4 + 12 + 1 + 4 + 8) + (size_t)n_points * (4 + 9 * 8 * 2 + 6 * 8 + 12 + 12) + (size_t)n_poses * (2 * 56 + 8 + 2 * 28) +
-                    (size_t)n_opt * (27 * 8 + 8 + 6 * 8 * 3) + (size_t)n * n * 8 + (size_t)n_part * 8 * 3 + (1 << 16));
-    if (!a.base) { c->err = "device allocation failed (local BA)"; return RGBL_E_CUDA; }
+                    (size_t)n_opt * (27 * 8 + 8 + 6 * 8 * 4) + (size_t)n * n * 8 + (size_t)n_part * 8 * 3 + (1 << 16));
+    if (!a.base) { c->err = std::string("device allocation failed (") + o.what + ")"; return RGBL_E_CUDA; }
     int* d_epoint = a.take<int>(n_edges); int* d_epose = a.take<int>(n_edges); float* d_obs = a.take<float>((size_t)3 * n_edges);
     uint8_t* d_stereo = a.take<uint8_t>(n_edges); float* d_info = a.take<float>(n_edges); uint8_t* d_erase = a.take<uint8_t>(n_edges);
     int* d_slot = a.take<int>(n_poses); int* d_ptstart = a.take<int>(n_points + 1); int* d_ptedges = a.take<int>(n_edges);
@@ -539,8 +507,9 @@ extern "C" int rgbl_local_bundle_adjustment(rgbl_ctx* ctx, int n_poses, const fl
     double* d_Hll = a.take<double>((size_t)6 * n_points); double* d_bl = a.take<double>((size_t)3 * n_points);
     double* d_Hpp = a.take<double>((size_t)21 * std::max(n_opt, 1)); double* d_bp = a.take<double>((size_t)6 * std::max(n_opt, 1));
     double* d_S = a.take<double>((size_t)std::max(n, 1) * std::max(n, 1)); double* d_coef = a.take<double>(std::max(n, 1)); double* d_xp = a.take<double>(std::max(n, 1));
+    double* d_work = a.take<double>(std::max(n, 1));
     double* d_part = a.take<double>((size_t)3 * n_part); double* d_scal = a.take<double>(8); int* d_status = a.take<int>(4);
-    if (a.used > a.cap) { c->err = "local BA arena too small (internal)"; return RGBL_E_CUDA; }
+    if (a.used > a.cap) { c->err = std::string(o.what) + " arena too small (internal)"; return RGBL_E_CUDA; }
 
     auto up = [&](void* d, const void* h, size_t bytes) { return cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, st); };
     CU(up(d_epoint, e_point, (size_t)n_edges * 4)); CU(up(d_epose, e_pose, (size_t)n_edges * 4)); CU(up(d_obs, obs, (size_t)n_edges * 12));
@@ -550,26 +519,19 @@ extern "C" int rgbl_local_bundle_adjustment(rgbl_ctx* ctx, int n_poses, const fl
     CU(up(d_poses_f, poses, (size_t)n_poses * 28)); CU(up(d_pts_f, points, (size_t)n_points * 12));
     CU(cudaMemsetAsync(d_status, 0, 16, st));
     CU(cudaMemsetAsync(d_err, 0, (size_t)3 * n_edges * sizeof(double), st));      // iterations = 0: the erase test sees zero errors, only depth can flag
-    BaDev g{n_poses, n_opt, n_points, n_edges, fx, fy, cx, cy, bf, d_epoint, d_epose, d_obs, d_stereo, d_info, d_slot, d_ptstart, d_ptedges, d_psstart, d_psedges};
+    BaDev g{n_poses, n_opt, n_points, n_edges, fx, fy, cx, cy, bf, d_epoint, d_epose, d_obs, d_stereo, d_info, d_slot, d_ptstart, d_ptedges, d_psstart, d_psedges,
+            o.robust ? 1 : 0, (double)(float)std::sqrt(o.delta2_mono), (double)(float)std::sqrt(o.delta2_stereo)};
     const int init_n = std::max(n_poses, 3 * n_points);
     ba_init_state_kernel<<<(init_n + 255) / 256, 256, 0, st>>>(n_poses, d_poses_f, d_pose[0], 3 * n_points, d_pts_f, d_pts[0]);
 
-    const size_t chol_need = ((size_t)n * n + n) * sizeof(double);
-    const int chol_in_smem = chol_need <= 200 * 1024 ? 1 : 0;
-    const size_t chol_smem = chol_in_smem ? chol_need : 0;
-    const int chol_threads = n <= 192 ? 256 : 1024;          // small systems: cheaper barriers matter more than lanes
-    {
-        static bool done[64] = {};
-        const int dev = c->cfg.device;
-        if (dev >= 0 && dev < 64 && !done[dev]) { cudaFuncSetAttribute(ba_cholesky_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024); done[dev] = true; }
-    }
+    auto stopped = [&] { return o.stop && *o.stop != 0; };
     double* h = reinterpret_cast<double*>(c->h_scalars.get());      // 16 pinned ints = 8 doubles
     int cur = 0, it_run = 0;
     double lambda = 0, ni = 2;
     int n_bad = 0;
     long launches = 1;
     stage_begin(c, ST_POSE, st);
-    for (int it = 0; it < iterations; ++it) {
+    for (int it = 0; it < iterations && !stopped(); ++it) {
         // computeActiveErrors + activeRobustChi2 + buildSystem at the current estimates
         ba_linearize_kernel<<<eb, 128, 0, st>>>(g, d_pose[cur], d_pts[cur], d_err, d_blk, d_part);
         ba_final_sum_kernel<<<1, 256, 0, st>>>(d_part, eb, d_scal + 0);
@@ -588,8 +550,7 @@ extern "C" int rgbl_local_bundle_adjustment(rgbl_ctx* ctx, int n_poses, const fl
             if (n_opt) {
                 ba_schur_init_kernel<<<std::min((n * n + 255) / 256, 1024), 256, 0, st>>>(g, d_Hpp, lambda, d_S, d_coef);
                 ba_schur_kernel<<<(n_points + 3) / 4, 128, 0, st>>>(g, d_blk, d_Hll, d_bl, lambda, d_S, d_coef);
-                ba_cholesky_kernel<<<1, chol_threads, chol_smem, st>>>(n, chol_in_smem, d_S, d_bp, d_coef, d_xp, d_status);
-                launches += 3;
+                launches += 2 + ba_solve_reduced(st, n, d_S, d_bp, d_coef, d_xp, d_work, d_status);
             }
             ba_point_update_kernel<<<pb, 128, 0, st>>>(g, d_blk, d_Hll, d_bl, lambda, d_xp, d_status, d_pts[cur], d_pts[nxt], d_part);
             ba_final_sum_kernel<<<1, 256, 0, st>>>(d_part, pb, d_scal + 2);
@@ -615,22 +576,47 @@ extern "C" int rgbl_local_bundle_adjustment(rgbl_ctx* ctx, int n_poses, const fl
                 lambda *= ni; ni *= 2;
             }
             ++qmax;
-        } while (rho < 0 && qmax < 10);
+        } while (rho < 0 && qmax < 10 && !stopped());
         ++it_run;
         if (qmax == 10 || rho == 0) break;
         if ((ini - current) * 1e3 < ini) ++n_bad; else n_bad = 0;
         if (n_bad >= 3) break;
     }
-    ba_flags_kernel<<<eb, 128, 0, st>>>(g, d_pose[cur], d_pts[cur], d_err, d_erase);
+    if (o.want_erase) { ba_flags_kernel<<<eb, 128, 0, st>>>(g, d_pose[cur], d_pts[cur], d_err, d_erase); ++launches; }
     ba_export_kernel<<<(init_n + 255) / 256, 256, 0, st>>>(n_poses, d_pose[cur], d_slot, d_poses_f, d_poses_o, 3 * n_points, d_pts[cur], d_pts_o);
-    launches += 2;
+    ++launches;
     stage_end(c, ST_POSE, st, (int)launches);
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(poses_out, d_poses_o, (size_t)n_poses * 28, cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(points_out, d_pts_o, (size_t)n_points * 12, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(edge_erase, d_erase, n_edges, cudaMemcpyDeviceToHost, st));
+    if (o.want_erase) CU(cudaMemcpyAsync(edge_erase, d_erase, n_edges, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     prof_collect(c);
     if (iterations_run) *iterations_run = it_run;
     return RGBL_OK;
+}
+
+}  // namespace
+}  // namespace rgbl
+
+using namespace rgbl;
+
+extern "C" int rgbl_local_bundle_adjustment(rgbl_ctx* ctx, int n_poses, const float* poses, const uint8_t* pose_fixed, int n_points, const float* points,
+                                            int n_edges, const int32_t* e_point, const int32_t* e_pose, const float* obs, const uint8_t* stereo,
+                                            const float* inv_sigma2, float fx, float fy, float cx, float cy, float bf, int iterations,
+                                            float* poses_out, float* points_out, uint8_t* edge_erase, int* iterations_run) {
+    // Optimizer::LocalBundleAdjustment: Huber on every edge, deltas sqrt(5.991) / sqrt(7.815), no stop flag here, the erase test
+    const BaOptions o{"local BA", -1, true, 5.991, 7.815, nullptr, true};
+    return ba_run(reinterpret_cast<Ctx*>(ctx), o, n_poses, poses, pose_fixed, n_points, points, n_edges, e_point, e_pose, obs, stereo, inv_sigma2, fx, fy,
+                  cx, cy, bf, iterations, poses_out, points_out, edge_erase, iterations_run);
+}
+
+extern "C" int rgbl_global_bundle_adjustment(rgbl_ctx* ctx, int n_poses, const float* poses, const uint8_t* pose_fixed, int n_points, const float* points,
+                                             int n_edges, const int32_t* e_point, const int32_t* e_pose, const float* obs, const uint8_t* stereo,
+                                             const float* inv_sigma2, float fx, float fy, float cx, float cy, float bf, int iterations, int robust,
+                                             const volatile uint8_t* stop, float* poses_out, float* points_out, int* iterations_run) {
+    // Optimizer::BundleAdjustment: Huber only when bRobust, deltas sqrt(5.99) / sqrt(7.815), pbStopFlag, no outlier pass
+    const BaOptions o{"global BA", RGBL_GBA_MAX_FREE_POSES, robust != 0, 5.99, 7.815, stop, false};
+    return ba_run(reinterpret_cast<Ctx*>(ctx), o, n_poses, poses, pose_fixed, n_points, points, n_edges, e_point, e_pose, obs, stereo, inv_sigma2, fx, fy,
+                  cx, cy, bf, iterations, poses_out, points_out, nullptr, iterations_run);
 }

@@ -180,7 +180,7 @@ int structuring_element(const char* kind, int ku, int kv, uint8_t* mask) {
 
 extern "C" {
 
-int rgbl_abi_version(void) { return 4; }
+int rgbl_abi_version(void) { return 5; }
 
 int rgbl_orb_tables(const rgbl_orb_params* p, float* scale, float* inv_scale, float* sigma2, float* inv_sigma2,
                     int32_t* features_per_level, int32_t* umax16) {

@@ -346,5 +346,14 @@ void launch_bow_descend(cudaStream_t st, const VocabDev& voc, int n, const uint8
 int launch_bow_assemble(cudaStream_t st, int n, const int* f_word, const double* f_weight, const int* f_node, int* bow_word,
                         double* bow_value, int* fv_node, int* fv_start, int* fv_feature, int* counts /*3*/, int* scratch);
 
+// ba_factor.cu --------------------------------------------------------------------------------------
+// S x = bp - coef for the reduced camera system of bundle adjustment (S: n x n doubles, n = 6 n_opt, lower triangle, factored in place;
+// work: n doubles).  by_size: the one-CTA kernel up to kSingleCtaMaxOpt free poses, the tiled multi-CTA factorisation above.
+// status[0] = 1 and x = 0 on a non-positive or non-finite pivot, else 0.  Returns the number of launches.
+enum class BaSolvePath { by_size, single_cta, tiled };
+constexpr int kSingleCtaMaxOpt = 64;
+int ba_solve_reduced(cudaStream_t st, int n, double* S, const double* bp, const double* coef, double* x, double* work, int* status,
+                     BaSolvePath path = BaSolvePath::by_size);
+
 }  // namespace rgbl
 #endif

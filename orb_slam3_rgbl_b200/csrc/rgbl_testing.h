@@ -41,6 +41,12 @@ int rgbl_describe_staged_emulation(const rgbl_orb_params* orb, const uint8_t* le
  * together with the match count).  Exported by the emulated library (tests/cuda_emu), which compiles api_track.cu with this flag.    */
 int rgbl_last_match_rounds(const rgbl_ctx* ctx);
 
+/* Test hook: the reduced-system solve of bundle adjustment (ba_factor.cu) on a caller's matrix.  S: n x n doubles (any n >= 1), row-major,
+ * of which the lower triangle is read; b: n.  path 0: chosen by size as bundle adjustment chooses it (n <= 384: one CTA), 1: the one-CTA kernel, 2: the tiled
+ * multi-CTA factorisation.  x = S^-1 b, or 0 with *status = 1 when a pivot is non-positive or not finite (*status = 0 otherwise).
+ * Runs on the device (current device, default stream); RGBL_E_CUDA without one.                                                        */
+int rgbl_testing_reduced_solve(int n, const double* S, const double* b, int path, double* x, int* status);
+
 #ifdef __cplusplus
 }
 #endif

@@ -351,6 +351,26 @@ def local_bundle_adjustment(ctx: Context, poses, pose_fixed, points, e_point, e_
     return po, pt, er[:len(e_point)], it.value
 
 
+
+def global_bundle_adjustment(ctx: Context, poses, pose_fixed, points, e_point, e_pose, obs, stereo, inv_sigma2, fx, fy, cx, cy, bf, iterations=10,
+                             robust=False, stop=None):
+    """Optimizer::BundleAdjustment's numerical core on a flat graph (rgbl_global_bundle_adjustment).  stop: None or a one-element uint8
+    array, pbStopFlag; the call reads it before every iteration and after every LM trial, so another thread may raise it during the call.
+    -> (poses[n,7], points[m,3], iterations_run)"""
+    poses = np.ascontiguousarray(poses, np.float32).reshape(-1, 7); pose_fixed = np.ascontiguousarray(pose_fixed, np.uint8)
+    points = np.ascontiguousarray(points, np.float32).reshape(-1, 3)
+    e_point = np.ascontiguousarray(e_point, np.int32); e_pose = np.ascontiguousarray(e_pose, np.int32)
+    obs = np.ascontiguousarray(obs, np.float32).reshape(-1, 3); stereo = np.ascontiguousarray(stereo, np.uint8)
+    inv_sigma2 = np.ascontiguousarray(inv_sigma2, np.float32)
+    if stop is not None and not (isinstance(stop, np.ndarray) and stop.dtype == np.uint8 and stop.size == 1 and stop.flags.c_contiguous):
+        raise ValueError("stop must be a one-element contiguous uint8 array")
+    po = np.empty_like(poses); pt = np.empty_like(points); it = C.c_int(0)
+    nz = lambda a: ptr(a) if a.size else None
+    check(lib().rgbl_global_bundle_adjustment(ctx.handle, len(poses), nz(poses), nz(pose_fixed), len(points), nz(points), len(e_point), nz(e_point),
+                                              nz(e_pose), nz(obs), nz(stereo), nz(inv_sigma2), fx, fy, cx, cy, bf, iterations, int(robust),
+                                              None if stop is None else ptr(stop), nz(po), nz(pt), C.byref(it)), ctx.handle)
+    return po, pt, it.value
+
 class ORBVocabulary:
     """DBoW2 vocabulary (ORBVocabulary = TemplatedVocabulary<FORB::TDescriptor, FORB>, include/ORBVocabulary.h) uploaded once as a
     flat tree; `transform` = Frame::ComputeBoW's mpORBvocabulary->transform(vCurrentDesc, mBowVec, mFeatVec, 4)."""
